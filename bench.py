@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — node-expansions/sec of the B200 expansion engine (and of the reference CPU path).
+"""bench.py — node-expansions/sec of the H100 expansion engine (and of the reference CPU path).
 
 A "step" is one pass of the hot path (batched env_map::get_succ) over one batch of
 synthetic frontier nodes.  Default workload: the north_star target — 512^3 voxel map @0.1 m,
@@ -7,6 +7,7 @@ synthetic frontier nodes.  Default workload: the north_star target — 512^3 vox
 
   python bench.py --gpus 1 --steps K --warmup W [--workload 512c_acc27|cfg2|cfg3|cfg4]
   python bench.py --impl reference ...      # the reference's CPU path (oracle) on the host cores
+  python bench.py ... --dump-outputs DIR    # also write the last timed step's results as DIR/*.npy
 
 Prints ONE JSON line (rank 0).  See DESIGN.md §Measurement for the definition of every key.
 """
@@ -63,6 +64,8 @@ def parse():
     ap.add_argument("--mq-eps", type=float, default=2.0, help="cfg5: the planner's setEpsilon (weighted A*)")
     ap.add_argument("--kernel", type=int, default=0,
                     help="0 = auto, 1 = literal loop, 2 = register, 3 = flat, 4 = dealing, 5 = fixed-point")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (a fixed sample of its nodes) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -96,7 +99,7 @@ def make_env(sc, device):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md).
+    """SM clock and throttle reasons sampled DURING the timed region.
 
     Polls NVML from a background thread (a timed region of a few ms is far shorter than
     nvidia-smi's minimum loop period); falls back to `nvidia-smi -lms` when pynvml is missing."""
@@ -196,7 +199,7 @@ class CpuArm:
 
     def describe(self, threads):
         if self.kind == "reference":
-            return (f"unmodified reference env_map::get_succ (oracle/_ref: /root/reference/include + Eigen/Boost "
+            return (f"unmodified reference env_map::get_succ (oracle/_ref: the reference's include/ + Eigen/Boost "
                     f"stand-ins, g++ -O2), {threads} std::threads")
         return f"oracle restatement of env_map::get_succ (g++ -O2, no FMA), {threads} std::threads"
 
@@ -233,7 +236,7 @@ def config_dict(sc, n, world):
             "frontier": "reachable lattice states (random free cell centres + <=6 random valid controls), seed 7+rank",
             "parallelism": f"replicas x{world}, frontier sharded",
             "l2": f"per-step working set {(n * 112 + slots * 132 + int(np.prod(sc.dim_cells))) / 1e6:.0f} MB "
-                  f"(frontier + successor records + map) exceeds the 126 MB L2"}
+                  f"(frontier + successor records + map) exceeds the H100's 50 MB L2"}
 
 
 def run_reference(args, sc, rank, world):
@@ -427,8 +430,45 @@ def replay_sweep(env, sc, lib, stream, local, max_nodes=65536):
             "what": "A* pop order of one long query (MPL::MapPlanner::plan, GPU env) replayed through mplx_expand_device"}
 
 
-def kernel_name(which, sc, n_nodes):
-    """The kernel mplx_set_kernel(which) launches for this workload (auto rule: mplx_kernels.cu launch_expand)."""
+def dump_outputs(out_dir, n, nU, d_count, d_succ, d_cost, d_action, d_key, budget_bytes=48 << 20):
+    """What mplx_expand_device returned in the last timed step, for a fixed seeded sample of the frontier nodes
+    (all of them when they fit `budget_bytes`), as float64 .npy files: count [k], succ [k, nU, 14] (the
+    Waypoint's pos, vel, acc, jrk, yaw, t), cost [k, nU], blocked [k, nU], action [k, nU], key [k, nU, 2] (high
+    and low 32 bits).  A successor whose primitive collides has cost +inf in the API; here it has blocked = 1 and
+    cost 0, so that every value written is finite.  Slots past a node's count hold no successor and are 0."""
+    import torch
+
+    per_node = nU * (14 + 1 + 1 + 1 + 2) * 8 + 8
+    k = min(n, budget_bytes // per_node)
+    idx = np.sort(np.random.default_rng(0).choice(n, size=k, replace=False)) if k < n else np.arange(n)
+    it = torch.from_numpy(idx).to(d_count.device)
+    count = d_count[it].cpu().numpy()
+    valid = np.arange(nU)[None, :] < count[:, None]
+    key = d_key.view(n, nU)[it].cpu().numpy().view(np.uint64)
+    cost = d_cost.view(n, nU)[it].cpu().numpy()
+    blocked = np.isposinf(cost)
+    arrays = {
+        "sample_index": idx,
+        "count": count,
+        "succ": d_succ.view(n, nU, 112)[it].view(torch.float64).cpu().numpy(),
+        "cost": np.where(blocked, 0.0, cost),
+        "blocked": blocked,
+        "action": d_action.view(n, nU)[it].cpu().numpy(),
+        "key": np.stack([key >> np.uint64(32), key & np.uint64(0xFFFFFFFF)], axis=-1),
+    }
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.astype(np.float64)
+        if a.ndim >= 2:
+            a[~valid] = 0.0
+        if not np.isfinite(a).all():
+            raise RuntimeError(f"bench.py: non-finite values in the {name} output of the timed step")
+        np.save(out_dir / f"{name}.npy", a)
+
+
+def kernel_name(which, sc, n_nodes, sms):
+    """The kernel mplx_set_kernel(which) launches for this workload on a device with `sms` SMs (auto rule:
+    mplx_kernels.cu launch_expand)."""
     names = {1: "mplx::expand_seq_kernel", 2: "mplx::expand_reg_kernel", 3: "mplx::expand_flat_kernel", 4: "mplx::expand_deal_kernel"}
     if which in names:
         return names[which]
@@ -436,7 +476,7 @@ def kernel_name(which, sc, n_nodes):
         # occupancy planning: fixed-point sample loop; node-cooperative rows + flat items for large batches
         return "mplx::expand_fxn_kernel" if n_nodes * sc.nU >= 64 * 256 and sc.v_max > 0 else "mplx::expand_fx_kernel"
     heavy = (sc.control & 15) >= 7 or (sc.control & 16) != 0 or sc.potential_radius is not None
-    big = n_nodes * sc.nU >= 2 * 256 * 148 * 4 * 8
+    big = n_nodes * sc.nU >= 2 * 256 * sms * 4 * 8
     return "mplx::expand_deal_kernel" if heavy and big else "mplx::expand_reg_kernel"
 
 
@@ -530,6 +570,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     elapsed_ms = ev[0].elapsed_time(ev[-1])
     kernel_ms = [ev[k].elapsed_time(ev[k + 1]) for k in range(args.steps)]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), n, nU, d_count, d_succ, d_cost, d_action, d_key)
     gpu_launches = env.launch_count() - launches0  # kernels of this library launched inside the timed region
     t_el = torch.tensor([elapsed_ms], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -656,22 +698,15 @@ def main():
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         peaks = json.loads(pk.read_text())
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))  # fallback: H100 SXM data sheet
     k_ms = float(np.mean(kernel_ms))
     achieved = bytes_per_exp * n / (k_ms * 1e-3) / 1e9
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
                 "traffic": None, "peak_source": "measured" if pk.exists() else "fallback",
-                "kernel": kernel_name(args.kernel, sc, n), "kernel_ms": k_ms,
+                "kernel": kernel_name(args.kernel, sc, n, torch.cuda.get_device_properties(local).multi_processor_count),
+                "kernel_ms": k_ms,
                 "algorithmic_bytes_per_expansion": bytes_per_exp,
                 "mean_samples_per_expansion": mean_samples, "mean_successors_per_expansion": mean_succ}
-    prof = ROOT / "profiles" / "traffic.json"
-    if prof.exists():
-        try:
-            tr = json.loads(prof.read_text()).get(sc.name)
-            if tr:
-                roofline["traffic"] = tr["dram_bytes_per_launch"] * n / tr["nodes_per_launch"]
-        except Exception:
-            pass
 
     cpu_baseline = None
     if world == 1 and not args.no_cpu_baseline:

@@ -1,5 +1,5 @@
 /*
- * mplx.h — C ABI of libmplx.so, the B200 (sm_100a) node-expansion engine.
+ * mplx.h — C ABI of libmplx.so, the H100 (sm_90a) node-expansion engine.
  *
  * This is the drop-in boundary for ONE path of sikang/motion_primitive_library: the body of
  *   env_map<Dim>::get_succ               include/mpl_planner/env/env_map.h:147-172
@@ -233,7 +233,7 @@ void *mplx_stream(mplx_ctx *ctx);
  * internal pinned staging plus one host memcpy. */
 void *mplx_host_alloc(size_t bytes);
 void mplx_host_free(void *p);
-/* "sm_100a;<build flags>" */
+/* "libmplx sm_90a; <build flags>" */
 const char *mplx_build_info(void);
 
 #ifdef __cplusplus

@@ -94,7 +94,7 @@ class env_map_b200 : public env_map<Dim> {
 }  // namespace MPL
 
 namespace MPL {
-/// MapPlanner whose virtual setMapUtil (map_planner.h:29, map_planner.cpp:14-18) installs the B200 env:
+/// MapPlanner whose virtual setMapUtil (map_planner.h:29, map_planner.cpp:14-18) installs the GPU env:
 /// the drop-in that needs no edit of the reference's sources.
 template <int Dim>
 class MapPlannerB200 : public MapPlanner<Dim> {

@@ -104,7 +104,7 @@ def load() -> C.CDLL:
     path = Path(os.environ.get("MPLX_LIB", LIB_PATH))
     if not path.exists():
         raise ImportError(
-            f"{path} not found: the sm_100a CUDA engine is not built. Run "
+            f"{path} not found: the sm_90a CUDA engine is not built. Run "
             f"`python -c 'import __graft_entry__ as g; g.build()'` (or make -C "
             f"motion_primitive_library_b200/csrc). There is no CPU fallback for this path."
         )

@@ -65,7 +65,7 @@ extern "C" {
 const char *mplx_last_error(void) { return g_err; }
 
 const char *mplx_build_info(void) {
-  return "libmplx sm_100a; nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false; "
+  return "libmplx sm_90a; nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false; "
          "IEEE double, no CPU fallback";
 }
 

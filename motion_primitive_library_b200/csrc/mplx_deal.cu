@@ -196,14 +196,14 @@ static cudaError_t launch_deal_d(const EnvParams &P, const mplx_waypoint *d_node
 }
 
 // rounds: batches of 256 items per CTA.  More rounds = better lane use in phase C but fewer,
-// longer CTAs; keep at least ~8 CTAs per resident slot (148 SMs x 4 CTAs) so the grid tail stays small.
+// longer CTAs; keep at least ~8 CTAs per resident slot (SMs x 4 CTAs) so the grid tail stays small.
 cudaError_t launch_expand_deal(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &o,
                                cudaStream_t st, int rounds) {
   if (n_nodes <= 0) return cudaSuccess;
   const int npb = kThreads / P.nU;
   if (rounds <= 0) {
     const long ctas1 = ((long)n_nodes + npb - 1) / npb;  // CTAs at one round each
-    rounds = (int)(ctas1 / (148 * 4 * 8));
+    rounds = (int)(ctas1 / (sm_count() * 4 * 8));
     rounds = rounds < 1 ? 1 : (rounds > kDealMaxRounds ? kDealMaxRounds : rounds);
   }
   if (rounds > kDealMaxRounds) rounds = kDealMaxRounds;

@@ -1,4 +1,4 @@
-// mplx_device.cuh — device-side arithmetic of the node-expansion path (sm_100a).
+// mplx_device.cuh — device-side arithmetic of the node-expansion path (sm_90a).
 //
 // Everything here must reproduce the reference's IEEE-754 double results bit for bit where
 // they feed a lattice key, so this translation unit is compiled with -fmad=false (no FMA

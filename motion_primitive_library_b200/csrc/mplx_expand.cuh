@@ -190,33 +190,21 @@ __device__ __forceinline__ bool validate_yaw(const EnvParams &P, const PrimState
   return true;
 }
 
-// One successor Waypoint (112 bytes = 7 x 16) to global memory as seven 16-byte stores when the
-// destination allows it (cudaMalloc'ed arrays always do): half the store instructions and half the
-// partial-sector writes of fourteen 8-byte stores at a 112-byte stride between lanes.
+// One successor Waypoint (112 bytes = 7 x 16) to global memory as seven 16-byte stores, the widest
+// store sm_90 has, when the destination allows it (cudaMalloc'ed arrays always do): half the store
+// instructions and half the partial-sector writes of fourteen 8-byte stores at a 112-byte stride between lanes.
 // The stores are streaming (st.global.cs): the 132-byte records are written once and never read by the
 // kernel, and at ~0.9 GB per launch they would otherwise sweep the voxel bitmaps out of the L2.
-// A successor record is 112 bytes at a 112-byte stride: 16-byte aligned, every second one 32-byte aligned.
-// Three 256-bit stores and one 128-bit store (sm_100: st.global.v4.b64) instead of seven 128-bit ones: a warp's
-// store instruction touches ~28 different lines whatever its width, so fewer, wider stores cost the L1 fewer
-// tag look-ups.  .cs: the records are written once and never read by the device.
-__device__ __forceinline__ void st_cs_256(double *p, double a, double b, double c, double d) {
-  asm volatile("st.global.cs.v4.b64 [%0], {%1, %2, %3, %4};" ::"l"(p), "l"(__double_as_longlong(a)),
-               "l"(__double_as_longlong(b)), "l"(__double_as_longlong(c)), "l"(__double_as_longlong(d))
-               : "memory");
-}
 __device__ __forceinline__ void store_waypoint(mplx_waypoint *dst, const mplx_waypoint &w) {
-  const uintptr_t a = reinterpret_cast<uintptr_t>(dst);
-  double *d = reinterpret_cast<double *>(dst);
-  if ((a & 31u) == 0) {
-    st_cs_256(d + 0, w.pos[0], w.pos[1], w.pos[2], w.vel[0]);
-    st_cs_256(d + 4, w.vel[1], w.vel[2], w.acc[0], w.acc[1]);
-    st_cs_256(d + 8, w.acc[2], w.jrk[0], w.jrk[1], w.jrk[2]);
-    __stcs(reinterpret_cast<double2 *>(d + 12), make_double2(w.yaw, w.t));
-  } else if ((a & 15u) == 0) {
-    __stcs(reinterpret_cast<double2 *>(d + 0), make_double2(w.pos[0], w.pos[1]));
-    st_cs_256(d + 2, w.pos[2], w.vel[0], w.vel[1], w.vel[2]);
-    st_cs_256(d + 6, w.acc[0], w.acc[1], w.acc[2], w.jrk[0]);
-    st_cs_256(d + 10, w.jrk[1], w.jrk[2], w.yaw, w.t);
+  if ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) {
+    double2 *d = reinterpret_cast<double2 *>(dst);
+    __stcs(d + 0, make_double2(w.pos[0], w.pos[1]));
+    __stcs(d + 1, make_double2(w.pos[2], w.vel[0]));
+    __stcs(d + 2, make_double2(w.vel[1], w.vel[2]));
+    __stcs(d + 3, make_double2(w.acc[0], w.acc[1]));
+    __stcs(d + 4, make_double2(w.acc[2], w.jrk[0]));
+    __stcs(d + 5, make_double2(w.jrk[1], w.jrk[2]));
+    __stcs(d + 6, make_double2(w.yaw, w.t));
   } else {
     *dst = w;
   }

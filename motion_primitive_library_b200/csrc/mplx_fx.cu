@@ -375,7 +375,7 @@ __global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, 
 cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, uint2 *d_out, cudaStream_t st) {
   const size_t nwords = (nvox + 31) >> 5;
   int grid = (int)((nwords + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > sm_count() * 16) grid = sm_count() * 16;
   if (grid < 1) grid = 1;
   pack_occ2_kernel<<<grid, 256, 0, st>>>(d_occ, nvox, dim, nx, ny, d_out);
   return cudaGetLastError();

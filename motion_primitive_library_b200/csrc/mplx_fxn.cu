@@ -332,7 +332,7 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
         sp[5] = make_double2(tn.jrk[1], tn.jrk[2]);
         sp[6] = make_double2(tn.yaw, tn.t);
       } else {
-        // 256-bit stores (store_waypoint).  (Staging the CTA's records in shared memory for a coalesced copy-out
+        // 128-bit stores (store_waypoint).  (Staging the CTA's records in shared memory for a coalesced copy-out
         // by the threads themselves was measured: slower — the extra pass and barrier cost more than it saves.)
         store_waypoint(o.succ + (size_t)ni * nU + rank, tn);
       }
@@ -553,8 +553,8 @@ static cudaError_t launch_fxn_t(const EnvParams &P, const mplx_waypoint *d_nodes
   static const int sort_env = [] { const char *v = getenv("MPLX_FXN_SORT"); return v ? atoi(v) : -1; }();  // tuning
   const bool sort = sort_env >= 0 ? sort_env != 0 : ORD >= 3;
   // staging of the successor records for the bulk copies (expand_fxn_kernel): destination 16-byte aligned
-  // Measured: 0.518 -> 0.503-0.511 ms on the headline workload, 0.352 -> 0.330 ms on cfg2; with the CTA sort
-  // (JRK-125) 1.84 -> 1.94 ms, so the sorted path keeps the per-lane 256-bit stores.
+  // The sorted path (JRK-125 with the CTA sort) keeps the per-lane stores: on that workload the bulk copies
+  // were measured slower.
   static const int bulk_env = [] { const char *v = getenv("MPLX_FXN_BULK"); return v ? atoi(v) : -1; }();  // tuning / A-B
   const bool bulk = (bulk_env >= 0 ? bulk_env != 0 : !sort) && o.succ != nullptr &&
                     (reinterpret_cast<uintptr_t>(o.succ) & 15u) == 0;
@@ -576,7 +576,9 @@ static cudaError_t launch_fxn_t(const EnvParams &P, const mplx_waypoint *d_nodes
     if (cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &av) != cudaSuccess) cudaGetLastError();
   }
   static const int carve = [] { const char *v = getenv("MPLX_FXN_CARVE"); return v ? atoi(v) : -1; }();  // tuning: % of 228 KB
-  static const int pf_ahead = [] { const char *v = getenv("MPLX_FXN_PREFETCH"); return v ? atoi(v) : 1184; }();  // CTAs ahead (0 = off)
+  // CTAs ahead (0 = off); default: two waves of 4 CTAs per SM
+  static const int pf_env = [] { const char *v = getenv("MPLX_FXN_PREFETCH"); return v ? atoi(v) : -1; }();
+  const int pf_ahead = pf_env >= 0 ? pf_env : 2 * 4 * sm_count();
   static const int unr_env = [] { const char *v = getenv("MPLX_FXN_UNR"); return v ? atoi(v) : 0; }();    // tuning
   static const int minb_env = [] { const char *v = getenv("MPLX_FXN_MINB"); return v ? atoi(v) : 0; }();  // tuning
 #define MPLX_LAUNCH_FXN_S(UNR, MINB, LAT, REGION, SORT)                                                         \

@@ -1,5 +1,5 @@
 // mplx_kernels.cu — expand(frontier x U): the batched body of env_map<Dim>::get_succ
-// (include/mpl_planner/env/env_map.h:147-172) for sm_100a.
+// (include/mpl_planner/env/env_map.h:147-172) for sm_90a.
 //
 // Work decomposition.  A CTA of 256 threads covers NPB = 256/|U| whole frontier nodes, one
 // thread per (node, control) primitive:
@@ -18,7 +18,7 @@
 // The occupancy grid is read as 1 bit/voxel (16 MiB at 512^3: L2-resident); potential-field
 // planning reads the int8 grid.  No tensor cores: there is no dense contraction on this path.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false  (see mplx_device.cuh).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false  (see mplx_device.cuh).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -360,7 +360,7 @@ cudaError_t launch_expand(const EnvParams &P, const mplx_waypoint *d_nodes, int 
   const bool heavy = (P.control & 15) >= MPLX_JRK || (P.control & 16) != 0 || P.pot != nullptr;
   // (at one round per CTA the dealing kernel only adds overhead: 4096-node JRK launches of the lock-step
   // multi-query driver run 0.37 ms faster on the register kernel, so auto needs >= 2 rounds' worth of CTAs)
-  const bool deal = force_seq == 4 || (force_seq == 0 && heavy && (long)n_nodes * P.nU >= 2L * 256 * 148 * 4 * 8);
+  const bool deal = force_seq == 4 || (force_seq == 0 && heavy && (long)n_nodes * P.nU >= 2L * 256 * sm_count() * 4 * 8);
   if (deal && P.nU <= kThreads) {
     static const int rounds_env = [] {
       const char *e = getenv("MPLX_DEAL_ROUNDS");  // tuning override
@@ -370,6 +370,15 @@ cudaError_t launch_expand(const EnvParams &P, const mplx_waypoint *d_nodes, int 
   }
   return P.dim == 2 ? launch_d<2>(P, d_nodes, n_nodes, o, st, force_seq)
                     : launch_d<3>(P, d_nodes, n_nodes, o, st, force_seq);
+}
+
+int sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+    cudaGetLastError();  // the launch that follows reports the device error
+    return 1;
+  }
+  return n;
 }
 
 // ---- set-up kernels -------------------------------------------------------------------------
@@ -396,7 +405,7 @@ __global__ void pack_bits_kernel(const int8_t *__restrict__ bytes, size_t nvox, 
 cudaError_t launch_pack_bits(const int8_t *d_bytes, size_t nvox, uint32_t *d_bits, bool occ, cudaStream_t st) {
   const size_t nwords = (nvox + 31) >> 5;
   int grid = (int)((nwords + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > sm_count() * 16) grid = sm_count() * 16;
   if (grid < 1) grid = 1;
   if (occ)
     pack_bits_kernel<true><<<grid, 256, 0, st>>>(d_bytes, nvox, d_bits);

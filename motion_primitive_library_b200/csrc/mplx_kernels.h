@@ -1,4 +1,4 @@
-// mplx_kernels.h — host-callable launchers of the sm_100a kernels (internal).
+// mplx_kernels.h — host-callable launchers of the sm_90a kernels (internal).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -36,6 +36,8 @@ bool fxn_supported(const EnvParams &P, int n_nodes);
 cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &o,
                               cudaStream_t st, void *amb_q, unsigned *amb_n, unsigned amb_cap);
 size_t fx_amb_record_bytes();
+// SMs of the current device: the grid-size rules of the launchers scale with it
+int sm_count();
 // occupancy bits -> {occupancy word, candidate-summary word} per 32 voxels (mplx_fx.cu)
 cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, uint2 *d_out, cudaStream_t st);
 // bytes -> 1 bit/voxel: occ ? (byte == 100) : (byte != 0)

@@ -116,7 +116,8 @@ __global__ void region_stamp_kernel(const int *__restrict__ cells, int n_cells, 
 
 static int grid_for(size_t n) {
   size_t g = (n + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  const size_t cap = (size_t)sm_count() * 32;
+  if (g > cap) g = cap;
   return g < 1 ? 1 : (int)g;
 }
 

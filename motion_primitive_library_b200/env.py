@@ -4,7 +4,7 @@
 MPL::env_map<Dim> / env_base<Dim> (reference include/mpl_planner/env/env_map.h,
 include/mpl_planner/common/env_base.h:234-303) for the setters that feed get_succ, and
 `get_succ` itself (env_map.h:147-172) plus the batched `expand` the B200 engine adds.
-All computation happens in libmplx.so (CUDA, sm_100a); this file only marshals arguments.
+All computation happens in libmplx.so (CUDA, sm_90a); this file only marshals arguments.
 """
 from __future__ import annotations
 

@@ -7,6 +7,8 @@ from pathlib import Path
 
 import numpy as np
 
+from reference_record import reference
+
 ROOT = Path(__file__).resolve().parent.parent
 ORACLE_DIR = ROOT / "oracle"
 LIB = ORACLE_DIR / "liboracle.so"
@@ -168,8 +170,12 @@ def ref_available() -> bool:
     return REF_LIB.exists()
 
 
+def ref_info() -> str:
+    return reference(REF_LIB, lambda: ref_lib().ref_info().decode())
+
+
 def ref_lib():
-    """oracle/_ref/libmplref.so (built by `make -C oracle ref` where /root/reference exists)."""
+    """oracle/_ref/libmplref.so (built by `make -C oracle ref` where the reference sources are present)."""
     global _ref
     if _ref is None:
         L = C.CDLL(str(REF_LIB))
@@ -188,7 +194,28 @@ def ref_lib():
 
 
 def ref_expand(env: "OracleEnv", nodes, nthreads=1):
-    """Run the REFERENCE's env_map<Dim>::get_succ on `nodes` with the parameters held by `env`."""
+    """Run the REFERENCE's env_map<Dim>::get_succ on `nodes` with the parameters held by `env`.  Inside a test
+    without oracle/_ref: its recorded result, with only the emitted slots of each field (valid_only)."""
+    full = {}
+
+    def live():
+        full.update(_ref_expand(env, nodes, nthreads))
+        return emitted(full)
+
+    recorded = reference(REF_LIB, live)
+    return full or recorded
+
+
+def emitted(r):
+    """The fields a comparison reads: count, and action/succ/cost/key of the emitted slots only."""
+    if r.get("valid_only"):
+        return r
+    valid = (np.arange(r["nU"])[None, :] < r["count"][:, None]).reshape(-1)
+    return dict(valid_only=True, nU=r["nU"], count=r["count"], action=r["action"][valid], succ=r["succ"][valid],
+                cost=r["cost"][valid], key=r["key"][valid])
+
+
+def _ref_expand(env: "OracleEnv", nodes, nthreads=1):
     nodes = np.ascontiguousarray(nodes, dtype=WAYPOINT_DTYPE).reshape(-1)
     n, nU = nodes.size, env.nU
     succ = np.zeros(n * nU, dtype=WAYPOINT_DTYPE)
@@ -203,6 +230,10 @@ def ref_expand(env: "OracleEnv", nodes, nthreads=1):
 
 def ref_edges_is_free(env: "OracleEnv", parents, actions):
     """The REFERENCE's env_map::is_free(pr) / calculate_intrinsic_cost(pr) for stored edges."""
+    return reference(REF_LIB, lambda: _ref_edges_is_free(env, parents, actions))
+
+
+def _ref_edges_is_free(env, parents, actions):
     parents = np.ascontiguousarray(parents, dtype=WAYPOINT_DTYPE).reshape(-1)
     actions = np.ascontiguousarray(actions, dtype=np.int32).reshape(-1)
     free = np.zeros(parents.size, dtype=np.uint8)

@@ -7,6 +7,7 @@ from motion_primitive_library_b200.planner import (PlanArgs, PlanResult, QueryRe
                                                    iterative_plan, load_iter_fn, load_lpa_fn, load_traj_fn, lpa_session,
                                                    make_args, plan, plan_batch, plan_trajectory, run_iterative, run_lpa,
                                                    run_plan, run_trajectory)
+from reference_record import reference
 
 ROOT = Path(__file__).resolve().parent.parent
 
@@ -36,8 +37,11 @@ def lpa_oracle(args, script):
 def lpa_reference(args, script):
     """The REFERENCE's LPA* (setLPAstar / plan / getLinkedNodes / updateBlockedNodes / updateClearedNodes /
     getSubStateSpace, unmodified sources + Eigen/Boost stand-ins) on the same script."""
-    lib, fn = load_lpa_fn(REF_PLANNER, "refp_lpa_run")
-    return run_lpa(fn, lib, args, script)
+    def live():
+        lib, fn = load_lpa_fn(REF_PLANNER, "refp_lpa_run")
+        return run_lpa(fn, lib, args, script)
+
+    return reference(REF_PLANNER, live)
 
 
 def iterative_oracle(args, search_radius, max_iter=3):
@@ -48,8 +52,11 @@ def iterative_oracle(args, search_radius, max_iter=3):
 
 def iterative_reference(args, search_radius, max_iter=3):
     """The REFERENCE's plan() + MapPlanner::iterativePlan(start, goal, getTraj(), max_iter)."""
-    lib, fn = load_iter_fn(REF_PLANNER, "refp_iterative_plan")
-    return run_iterative(fn, lib, args, search_radius, max_iter)
+    def live():
+        lib, fn = load_iter_fn(REF_PLANNER, "refp_iterative_plan")
+        return run_iterative(fn, lib, args, search_radius, max_iter)
+
+    return reference(REF_PLANNER, live)
 
 
 def trajectory_oracle(args, n_samples=50):
@@ -59,8 +66,11 @@ def trajectory_oracle(args, n_samples=50):
 
 def trajectory_reference(args, n_samples=50):
     """The REFERENCE's plan() + its own Trajectory::sample / getWaypoints / evaluate / J."""
-    lib, fn = load_traj_fn(REF_PLANNER, "refp_plan_trajectory")
-    return run_trajectory(fn, lib, args, n_samples)
+    def live():
+        lib, fn = load_traj_fn(REF_PLANNER, "refp_plan_trajectory")
+        return run_trajectory(fn, lib, args, n_samples)
+
+    return reference(REF_PLANNER, live)
 
 
 def ref_planner_available():
@@ -69,25 +79,32 @@ def ref_planner_available():
 
 def plan_reference(args):
     """The REFERENCE's MapPlanner<Dim>::plan() (unmodified sources + Eigen/Boost stand-ins)."""
-    lib, fn = load_fn(REF_PLANNER, "refp_plan")
-    return run_plan(fn, lib, args)
+    def live():
+        lib, fn = load_fn(REF_PLANNER, "refp_plan")
+        return run_plan(fn, lib, args)
+
+    return reference(REF_PLANNER, live)
 
 
-def reference_potential_map(args, radius, n_cells, range_=None, pos=None):
-    """MapPlanner::updatePotentialMap (src/mpl_planner/map_planner.cpp:323-391) on args' map."""
+def reference_potential_map(args, radius, n_cells, range_=None, pos=None, record_all=False):
+    """MapPlanner::updatePotentialMap (src/mpl_planner/map_planner.cpp:323-391) on args' map.  record_all: the
+    recording keeps the whole map (a test that uses it as input data), not only its digest."""
     import ctypes as C
 
     import numpy as np
 
-    lib = C.CDLL(str(REF_PLANNER))
-    out = np.zeros(n_cells, dtype=np.int8)
-    rad = np.asarray(radius, dtype=np.float64)
-    rng = None if range_ is None else np.asarray(range_, dtype=np.float64)
-    p = None if pos is None else np.asarray(pos, dtype=np.float64)
-    lib.refp_update_potential_map.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.refp_update_potential_map(C.byref(args), rad.ctypes.data, None if rng is None else rng.ctypes.data,
-                                  None if p is None else p.ctypes.data, out.ctypes.data)
-    return out
+    def live():
+        lib = C.CDLL(str(REF_PLANNER))
+        out = np.zeros(n_cells, dtype=np.int8)
+        rad = np.asarray(radius, dtype=np.float64)
+        rng = None if range_ is None else np.asarray(range_, dtype=np.float64)
+        p = None if pos is None else np.asarray(pos, dtype=np.float64)
+        lib.refp_update_potential_map.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.refp_update_potential_map(C.byref(args), rad.ctypes.data, None if rng is None else rng.ctypes.data,
+                                      None if p is None else p.ctypes.data, out.ctypes.data)
+        return out
+
+    return reference(REF_PLANNER, live, max_bytes=None) if record_all else reference(REF_PLANNER, live)
 
 
 def reference_search_region(args, path, radius, n_cells, dense=False):
@@ -96,14 +113,17 @@ def reference_search_region(args, path, radius, n_cells, dense=False):
 
     import numpy as np
 
-    lib = C.CDLL(str(REF_PLANNER))
-    out = np.zeros(n_cells, dtype=np.uint8)
-    path = np.ascontiguousarray(path, dtype=np.float64)
-    rad = np.asarray(radius, dtype=np.float64)
-    lib.refp_set_search_region.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
-    lib.refp_set_search_region(C.byref(args), path.ctypes.data, len(path), rad.ctypes.data, 1 if dense else 0,
-                               out.ctypes.data)
-    return out
+    def live():
+        lib = C.CDLL(str(REF_PLANNER))
+        out = np.zeros(n_cells, dtype=np.uint8)
+        p = np.ascontiguousarray(path, dtype=np.float64)
+        rad = np.asarray(radius, dtype=np.float64)
+        lib.refp_set_search_region.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+        lib.refp_set_search_region(C.byref(args), p.ctypes.data, len(p), rad.ctypes.data, 1 if dense else 0,
+                                   out.ctypes.data)
+        return out
+
+    return reference(REF_PLANNER, live)
 
 
 REF_B200 = ROOT / "oracle" / "_ref" / "libmplref_b200.so"

@@ -22,7 +22,7 @@ def same(a, b):
 
 
 needs_libs = pytest.mark.skipif(not (pb.ref_b200_available() and pb.ref_planner_available()),
-                                reason="oracle/_ref not built (needs /root/reference at build time)")
+                                reason="oracle/_ref not built (needs the reference sources at build time)")
 
 
 @pytest.mark.gpu

@@ -8,8 +8,7 @@ import pytest
 
 import fixtures
 import planner_bindings as pb
-
-pytestmark = pytest.mark.skipif(not pb.ref_planner_available(), reason="oracle/_ref planner not built (needs /root/reference)")
+from reference_record import same_array
 ACC, JRK = 0x03, 0x07
 
 
@@ -20,8 +19,8 @@ def same(a, b):
         assert fa[k] == fb[k], ("first", k, fa[k], fb[k])
     assert la["ok"] == lb["ok"] and la["valid"] == lb["valid"]
     assert la["n_closed"] == lb["n_closed"] and la["n_open"] == lb["n_open"]
-    np.testing.assert_array_equal(la["closed"], lb["closed"])
-    np.testing.assert_array_equal(la["actions"], lb["actions"])
+    same_array(la["closed"], lb["closed"], "closed")
+    same_array(la["actions"], lb["actions"], "actions")
     if lb["valid"]:
         assert la["cost"] == lb["cost"]
 
@@ -46,7 +45,7 @@ def test_corridor_with_potential_field():
     a0 = pb.make_args(2, ACC, c["grid"], c["dim"], c["origin"], c["res"], fixtures.U_2d(), start=dict(pos=c["start"]),
                       goal=dict(pos=c["goal"]))
     # the field of the reference's own MapPlanner::updatePotentialMap (radius 0.5 m), used as plain input data
-    pot = pb.reference_potential_map(a0, (0.5, 0.5), int(np.prod(c["dim"])))
+    pot = pb.reference_potential_map(a0, (0.5, 0.5), int(np.prod(c["dim"])), record_all=True)
     assert 0 < (pot > 0).sum() and pot.max() == 100
     a = pb.make_args(2, ACC, c["grid"], c["dim"], c["origin"], c["res"], fixtures.U_2d(), start=dict(pos=c["start"]),
                      goal=dict(pos=c["goal"]), v_max=1.0, a_max=1.0, potential=pot, potential_weight=0.5)

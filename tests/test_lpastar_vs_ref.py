@@ -10,8 +10,7 @@ import pytest
 
 import fixtures
 import planner_bindings as pb
-
-pytestmark = pytest.mark.skipif(not pb.ref_planner_available(), reason="oracle/_ref planner not built (needs /root/reference)")
+from reference_record import same_array
 ACC, JRK, VEL = 0x03, 0x07, 0x01
 FIELDS = ("valid", "n_states", "n_closed", "n_open", "state_hash", "n_linked", "linked_hash", "n_actions")
 
@@ -22,7 +21,7 @@ def same_session(a, b):
         for f in FIELDS:
             assert x[f] == y[f], (x["op"], f, x[f], y[f])
         if x["op"] == "plan":
-            np.testing.assert_array_equal(x["actions"], y["actions"])
+            same_array(x["actions"], y["actions"], "actions")
             if y["valid"]:
                 assert x["cost"] == y["cost"] and x["expanded"] == y["expanded"]
 

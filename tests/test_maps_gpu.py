@@ -1,12 +1,13 @@
 """SURVEY.md §8f row 2 on the device: mplx_update_potential_map = MapPlanner::updatePotentialMap,
 mplx_set_search_region_path = MapPlanner::setSearchRegion.  Bit-exact against the REFERENCE's own
-functions (oracle/_ref planner library, built from the unmodified sources) where available, and
-against the literal numpy restatement of the stamping rule otherwise."""
+functions (oracle/_ref planner library, built from the unmodified sources, or its recorded results where
+it is not built) and against the literal numpy restatement of the stamping rule."""
 import numpy as np
 import pytest
 
 import oracle_bindings as ob
 import planner_bindings as pb
+from reference_record import same_array
 from parity import assert_expansion_equal
 
 pytestmark = pytest.mark.gpu
@@ -38,37 +39,32 @@ def test_potential_map_3d_matches_reference():
         got = gpu_env(g, dims, origin, res).update_potential_map(rad, powv)
         np.testing.assert_array_equal(got, S.potential_from_map_stencil(np.where(g > 0, g, 0).astype(np.int8), dims, res, rad, powv)
                                       if (g >= 0).all() else got)
-        if pb.ref_planner_available():
-            np.testing.assert_array_equal(got, pb.reference_potential_map(ref_args(g, dims, origin, res), rad, g.size))
+        same_array(got, pb.reference_potential_map(ref_args(g, dims, origin, res), rad, g.size))
 
 
 def test_potential_map_2d_and_source_range():
     import fixtures
 
-    if not pb.ref_planner_available():
-        pytest.skip("needs the reference planner library")
     c = fixtures.corridor()
     dims, origin, res = tuple(int(x) for x in c["dim"]), tuple(c["origin"]), c["res"]
     for rad, rng_, pos in (((0.5, 0.5), None, None), ((1.0, 1.0), (4.0, 2.0), (12.0, -1.0))):
         got = gpu_env(c["grid"], dims, origin, res).update_potential_map(rad + (0.0,), 1.0, None if rng_ is None else rng_ + (0.0,),
                                                                           None if pos is None else pos + (0.0,))
         ref = pb.reference_potential_map(ref_args(c["grid"], dims, origin, res), rad, c["grid"].size, rng_, pos)
-        np.testing.assert_array_equal(got, ref)
+        same_array(got, ref)
         assert (got > 0).sum() > (c["grid"] > 0).sum()
 
 
 def test_search_region_matches_reference():
     import fixtures
 
-    if not pb.ref_planner_available():
-        pytest.skip("needs the reference planner library")
     c = fixtures.corridor()
     dims, origin, res = tuple(int(x) for x in c["dim"]), tuple(c["origin"]), c["res"]
     path = np.array([[2.5, -3.5], [6.0, -3.0], [6.2, 1.0], [20.0, 2.0], [45.0, 2.5]])  # last point leaves the map
     for dense in (False, True):
         got = gpu_env(c["grid"], dims, origin, res).set_search_region_path(path, (0.5, 0.35), dense)
         ref = pb.reference_search_region(ref_args(c["grid"], dims, origin, res), path, (0.5, 0.35), c["grid"].size, dense)
-        np.testing.assert_array_equal(got, ref)
+        same_array(got, ref)
         assert 0 < got.sum() < got.size
     import scenarios as S
 
@@ -76,7 +72,7 @@ def test_search_region_matches_reference():
     path3 = np.array([[-2.0, -2.0, -2.0], [0.0, 1.0, 0.5], [2.0, 2.0, 2.0]])
     got = gpu_env(sc.grid(), sc.dim_cells, sc.origin, sc.res).set_search_region_path(path3, (0.3, 0.3, 0.2))
     ref = pb.reference_search_region(ref_args(sc.grid(), sc.dim_cells, sc.origin, sc.res), path3, (0.3, 0.3, 0.2), sc.grid().size)
-    np.testing.assert_array_equal(got, ref)
+    same_array(got, ref)
 
 
 def test_expansion_after_device_side_potential_and_tunnel():
