@@ -89,9 +89,24 @@ const char *mplx_last_error(void);
 /* MapUtil<Dim>::setMap (include/mpl_collision/map_util.h:85-91).  `data` is the x-fastest
  * int8 grid (occupied 100 / free 0 / unknown -1, map_util.h:309-313); it is copied to HBM.
  * dim/origin have ctx-dim entries.  Clears any potential map and search region
- * (their sizes are tied to the grid). */
+ * (their sizes are tied to the grid).  Edits of a few voxels of the same grid: mplx_update_cells. */
 int mplx_set_map(mplx_ctx *ctx, const int8_t *data, const int32_t *dim, const double *origin,
                  double res);
+
+/* Sparse MapUtil edit: grid[idx[k]] = values[k] for k < n, applied in array order (a later entry for
+ * the same voxel wins).  idx are getIndex() values (map_util.h:34-41), 0 <= idx < nvox.  Updates the
+ * int8 grid and both packed views derived from it (occupancy bits, occ2 pairs) with O(n) device work
+ * and 5n bytes over PCIe: no pass over the full grid.  The result is bit-identical to mplx_set_map of
+ * the edited grid.  Unlike mplx_set_map, the potential map and the search region are kept (the
+ * reference env holds its own copies of both: env_map.h:181-183,290; env_base.h:301-303).
+ * Synchronous, like mplx_set_map.  n == 0 is a no-op.  Any invalid argument (n < 0, a NULL array
+ * with n > 0, an index outside the grid) -> MPLX_ERR_ARG with nothing applied. */
+int mplx_update_cells(mplx_ctx *ctx, const int32_t *idx, const int8_t *values, int n);
+
+/* Diagnostics: copy the device grid (nvox bytes), the occupancy words and the occ2 pairs
+ * ((nvox+31)/32 each; a pair is {occupancy word, candidate-summary word}, 2 uint32 per pair) to
+ * host buffers; any pointer may be NULL. */
+int mplx_read_map(mplx_ctx *ctx, int8_t *grid, uint32_t *occ, uint32_t *occ2);
 
 /* env_map::set_potential_map / set_potential_weight / set_gradient_weight
  * (include/mpl_planner/env/env_map.h:181-186, 175-178).  data == NULL restores

@@ -32,6 +32,8 @@ EXPORTED_SYMBOLS = (
     "mplx_destroy",
     "mplx_last_error",
     "mplx_set_map",
+    "mplx_update_cells",
+    "mplx_read_map",
     "mplx_set_potential",
     "mplx_set_potential_weights",
     "mplx_set_search_region",
@@ -118,6 +120,10 @@ def load() -> C.CDLL:
     lib.mplx_last_error.restype = C.c_char_p
     lib.mplx_set_map.argtypes = [vp, vp, vp, vp, f64]
     lib.mplx_set_map.restype = i32
+    lib.mplx_update_cells.argtypes = [vp, vp, vp, i32]
+    lib.mplx_update_cells.restype = i32
+    lib.mplx_read_map.argtypes = [vp, vp, vp, vp]
+    lib.mplx_read_map.restype = i32
     lib.mplx_set_potential.argtypes = [vp, vp, f64, f64]
     lib.mplx_set_potential.restype = i32
     lib.mplx_set_potential_weights.argtypes = [vp, f64, f64]

@@ -29,6 +29,7 @@
 // Results are bit-identical to the other kernels: every decision is either proven equal to the
 // reference's (certain), independent of it (all candidates free), or made by the exact chain.
 #include "mplx_fx.cuh"
+#include "mplx_pack.cuh"
 
 namespace mplx {
 
@@ -336,40 +337,13 @@ cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, i
   return cudaErrorInvalidValue;
 }
 
-// {occupancy word, candidate-summary word} per 32 voxels.  Summary bit of voxel (x,y,z) = OR of the
-// occupancy of the cells {x-1,x} x {y-1,y} (x {z-1,z}), a cell outside the map counting as occupied.
+// {occupancy word, candidate-summary word} per 32 voxels (the summary rule: occ2_summary_word).
 __global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, int dim, int nx, int ny,
                                  uint2 *__restrict__ out) {
   const size_t nwords = (nvox + 31) >> 5;
-  const size_t sxy = (size_t)nx * ny;
   for (size_t wd = (size_t)blockIdx.x * blockDim.x + threadIdx.x; wd < nwords;
-       wd += (size_t)gridDim.x * blockDim.x) {
-    uint32_t d = 0;
-    const size_t b0 = wd << 5;
-    for (int b = 0; b < 32; b++) {
-      const size_t i = b0 + b;
-      if (i >= nvox) {
-        d |= 1u << b;
-        continue;
-      }
-      const int x = (int)(i % nx);
-      const int y = (int)((i / nx) % ny);
-      const int z = (int)(i / sxy);
-      unsigned any = 0;
-      for (int dz = 0; dz <= (dim == 3 ? 1 : 0); dz++)
-        for (int dy = 0; dy <= 1; dy++)
-          for (int dx = 0; dx <= 1; dx++) {
-            if (x - dx < 0 || y - dy < 0 || z - dz < 0) {
-              any = 1;
-            } else {
-              const size_t jdx = i - dx - (size_t)dy * nx - (size_t)dz * sxy;
-              any |= (occ[jdx >> 5] >> (jdx & 31)) & 1u;
-            }
-          }
-      d |= any << b;
-    }
-    out[wd] = make_uint2(occ[wd], d);
-  }
+       wd += (size_t)gridDim.x * blockDim.x)
+    out[wd] = make_uint2(occ[wd], occ2_summary_word(occ, wd, nvox, dim, nx, ny));
 }
 
 cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, uint2 *d_out, cudaStream_t st) {

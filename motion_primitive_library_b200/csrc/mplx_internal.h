@@ -147,6 +147,19 @@ struct EdgeBufs {
   }
 };
 
+// staging of the sparse grid edits (mplx_update.cu)
+struct UpdateBufs {
+  PinBuf<uint32_t> h_idx;
+  PinBuf<int8_t> h_val;
+  DevBuf<uint32_t> idx, idx_sorted;
+  DevBuf<int8_t> val, val_sorted;
+  DevBuf<uint8_t> sort_tmp;
+  void release() {
+    h_idx.release(); h_val.release(); idx.release(); idx_sorted.release(); val.release(); val_sorted.release();
+    sort_tmp.release();
+  }
+};
+
 struct mplx_ctx {
   int dim = 0, device = 0;
   cudaStream_t stream = nullptr;
@@ -178,6 +191,7 @@ struct mplx_ctx {
   cudaStream_t d2h_stream = nullptr;  // result copies of the packed pipeline
   FxQueue fxq;
   EdgeBufs eb;
+  UpdateBufs ub;
   int64_t launches = 0;
   unsigned long long last_stats[2] = {0, 0};
 };

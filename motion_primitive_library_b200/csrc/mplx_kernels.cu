@@ -27,6 +27,7 @@
 #include "../../include/mplx.h"
 #include "mplx_device.cuh"
 #include "mplx_expand.cuh"
+#include "mplx_pack.cuh"
 
 namespace mplx {
 
@@ -390,16 +391,8 @@ template <bool OCC>
 __global__ void pack_bits_kernel(const int8_t *__restrict__ bytes, size_t nvox, uint32_t *__restrict__ bits) {
   const size_t nwords = (nvox + 31) >> 5;
   for (size_t wd = (size_t)blockIdx.x * blockDim.x + threadIdx.x; wd < nwords;
-       wd += (size_t)gridDim.x * blockDim.x) {
-    uint32_t m = 0;
-    const size_t b0 = wd << 5;
-#pragma unroll 8
-    for (int b = 0; b < 32; b++) {
-      const size_t i = b0 + b;
-      if (i < nvox && (OCC ? bytes[i] == 100 : bytes[i] != 0)) m |= 1u << b;
-    }
-    bits[wd] = m;
-  }
+       wd += (size_t)gridDim.x * blockDim.x)
+    bits[wd] = pack_word<OCC>(bytes, wd, nvox);
 }
 
 cudaError_t launch_pack_bits(const int8_t *d_bytes, size_t nvox, uint32_t *d_bits, bool occ, cudaStream_t st) {

@@ -122,6 +122,44 @@ class env_map:
         abi.check(self._lib.mplx_set_map(self._h, mu.map.ctypes.data, dim.ctypes.data, org.ctypes.data, mu.res))
         self._potential = None
 
+    def update_cells(self, idx_or_cells, values):
+        """Set a few voxels of the MapUtil grid, in place, and on the device (mplx_update_cells).
+        `idx_or_cells` is either getIndex() values (1-D) or n x Dim cell coordinates; `values` has one
+        int8 per entry, and a later entry for the same voxel wins.  Costs O(n), not a re-upload, and
+        unlike upload_map() keeps the potential map and the search region."""
+        mu = self.map_util_
+        a = np.asarray(idx_or_cells)
+        if a.ndim == 2:
+            cells = a.astype(np.int64).reshape(-1, self.Dim)
+            dims = np.asarray(mu.dim, dtype=np.int64)
+            if ((cells < 0) | (cells >= dims)).any():
+                raise ValueError("cell outside the map")
+            idx = cells[:, 0] + dims[0] * cells[:, 1]
+            if self.Dim == 3:
+                idx = idx + dims[0] * dims[1] * cells[:, 2]
+        else:
+            idx = a.astype(np.int64).reshape(-1)
+        vals = np.ascontiguousarray(values, dtype=np.int8).reshape(-1)
+        if vals.size != idx.size:
+            raise ValueError("one value per cell")
+        if ((idx < 0) | (idx >= mu.map.size)).any():
+            raise ValueError("index outside the map")
+        idx32 = np.ascontiguousarray(idx, dtype=np.int32)
+        abi.check(self._lib.mplx_update_cells(self._h, idx32.ctypes.data, vals.ctypes.data, idx32.size))
+        # last write wins: the first occurrence of each index in the reversed arrays
+        u, first = np.unique(idx32[::-1], return_index=True)
+        mu.map[u] = vals[::-1][first]
+
+    def read_map(self):
+        """The device grid, occupancy words and occ2 pairs (mplx_read_map): (int8[nvox], uint32[nw], uint32[nw, 2])."""
+        nvox = self.map_util_.map.size
+        nw = (nvox + 31) // 32
+        grid = np.empty(nvox, dtype=np.int8)
+        occ = np.empty(nw, dtype=np.uint32)
+        occ2 = np.empty((nw, 2), dtype=np.uint32)
+        abi.check(self._lib.mplx_read_map(self._h, grid.ctypes.data, occ.ctypes.data, occ2.ctypes.data))
+        return grid, occ, occ2
+
     # -- setters (env_base.h:234-303, env_map.h:175-186) -------------------------------------
     def set_u(self, U):
         self.U_ = np.ascontiguousarray(U, dtype=np.float64)

@@ -245,6 +245,46 @@ int mplh_batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypo
   }
 }
 
+/* MapUtil::setCells on the session's map: cells (n x dim cell coordinates) get values[k], a later entry
+ * for the same cell winning.  The next mplh_batch_plan sends only these voxels to the device and keeps
+ * the potential map.  A cell outside the map fails the call with nothing changed. */
+int mplh_batch_update_cells(void *session, const int32_t *cells, const int8_t *values, int n) {
+  try {
+    BatchSession *s = (BatchSession *)session;
+    if (!s || !s->mq) throw std::runtime_error("null session");
+    if (n < 0 || (n > 0 && (!cells || !values))) throw std::runtime_error("cells/values missing");
+    auto go = [&](auto *mq, auto dimtag) {
+      constexpr int Dim = decltype(dimtag)::value;
+      vec_E<Veci<Dim>> pns(n);
+      for (int i = 0; i < n; i++)
+        for (int d = 0; d < Dim; d++) pns[i](d) = cells[(size_t)i * Dim + d];
+      mq->map_util().setCells(pns, std::vector<int8_t>(values, values + n));
+    };
+    if (s->dim == 2) go((MPL::MultiQueryPlanner<2> *)s->mq, std::integral_constant<int, 2>());
+    else go((MPL::MultiQueryPlanner<3> *)s->mq, std::integral_constant<int, 3>());
+    return 0;
+  } catch (const std::exception &e) {
+    g_err = e.what();
+    return 1;
+  }
+}
+
+/* Grid transfers of the session's env so far: *full = whole-grid uploads, *delta = sparse updates. */
+int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq) {
+    g_err = "null session";
+    return 1;
+  }
+  auto put = [&](const auto &env) {
+    if (full) *full = env.full_uploads();
+    if (delta) *delta = env.delta_uploads();
+  };
+  if (s->dim == 2) put(((MPL::MultiQueryPlanner<2> *)s->mq)->env());
+  else put(((MPL::MultiQueryPlanner<3> *)s->mq)->env());
+  return 0;
+}
+
 /* Frees the session incl. the search states it kept; seconds spent are returned in *release_seconds. */
 int mplh_batch_close(void *session, double *release_seconds) {
   BatchSession *s = (BatchSession *)session;

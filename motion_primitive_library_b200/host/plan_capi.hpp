@@ -195,15 +195,14 @@ void run_lpa(MPL::MapPlanner<Dim> &planner, const std::shared_ptr<MPL::MapUtil<D
       for (const auto &r : recs) fnv(h, &r, sizeof r);
       o->linked_hash = h;
     } else if (st.op == MPLH_OP_BLOCK || st.op == MPLH_OP_CLEAR) {
-      MPL::Tmap m = mu->getMap();
-      vec_E<Veci<Dim>> pns;
+      vec_E<Veci<Dim>> pns, inside;
       for (int i = 0; i < st.n; i++) {
         Veci<Dim> pn;
         for (int d = 0; d < Dim; d++) pn(d) = st.cells[(size_t)i * Dim + d];
         pns.push_back(pn);
-        if (!mu->isOutside(pn)) m[mu->getIndex(pn)] = st.op == MPLH_OP_BLOCK ? 100 : 0;
+        if (!mu->isOutside(pn)) inside.push_back(pn);
       }
-      mu->setMap(mu->getOrigin(), mu->getDim(), m, mu->getRes());
+      mu->setCells(inside, std::vector<int8_t>(inside.size(), st.op == MPLH_OP_BLOCK ? 100 : 0));
       if (st.op == MPLH_OP_BLOCK) planner.updateBlockedNodes(pns);
       else planner.updateClearedNodes(pns);
     } else if (st.op == MPLH_OP_SUBTREE) {

@@ -253,6 +253,10 @@ def _host():
     lib.mplh_batch_plan.restype = C.c_int
     lib.mplh_batch_close.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     lib.mplh_batch_close.restype = C.c_int
+    lib.mplh_batch_update_cells.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.mplh_batch_update_cells.restype = C.c_int
+    lib.mplh_batch_map_uploads.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.mplh_batch_map_uploads.restype = C.c_int
     return lib, fn
 
 
@@ -328,6 +332,23 @@ class BatchPlanner:
             res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
         return res, dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),
                          t_device=float(totals[4]), t_relax=float(totals[5]), t_release=0.0)
+
+    def update_cells(self, cells, values):
+        """MapUtil::setCells on the session's map: cells[k] (n x Dim cell coordinates) := values[k], a later
+        entry for the same cell winning.  The next plan() sends only these voxels to the device."""
+        cells = np.ascontiguousarray(cells, dtype=np.int32).reshape(-1, self._args.dim)
+        values = np.ascontiguousarray(values, dtype=np.int8).reshape(-1)
+        if values.size != len(cells):
+            raise ValueError("one value per cell")
+        if self._lib.mplh_batch_update_cells(self._h, cells.ctypes.data, values.ctypes.data, len(cells)) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+
+    def map_uploads(self):
+        """(full, delta): whole-grid uploads and sparse updates the session's env has made."""
+        full, delta = C.c_int64(0), C.c_int64(0)
+        if self._lib.mplh_batch_map_uploads(self._h, C.byref(full), C.byref(delta)) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+        return full.value, delta.value
 
     def close(self) -> float:
         """Free the session (incl. the kept search states); returns the seconds that took."""
