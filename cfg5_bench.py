@@ -68,10 +68,11 @@ def run(sc, grid, local: int, n_queries: int = 4096, max_expand: int = 1000, min
     def run_slice(mine):
         if len(mine) == 0:
             return np.zeros(0, dtype=res_dtype), dict(expansions=0, iterations=0, seconds_max=0.0, t_pop_max=0.0,
-                                                      t_device_max=0.0, t_relax_max=0.0)
+                                                      t_device_max=0.0, t_relax_max=0.0, device_path=0)
         res, tot = session.plan(mine["start"], mine["goal"])
         return res, dict(expansions=tot["nodes"], iterations=tot["iterations"], seconds_max=tot["seconds"],
-                         t_pop_max=tot["t_pop"], t_device_max=tot["t_device"], t_relax_max=tot["t_relax"])
+                         t_pop_max=tot["t_pop"], t_device_max=tot["t_device"], t_relax_max=tot["t_relax"],
+                         device_path=1 if tot["path"] == "device" else 0)
 
     # pass 0 allocates (and page-faults) the search-state memory of every query; later passes recycle it
     passes = []
@@ -90,16 +91,20 @@ def run(sc, grid, local: int, n_queries: int = 4096, max_expand: int = 1000, min
         t_rel = float(tr.item())
     cnt["t_release_max"] = t_rel
     secs = cnt["seconds_max"]
+    # the device search (mplx_plan_batch) runs each query's whole A* on the GPU: no pop / relax phases on the host
+    path = "device" if cnt.get("device_path", 0) else "lockstep"
+    phases = ({"device_search": cnt["t_device_max"]} if path == "device" else
+              {"pop": cnt["t_pop_max"], "device+pcie": cnt["t_device_max"], "relax": cnt["t_relax_max"]})
     out = {
         "workload": f"cfg5: {n_queries} start/goal pairs >= {min_dist} m apart, {sc.name}, setEpsilon({eps:g}), <= {max_expand} expansions/query, "
                     f"queries sharded over {world} rank(s)",
         "n_gpus": world, "scaling": "strong", "value": cnt["expansions"] / secs, "unit": "expansions/s",
         "expansions": int(cnt["expansions"]), "seconds": secs, "passes": len(passes),
-        "first_pass_seconds": first_seconds, "session_close_seconds": cnt["t_release_max"], "lockstep_iterations_sum": int(cnt["iterations"]),
+        "first_pass_seconds": first_seconds, "session_close_seconds": cnt["t_release_max"], "lockstep_iterations_sum": int(cnt["iterations"]) if path == "lockstep" else 0,
         "queries": n_queries, "queries_solved": int(res["valid"].sum()), "epsilon": eps, "max_expand": max_expand, "host_threads_per_rank": n_threads,
-        "phase_seconds_max": {"pop": cnt["t_pop_max"], "device+pcie": cnt["t_device_max"], "relax": cnt["t_relax_max"]},
-        "what": "sum of node expansions / max over ranks of MultiQueryPlanner::plan wall time (device expansion + PCIe + "
-                "host A* bookkeeping) for one pass over the query set in a session whose search states are recycled from "
+        "path": path, "phase_seconds_max": phases,
+        "what": "sum of node expansions / max over ranks of MultiQueryPlanner::plan wall time (path device: every query's "
+                "whole A* on the GPU, mplx_plan_batch; path lockstep: device expansion + PCIe + host A* bookkeeping) for one pass over the query set in a session whose search states are recycled from "
                 "the previous pass (first_pass_seconds = the pass that allocates them; session_close_seconds = freeing "
                 "them at the end, once per session)",
     }

@@ -219,6 +219,50 @@ int mplx_edges_cells(mplx_ctx *ctx, const mplx_waypoint *parents, const int32_t 
                      int64_t *out_offset, int32_t *out_cells, int64_t capacity, int64_t *out_total,
                      int32_t *out_table_voxel, int32_t *out_table_edge);
 
+/* ---- batched A* on the device (occupancy planning) ----------------------------------------- */
+
+/* Results of mplx_plan_batch (HOST arrays).  Query q's trajectory is actions[action_offset[q],
+ * action_offset[q+1]) (action ids from start to goal; recoverTraj, graph_search.h:369-455); its closed
+ * set is closed_keys[closed_offset[q], closed_offset[q+1]) sorted ascending (NULL closed_keys skips it).
+ * Both capacities must be at least n_q*max_expand, which always suffices. */
+typedef struct {
+  int32_t *valid;          /* [n_q] a trajectory was found (or the start is already a goal)      */
+  double *cost;            /* [n_q] its cost; +inf when none                                     */
+  int32_t *expanded;       /* [n_q] expansion iterations (pops)                                  */
+  int32_t *n_closed;       /* [n_q] closed states                                                */
+  int64_t *action_offset;  /* [n_q+1]                                                            */
+  int32_t *actions;
+  int64_t action_capacity;
+  int64_t *closed_offset;  /* [n_q+1], needed with closed_keys                                   */
+  uint64_t *closed_keys;
+  int64_t closed_capacity;
+  int32_t slots;           /* out: queries searched at once (arena slots)                        */
+  int64_t arena_bytes;     /* out: device bytes of one slot's arena                              */
+  double seconds;          /* out: device time of the search (CUDA events)                       */
+} mplx_batch_out;
+
+/* Graph search A* (graph_search.h:39-182, setEpsilon(eps), setMaxNum(max_expand)) for n_q independent
+ * (starts[q], goals[q]) queries on the ctx's map and parameters, entirely on the device: each query gives
+ * what the host planner (MPL::AstarStepper with env_map's goal test and heuristic) gives, bit for bit.
+ * The goal test is env_map::is_goal with tolerances tol_pos / tol_vel / tol_acc / tol_yaw (< 0 = off).
+ * start_free[q] != 0 says the start is free (planner_base.h:283-287); NULL = is_free(start.pos) on the
+ * device grid.  Occupancy planning only: the call fails with MPLX_ERR_ARG, and does nothing, when a
+ * potential map is installed, the control carries yaw, max_expand <= 0, nU > 256, or the map or the
+ * parameters are missing, and with MPLX_ERR_ALLOC, also doing nothing, when one worst-case arena does not fit the
+ * budget (mplx_plan_batch_fits).  Every query slot owns an arena for the worst case (1 + max_expand*nU
+ * states), so no query can overflow; the arenas stay in the ctx for the next call.  Synchronous. */
+int mplx_plan_batch(mplx_ctx *ctx, const mplx_waypoint *starts, const mplx_waypoint *goals, const uint8_t *start_free,
+                    int n_q, double eps, int max_expand, double tol_pos, double tol_vel, double tol_acc,
+                    double tol_yaw, mplx_batch_out *out);
+
+/* Whether mplx_plan_batch can run n_q queries with this max_expand (with_closed: the closed keys are
+ * asked for) on the ctx as it stands: MPLX_OK with the slots and bytes per slot it would use, MPLX_ERR_ALLOC
+ * when one worst-case arena next to the results exceeds the device-memory budget (a quarter of the free
+ * device memory, counting the search buffers the ctx holds, at most 8 GiB), MPLX_ERR_ARG for the plans
+ * mplx_plan_batch refuses.  Allocates and changes nothing.  slots / arena_bytes may be NULL. */
+int mplx_plan_batch_fits(mplx_ctx *ctx, int n_q, int max_expand, int with_closed, int32_t *slots,
+                         int64_t *arena_bytes);
+
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field
  * planning once a batch fills the GPU, else the register kernel),

@@ -45,6 +45,8 @@ EXPORTED_SYMBOLS = (
     "mplx_expand_packed",
     "mplx_edges_is_free",
     "mplx_edges_cells",
+    "mplx_plan_batch",
+    "mplx_plan_batch_fits",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -87,6 +89,26 @@ class PackedOut(C.Structure):
 
 
 PACK_DROP_INF = 1
+
+
+class BatchOut(C.Structure):
+    """mplx_batch_out"""
+
+    _fields_ = [
+        ("valid", C.c_void_p),
+        ("cost", C.c_void_p),
+        ("expanded", C.c_void_p),
+        ("n_closed", C.c_void_p),
+        ("action_offset", C.c_void_p),
+        ("actions", C.c_void_p),
+        ("action_capacity", C.c_int64),
+        ("closed_offset", C.c_void_p),
+        ("closed_keys", C.c_void_p),
+        ("closed_capacity", C.c_int64),
+        ("slots", C.c_int32),
+        ("arena_bytes", C.c_int64),
+        ("seconds", C.c_double),
+    ]
 
 
 class MplxError(RuntimeError):
@@ -146,6 +168,10 @@ def load() -> C.CDLL:
     lib.mplx_edges_is_free.restype = i32
     lib.mplx_edges_cells.argtypes = [vp, vp, vp, i32, vp, vp, C.c_int64, C.POINTER(C.c_int64), vp, vp]
     lib.mplx_edges_cells.restype = i32
+    lib.mplx_plan_batch.argtypes = [vp, vp, vp, vp, i32, f64, i32, f64, f64, f64, f64, C.POINTER(BatchOut)]
+    lib.mplx_plan_batch.restype = i32
+    lib.mplx_plan_batch_fits.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+    lib.mplx_plan_batch_fits.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

@@ -498,4 +498,22 @@ __device__ __forceinline__ int sample_group(const EnvParams &P, const double (&c
   return left <= UNR ? 1 : 0;
 }
 
+// Phase C of the register kernel (mplx_kernels.cu) and the edge cost of the device search
+// (mplx_search.cu): the reference's loop `for (t = 0; t < T; t += dt)` (env_map.h:99) in groups of UNR
+// samples with group-level control flow only (sample_group).  count = iterations of that loop
+// (sample_loop_count).
+template <int DIM, int ORD, bool YAW, int UNR>
+__device__ __forceinline__ double traverse_groups(const EnvParams &P, const double (&cf)[CoefLayout<DIM, ORD, YAW>::NCMAX],
+                                                 bool need_vel, double dt, int count, unsigned &n_samples) {
+  double c = 0;
+  double t = 0;
+  YawRot yr;
+  if (YAW) yr.init(cf[CoefLayout<DIM, ORD, YAW>::ncoef(need_vel) - 2], cf[CoefLayout<DIM, ORD, YAW>::ncoef(need_vel) - 1], dt);
+  for (int left = count;; left -= UNR) {
+    const int st = sample_group<DIM, ORD, YAW, UNR>(P, cf, need_vel, dt, left, t, c, n_samples, yr);
+    if (st == 2) return INFINITY;
+    if (st == 1) return c;
+  }
+}
+
 }  // namespace mplx

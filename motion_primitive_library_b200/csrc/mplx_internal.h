@@ -160,6 +160,30 @@ struct UpdateBufs {
   }
 };
 
+// Device memory one mplx_plan_batch call may take (arenas and results): a quarter of the free device
+// memory, at most this much.  The slot count follows from it (mplx_search.cu, size_batch).
+constexpr size_t kSearchArenaBudget = (size_t)8 << 30;
+
+// the device search (mplx_search.cu): per-slot arenas kept across calls, per-call staging
+struct SearchBufs {
+  DevBuf<unsigned char> arena;
+  int64_t layout_bytes = 0;  // bytes per slot of the layout the arena was cleared for
+  size_t cleared = 0;        // leading arena bytes cleared for that layout
+  uint32_t next_epoch = 1;   // key-table entries of earlier queries carry smaller epochs
+  DevBuf<mplx_waypoint> succ, queries;
+  DevBuf<double> cost, dres;
+  DevBuf<uint64_t> key, closed;
+  DevBuf<int32_t> action, count, ires, actions;
+  DevBuf<uint8_t> free_;
+  void release() {
+    arena.release(); succ.release(); queries.release(); cost.release(); dres.release(); key.release();
+    closed.release(); action.release(); count.release(); ires.release(); actions.release(); free_.release();
+    layout_bytes = 0;
+    cleared = 0;
+    next_epoch = 1;
+  }
+};
+
 struct mplx_ctx {
   int dim = 0, device = 0;
   cudaStream_t stream = nullptr;
@@ -192,6 +216,7 @@ struct mplx_ctx {
   FxQueue fxq;
   EdgeBufs eb;
   UpdateBufs ub;
+  SearchBufs sb;
   int64_t launches = 0;
   unsigned long long last_stats[2] = {0, 0};
 };

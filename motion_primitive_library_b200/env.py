@@ -367,6 +367,33 @@ class env_map:
             cap = int(total.value)
         abi.check(rc)
 
+    def plan_batch(self, starts, goals, eps=1.0, max_expand=1000, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
+                   tol_yaw=-1.0, start_free=None, closed=True):
+        """mplx_plan_batch: the A* searches of n (start, goal) queries on the device (occupancy planning).
+        Returns a dict: valid, cost, expanded, n_closed (arrays), actions / closed (one array per query),
+        slots, arena_bytes, seconds.  Raises MplxError (code MPLX_ERR_ARG) for the plans it refuses."""
+        self._sync_params()
+        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)
+        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE).reshape(-1)
+        n = starts.size
+        cap = max(1, n * max(int(max_expand), 0))
+        valid, expanded, n_closed = (np.zeros(n, np.int32) for _ in range(3))
+        cost = np.zeros(n)
+        aoff, coff = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+        acts = np.zeros(cap, np.int32)
+        keys = np.zeros(cap, np.uint64) if closed else None
+        sf = None if start_free is None else np.ascontiguousarray(start_free, dtype=np.uint8)
+        out = abi.BatchOut(valid.ctypes.data, cost.ctypes.data, expanded.ctypes.data, n_closed.ctypes.data,
+                           aoff.ctypes.data, acts.ctypes.data, cap, coff.ctypes.data, abi.ptr(keys), cap if closed else 0,
+                           0, 0, 0.0)
+        abi.check(self._lib.mplx_plan_batch(self._h, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps),
+                                            int(max_expand), float(tol_pos), float(tol_vel), float(tol_acc),
+                                            float(tol_yaw), C.byref(out)))
+        return dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
+                    actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
+                    closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
+                    slots=int(out.slots), arena_bytes=int(out.arena_bytes), seconds=float(out.seconds))
+
     def set_kernel(self, which: int):
         """0 = auto, 1 = literal sequential loop, 2 = register kernel, 3 = flat kernel, 4 = dealing kernel."""
         abi.check(self._lib.mplx_set_kernel(self._h, int(which)))

@@ -805,6 +805,11 @@ class env_map_gpu : public env_map_host<Dim> {
   static mplx_waypoint pod(const Waypoint<Dim> &w) { return to_pod(w); }
   int control() const { return control_; }
 
+  /// bring the device copy of the map (sparse edits as sparse updates), the parameters, the potential
+  /// map and the tunnel up to date, for callers of the ctx's other entry points (mplx_plan_batch)
+  void prepare_device() const { sync(); }
+  mplx_ctx *ctx() const { return ctx_; }
+
   long stats_nodes() const { return stats_nodes_; }
   long stats_calls() const { return stats_calls_; }
   long stats_hits() const { return stats_hits_; }
@@ -2040,7 +2045,18 @@ class MultiQueryPlanner {
     int expanded = 0;
     std::size_t n_closed = 0;
     std::vector<int> actions;
+    std::vector<uint64_t> closed_keys;  // sorted; only with setCollectClosed(true)
   };
+  /// Which loop plan() runs: AUTO picks the device search (mplx_plan_batch) for occupancy planning with
+  /// max_expand > 0 and |U| <= 256 once the batch has kDeviceSearchMinQueries queries and its worst-case
+  /// search memory fits the device-memory budget (mplx_plan_batch_fits), else the lock-step loop;
+  /// LOCKSTEP always runs the lock-step loop; DEVICE takes the device search whenever the control and
+  /// the cap allow it, whatever the batch size, and fails when the memory does not fit.  Both loops give
+  /// every query the same result.
+  enum Path { AUTO = 0, LOCKSTEP = 1, DEVICE = 2 };
+  /// Smallest batch AUTO sends to the device search.  search_bench.py, one H100 80GB HBM3 (the
+  /// measurements are cited in DESIGN.md §7): the device search was faster at every measured batch size.
+  static constexpr std::size_t kDeviceSearchMinQueries = 16;
   explicit MultiQueryPlanner(const std::shared_ptr<MapUtil<Dim>> &map_util, int device = 0)
       : map_util_(map_util), gpu_(new env_map_gpu<Dim>(map_util, device)) {}
   /// the shared env: set U, limits, weights, control, tolerances on it
@@ -2058,9 +2074,32 @@ class MultiQueryPlanner {
   void setHostThreads(int n) { host_threads_ = n; }
   /// keys-only result stream for occupancy planning (default on; see env_map_gpu::expand_packed)
   void setKeysOnly(bool on) { keys_only_ = on; }
+  /// diagnostics: force a path (Path); AUTO is the default
+  void setPath(int p) { path_ = p; }
+  /// also return each query's closed set (sorted lattice keys) in Result::closed_keys
+  void setCollectClosed(bool on) { collect_closed_ = on; }
+  /// the path the last plan() ran: true = device search
+  bool lastPlanOnDevice() const { return last_device_; }
+  /// device search of the last plan(): arena slots and bytes per slot (0 after a lock-step plan)
+  int searchSlots() const { return slots_; }
+  long long searchArenaBytes() const { return arena_bytes_; }
+
+  /// the device search serves this plan: occupancy planning, a bounded search, |U| within one CTA
+  bool deviceSearchPossible(int max_expand) const {
+    return gpu_->keys_only_possible() && max_expand > 0 && gpu_->U_.size() <= 256;
+  }
 
   std::vector<Result> plan(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
                            int max_expand) {
+    last_device_ = false;
+    slots_ = 0;
+    arena_bytes_ = 0;
+    if (path_ != LOCKSTEP && deviceSearchPossible(max_expand) &&
+        (path_ == DEVICE || starts.size() >= kDeviceSearchMinQueries)) {
+      std::vector<Result> res;
+      if (plan_device(starts, goals, eps, max_expand, res)) return res;
+    }
+    last_device_ = false;
     // the search states of the previous plan() are recycled, not freed: a planner that answers batch
     // after batch allocates (and page-faults) its state memory once
     if (ss_.size() != starts.size()) release();
@@ -2132,9 +2171,70 @@ class MultiQueryPlanner {
       res[q].valid = !std::isinf(res[q].cost);
       res[q].expanded = st[q]->expanded();
       for (const auto &e : traj) res[q].actions.push_back(e.action_id);
-      for (const auto *stt : ss[q]->order_) if (stt->iterationclosed) res[q].n_closed++;
+      for (const auto *stt : ss[q]->order_)
+        if (stt->iterationclosed) {
+          res[q].n_closed++;
+          if (collect_closed_) res[q].closed_keys.push_back((uint64_t)stt->key);
+        }
+      std::sort(res[q].closed_keys.begin(), res[q].closed_keys.end());
     });
     return res;
+  }
+
+  /// plan() on the device: every query's whole A* in one mplx_plan_batch call.  The start-is-free test
+  /// runs here on the host map, as in the lock-step loop.  Returns false, with nothing planned, when the
+  /// worst-case search memory does not fit the device-memory budget (MPLX_ERR_ALLOC) under AUTO: the
+  /// caller then runs the lock-step loop, which served such plans before.  DEVICE reports it as an error.
+  bool plan_device(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
+                   int max_expand, std::vector<Result> &res) {
+    const std::size_t Q = starts.size();
+    res.assign(Q, Result());
+    iterations_ = nodes_ = 0;
+    t_pop_ = t_dev_ = t_relax_ = 0;
+    gpu_->prepare_device();
+    // sized before any result buffer exists: the host arrays below are as large as the device's
+    const int fit = mplx_plan_batch_fits(gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
+    if (fit == MPLX_ERR_ALLOC && path_ == AUTO) return false;
+    if (fit != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    last_device_ = true;
+    if (Q == 0) return true;
+    std::vector<mplx_waypoint> S(Q), G(Q);
+    std::vector<uint8_t> fr(Q);
+    for (std::size_t q = 0; q < Q; q++) {
+      S[q] = env_map_gpu<Dim>::pod(starts[q]);
+      G[q] = env_map_gpu<Dim>::pod(goals[q]);
+      fr[q] = map_util_->isFree(map_util_->floatToInt(starts[q].pos)) ? 1 : 0;  // env_map.h:48-51
+    }
+    std::vector<int32_t> valid(Q), expd(Q), ncl(Q), acts(Q * (std::size_t)max_expand);
+    std::vector<double> cost(Q);
+    std::vector<int64_t> aoff(Q + 1), coff(Q + 1);
+    std::vector<uint64_t> keys(collect_closed_ ? Q * (std::size_t)max_expand : 0);
+    mplx_batch_out out{valid.data(), cost.data(), expd.data(), ncl.data(), aoff.data(), acts.data(),
+                       (int64_t)acts.size(), collect_closed_ ? coff.data() : nullptr,
+                       collect_closed_ ? keys.data() : nullptr, (int64_t)keys.size(), 0, 0, 0.0};
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc = mplx_plan_batch(gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_,
+                                   gpu_->tol_vel_, gpu_->tol_acc_, gpu_->tol_yaw_, &out);
+    // the device allocation itself can still fail when other users of the card took memory in between
+    if (rc == MPLX_ERR_ALLOC && path_ == AUTO) {
+      last_device_ = false;
+      return false;
+    }
+    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    slots_ = out.slots;
+    arena_bytes_ = out.arena_bytes;
+    for (std::size_t q = 0; q < Q; q++) {
+      res[q].valid = valid[q] != 0;
+      res[q].cost = cost[q];
+      res[q].expanded = expd[q];
+      res[q].n_closed = (std::size_t)ncl[q];
+      res[q].actions.assign(acts.begin() + aoff[q], acts.begin() + aoff[q + 1]);
+      if (collect_closed_) res[q].closed_keys.assign(keys.begin() + coff[q], keys.begin() + coff[q + 1]);
+      iterations_ = std::max<long>(iterations_, expd[q]);
+      nodes_ += expd[q];
+    }
+    return true;
   }
   /// Free the search states of the last plan() (tens of millions of states for a large batch), on
   /// the host cores.  Called by the next plan() and the destructor.
@@ -2165,6 +2265,10 @@ class MultiQueryPlanner {
   double t_pop_ = 0, t_dev_ = 0, t_relax_ = 0;
   int host_threads_ = 0;
   bool keys_only_ = true;
+  int path_ = AUTO;
+  bool collect_closed_ = false, last_device_ = false;
+  int slots_ = 0;
+  long long arena_bytes_ = 0;
   static constexpr int kMaxSucc = 1024;  // |U| upper bound of libmplx
 };
 }  // namespace MPL

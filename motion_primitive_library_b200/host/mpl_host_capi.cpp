@@ -285,6 +285,96 @@ int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
   return 0;
 }
 
+/* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (the device search for
+ * occupancy planning with a bounded search once the batch is large enough), 1 = always lock-step,
+ * 2 = the device search whenever the plan allows it. */
+int mplh_batch_set_path(void *session, int path) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq || path < 0 || path > 2) {
+    g_err = "null session or path not in 0..2";
+    return 1;
+  }
+  if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setPath(path);
+  else ((MPL::MultiQueryPlanner<3> *)s->mq)->setPath(path);
+  return 0;
+}
+
+/* The last plan of the session: *device = 1 when it ran the device search (then *slots and *arena_bytes
+ * describe its arenas), 0 when it ran the lock-step loop. */
+int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t *arena_bytes) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq) {
+    g_err = "null session";
+    return 1;
+  }
+  auto put = [&](const auto *mq) {
+    if (device) *device = mq->lastPlanOnDevice() ? 1 : 0;
+    if (slots) *slots = mq->searchSlots();
+    if (arena_bytes) *arena_bytes = mq->searchArenaBytes();
+  };
+  if (s->dim == 2) put((const MPL::MultiQueryPlanner<2> *)s->mq);
+  else put((const MPL::MultiQueryPlanner<3> *)s->mq);
+  return 0;
+}
+
+/* mplh_batch_plan that also returns every query's trajectory (action ids, query q's at
+ * actions[action_offset[q], action_offset[q+1])) and closed set (sorted lattice keys, likewise with
+ * closed_offset; closed_keys NULL = skip).  A capacity that is too small fails the call. */
+int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
+                           int max_num, mplh_query_result *out, double *totals, int64_t *action_offset, int32_t *actions,
+                           int64_t cap_actions, int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
+  try {
+    BatchSession *s = (BatchSession *)session;
+    if (!s || !s->mq) throw std::runtime_error("null session");
+    if (!action_offset || !actions || (closed_keys && !closed_offset)) throw std::runtime_error("missing output array");
+    auto go = [&](auto *mq, auto dimtag) {
+      constexpr int Dim = decltype(dimtag)::value;
+      mq->setCollectClosed(closed_keys != nullptr);
+      // the session's later plans must not keep collecting, whatever plan() does
+      struct Reset {
+        decltype(mq) p;
+        ~Reset() { p->setCollectClosed(false); }
+      } reset{mq};
+      vec_E<Waypoint<Dim>> S, G;
+      for (int q = 0; q < n_q; q++) {
+        S.push_back(mplh::wp_from<Dim>(starts[q], s->control));
+        G.push_back(mplh::wp_from<Dim>(goals[q], s->control));
+      }
+      auto t0 = std::chrono::steady_clock::now();
+      auto res = mq->plan(S, G, eps, max_num);
+      const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      int64_t ao = 0, co = 0;
+      action_offset[0] = 0;
+      if (closed_offset) closed_offset[0] = 0;
+      for (int q = 0; q < n_q; q++) {
+        out[q].valid = res[q].valid ? 1 : 0;
+        out[q].cost = res[q].cost;
+        out[q].expanded = res[q].expanded;
+        out[q].n_closed = (int)res[q].n_closed;
+        out[q].n_actions = (int)res[q].actions.size();
+        if (ao + (int64_t)res[q].actions.size() > cap_actions) throw std::runtime_error("action capacity too small");
+        for (int a : res[q].actions) actions[ao++] = a;
+        action_offset[q + 1] = ao;
+        if (closed_keys) {
+          if (co + (int64_t)res[q].closed_keys.size() > cap_closed) throw std::runtime_error("closed capacity too small");
+          for (uint64_t k : res[q].closed_keys) closed_keys[co++] = k;
+          closed_offset[q + 1] = co;
+        }
+      }
+      if (totals) {
+        totals[0] = (double)mq->iterations(); totals[1] = (double)mq->nodes_expanded(); totals[2] = secs;
+        totals[3] = mq->t_pop(); totals[4] = mq->t_device(); totals[5] = mq->t_relax(); totals[6] = 0.0;
+      }
+    };
+    if (s->dim == 2) go((MPL::MultiQueryPlanner<2> *)s->mq, std::integral_constant<int, 2>());
+    else go((MPL::MultiQueryPlanner<3> *)s->mq, std::integral_constant<int, 3>());
+    return 0;
+  } catch (const std::exception &e) {
+    g_err = e.what();
+    return 1;
+  }
+}
+
 /* Frees the session incl. the search states it kept; seconds spent are returned in *release_seconds. */
 int mplh_batch_close(void *session, double *release_seconds) {
   BatchSession *s = (BatchSession *)session;

@@ -257,6 +257,14 @@ def _host():
     lib.mplh_batch_update_cells.restype = C.c_int
     lib.mplh_batch_map_uploads.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.mplh_batch_map_uploads.restype = C.c_int
+    lib.mplh_batch_set_path.argtypes = [C.c_void_p, C.c_int]
+    lib.mplh_batch_set_path.restype = C.c_int
+    lib.mplh_batch_last_path.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+    lib.mplh_batch_last_path.restype = C.c_int
+    lib.mplh_batch_plan_detail.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                           C.c_int64]
+    lib.mplh_batch_plan_detail.restype = C.c_int
     return lib, fn
 
 
@@ -282,23 +290,18 @@ def plan_trace(args, cap=1 << 20):
     return out
 
 
-def plan_batch(args, starts, goals):
-    """MPL::MultiQueryPlanner: lock-step A* over many (start, goal) pairs; one device launch per
-    iteration expands the current node of every live query.  starts/goals: WAYPOINT_DTYPE arrays."""
-    lib, _ = _host()
-    starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
-    goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
-    nq = len(starts)
-    out = (QueryResult * max(nq, 1))()
-    totals = np.zeros(7)
-    rc = lib.mplh_plan_batch(C.byref(args), starts.ctypes.data, goals.ctypes.data, nq, out, totals.ctypes.data)
-    if rc != 0:
-        raise RuntimeError(lib.mplh_last_error().decode())
-    res = np.zeros(nq, dtype=[("valid", "i4"), ("cost", "f8"), ("expanded", "i4"), ("n_closed", "i4"), ("n_actions", "i4")])
-    for q in range(nq):
-        res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
-    return res, dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),
-                     t_device=float(totals[4]), t_relax=float(totals[5]), t_release=float(totals[6]))
+def plan_batch(args, starts, goals, path="auto"):
+    """MPL::MultiQueryPlanner over many (start, goal) pairs, one session opened and closed around the call.
+    path: "auto" (the device search for occupancy planning with a bounded search once the batch is large
+    enough, else the lock-step loop: one device launch per iteration expands the current node of every live
+    query), "lockstep" or "device" (see BatchPlanner).  starts/goals: WAYPOINT_DTYPE arrays."""
+    s = BatchPlanner(args, path=path)
+    try:
+        res, tot = s.plan(starts, goals)
+    finally:
+        tot_release = s.close()
+    tot["t_release"] = tot_release
+    return res, tot
 
 
 _QRES = [("valid", "i4"), ("cost", "f8"), ("expanded", "i4"), ("n_closed", "i4"), ("n_actions", "i4")]
@@ -307,14 +310,69 @@ _QRES = [("valid", "i4"), ("cost", "f8"), ("expanded", "i4"), ("n_closed", "i4")
 class BatchPlanner:
     """A MPL::MultiQueryPlanner session: the map is uploaded once, and the search states of one query set
     are recycled for the next (a planner that answers batch after batch allocates its state memory once).
-    `args` supplies the map, the controls and the limits (its start/goal are ignored)."""
+    `args` supplies the map, the controls and the limits (its start/goal are ignored).
 
-    def __init__(self, args):
+    path: "auto" runs each query's whole A* on the device (mplx_plan_batch) for occupancy planning (no
+    potential map, no yaw control) with max_num > 0 once the batch is large enough, and the lock-step loop
+    otherwise; "lockstep" always runs the lock-step loop, "device" the device search whenever the plan allows
+    it.  Every path gives each query the same result; the choice is a diagnostic.  The totals of plan()
+    say which ran ("path")."""
+
+    PATHS = {"auto": 0, "lockstep": 1, "device": 2}
+
+    def __init__(self, args, path="auto"):
         self._lib, _ = _host()
         self._args = args  # keeps the arrays the struct points at alive
         self._h = self._lib.mplh_batch_open(C.byref(args))
         if not self._h:
             raise RuntimeError(self._lib.mplh_last_error().decode())
+        self.set_path(path)
+
+    def set_path(self, path):
+        if path not in self.PATHS:
+            raise ValueError(f"path must be one of {sorted(self.PATHS)}")
+        if self._lib.mplh_batch_set_path(self._h, self.PATHS[path]) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+
+    def _last_path(self):
+        dev, slots, nbytes = C.c_int32(0), C.c_int32(0), C.c_int64(0)
+        if self._lib.mplh_batch_last_path(self._h, C.byref(dev), C.byref(slots), C.byref(nbytes)) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+        return dict(path="device" if dev.value else "lockstep", slots=int(slots.value), arena_bytes=int(nbytes.value))
+
+    def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True):
+        """plan() that also returns every query's trajectory (action ids) and closed set (sorted lattice keys):
+        (res, totals, actions, closed) with one array per query in actions / closed."""
+        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
+        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
+        nq = len(starts)
+        mx = self._args.max_num if max_num is None else max_num
+        if mx <= 0:
+            raise ValueError("plan_detail needs max_num > 0 (it sizes the outputs)")
+        out = (QueryResult * max(nq, 1))()
+        totals = np.zeros(7)
+        cap = max(1, nq * mx)
+        aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
+        acts = np.zeros(cap, np.int32)
+        keys = np.zeros(cap, np.uint64) if closed else None
+        rc = self._lib.mplh_batch_plan_detail(self._h, starts.ctypes.data, goals.ctypes.data, nq,
+                                              self._args.eps if eps is None else eps, mx, out, totals.ctypes.data,
+                                              aoff.ctypes.data, acts.ctypes.data, cap, coff.ctypes.data,
+                                              None if keys is None else keys.ctypes.data, cap if closed else 0)
+        if rc != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+        res = np.zeros(nq, dtype=_QRES)
+        for q in range(nq):
+            res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        tot = self._totals(totals)
+        return (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
+                [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
+
+    def _totals(self, totals):
+        t = dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),
+                 t_device=float(totals[4]), t_relax=float(totals[5]), t_release=0.0)
+        t.update(self._last_path())
+        return t
 
     def plan(self, starts, goals, eps=None, max_num=None):
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
@@ -330,8 +388,7 @@ class BatchPlanner:
         res = np.zeros(nq, dtype=_QRES)
         for q in range(nq):
             res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
-        return res, dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),
-                         t_device=float(totals[4]), t_relax=float(totals[5]), t_release=0.0)
+        return res, self._totals(totals)
 
     def update_cells(self, cells, values):
         """MapUtil::setCells on the session's map: cells[k] (n x Dim cell coordinates) := values[k], a later
