@@ -206,6 +206,7 @@ def test_cfg5_full_set_identical():
                              a_max=sc.a_max, T=sc.T, w=sc.w, max_num=1000, eps=2.0)
             o = pb.plan_reference(a)
             assert o["n_closed"] == d[0]["n_closed"][k] and o["valid"] == d[0]["valid"][k]
+            assert np.array_equal(np.sort(o["closed"]), d[3][k]) and np.array_equal(o["actions"], d[2][k])
             if o["valid"]:
                 assert o["cost"] == d[0]["cost"][k]
 
