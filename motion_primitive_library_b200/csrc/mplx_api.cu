@@ -88,7 +88,7 @@ int mplx_create(int dim, int device, mplx_ctx **out) {
   c->device = device;
   if (const char *k = getenv("MPLX_KERNEL")) {  // diagnostics: initial mplx_set_kernel value
     const int w = atoi(k);
-    if (w >= 0 && w <= 5) c->force_seq = w;
+    if (w >= 0 && w <= 5) c->kernel = w;
   }
   memset(&c->P, 0, sizeof c->P);
   c->P.dim = dim;
@@ -312,8 +312,9 @@ int mplx_expand_device(mplx_ctx *c, const void *d_nodes, int n_nodes, const mplx
   cudaStream_t st = stream ? (cudaStream_t)stream : c->stream;
   if (c->stats_on) CU(cudaMemsetAsync(c->stats.p, 0, 2 * sizeof(unsigned long long), st));
   CU(c->fxq.reserve((size_t)n_nodes * c->P.nU));
-  CU(mplx::launch_expand(c->P, (const mplx_waypoint *)d_nodes, n_nodes, *out, st, c->force_seq, &c->fxq.view));
-  c->launches += mplx::fxn_supported(c->P, n_nodes) && c->force_seq == 0 ? 2 : 1;
+  int launches = 0;
+  CU(mplx::launch_expand(c->P, (const mplx_waypoint *)d_nodes, n_nodes, *out, st, c->kernel, &c->fxq.view, &launches));
+  c->launches += launches;
   if (c->stats_on)
     CU(cudaMemcpyAsync(c->last_stats, c->stats.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   return MPLX_OK;
@@ -372,8 +373,9 @@ int mplx_expand(mplx_ctx *c, const mplx_waypoint *nodes, int n_nodes, const mplx
     d.key = out->key ? (pin_key ? out->key : c->h_key.p) : nullptr;
     d.lattice = out->lattice ? (pin_lat ? out->lattice : c->h_lattice.p) : nullptr;
     CU(c->fxq.reserve(sm));
-    CU(mplx::launch_expand(c->P, src, m, d, st, c->force_seq, &c->fxq.view));
-    c->launches += mplx::fxn_supported(c->P, m) && c->force_seq == 0 ? 2 : 1;
+    int launches = 0;
+    CU(mplx::launch_expand(c->P, src, m, d, st, c->kernel, &c->fxq.view, &launches));
+    c->launches += launches;
     CU(cudaStreamSynchronize(st));
     if (!pin_count) memcpy(out->count, c->h_count.p, sizeof(int32_t) * m);
     if (out->succ && !pin_succ) memcpy(out->succ, c->h_succ.p, sizeof(mplx_waypoint) * sm);
@@ -403,8 +405,9 @@ int mplx_expand(mplx_ctx *c, const mplx_waypoint *nodes, int n_nodes, const mplx
     d.lattice = out->lattice ? c->d_lattice.p : nullptr;
     if (c->stats_on) CU(cudaMemsetAsync(c->stats.p, 0, 2 * sizeof(unsigned long long), st));
     CU(c->fxq.reserve((size_t)m * nU));
-    CU(mplx::launch_expand(c->P, c->d_nodes.p, m, d, st, c->force_seq, &c->fxq.view));
-    c->launches += mplx::fxn_supported(c->P, m) && c->force_seq == 0 ? 2 : 1;
+    int launches = 0;
+    CU(mplx::launch_expand(c->P, c->d_nodes.p, m, d, st, c->kernel, &c->fxq.view, &launches));
+    c->launches += launches;
     if (c->stats_on)
       CU(cudaMemcpyAsync(c->last_stats, c->stats.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
 #define D2H(field, T, mult, pinflag, hbuf)                                                              \
@@ -446,7 +449,7 @@ int mplx_set_kernel(mplx_ctx *c, int which) {
   if (!c) return fail(MPLX_ERR_ARG, "null ctx");
   if (which < 0 || which > 5)
     return fail(MPLX_ERR_ARG, "which must be 0 (auto), 1 (sequential), 2 (register), 3 (flat), 4 (dealing) or 5 (fixed-point)");
-  c->force_seq = which;
+  c->kernel = which;
   return MPLX_OK;
 }
 

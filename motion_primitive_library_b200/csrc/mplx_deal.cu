@@ -13,6 +13,7 @@
 // which primitives are sampled does not enter any result).
 #include <stdlib.h>
 
+#include "mplx_dispatch.h"
 #include "mplx_expand.cuh"
 
 namespace mplx {
@@ -155,51 +156,10 @@ expand_deal_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__r
   }
 }
 
-template <int DIM, int ORD, bool YAW>
-static cudaError_t launch_deal_t(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &so,
-                                 cudaStream_t st, int rounds) {
-  const OutPtrs o{so.count, so.succ, so.cost, so.action, so.key, so.lattice};
-  const int npb = kThreads / P.nU;
-  const int per_cta = npb * rounds;
-  const int grid = (n_nodes + per_cta - 1) / per_cta;
-  const size_t smem = (size_t)rounds * kThreads * sizeof(Ticket);
-  const bool nv = YAW || (P.pot != nullptr && P.grad_w != 0.0);
-  static const int unr_env = [] { const char *v = getenv("MPLX_DEAL_UNR"); return v ? atoi(v) : 0; }();  // tuning
-  // groups of 2 samples when per-sample cost terms are summed (yaw alignment, gradient): groups of 4 spill
-  // ~220 B per thread there (cfg4: 2.00 -> 1.68 ms per 262 144 nodes), and for short loops
-  const bool short_loops = unr_env ? unr_env == 2 : (P.maxn <= 15 || nv);
-  const bool lat = o.lattice != nullptr;
-#define MPLX_LAUNCH_DEAL(VEL, UNR, LAT) \
-  expand_deal_kernel<DIM, ORD, YAW, VEL, UNR, 4, LAT><<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, o, rounds)
-  if (nv) {
-    if (short_loops) { if (lat) MPLX_LAUNCH_DEAL(true, 2, true); else MPLX_LAUNCH_DEAL(true, 2, false); }
-    else { if (lat) MPLX_LAUNCH_DEAL(true, 4, true); else MPLX_LAUNCH_DEAL(true, 4, false); }
-  } else {
-    if (short_loops) { if (lat) MPLX_LAUNCH_DEAL(YAW, 2, true); else MPLX_LAUNCH_DEAL(YAW, 2, false); }
-    else { if (lat) MPLX_LAUNCH_DEAL(YAW, 4, true); else MPLX_LAUNCH_DEAL(YAW, 4, false); }
-  }
-#undef MPLX_LAUNCH_DEAL
-  return cudaGetLastError();
-}
-
-template <int DIM>
-static cudaError_t launch_deal_d(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &o,
-                                 cudaStream_t st, int rounds) {
-  const bool yaw = (P.control & 16) != 0;
-  switch (P.control & 15) {
-    case MPLX_VEL: return yaw ? launch_deal_t<DIM, 1, true>(P, d_nodes, n_nodes, o, st, rounds) : launch_deal_t<DIM, 1, false>(P, d_nodes, n_nodes, o, st, rounds);
-    case MPLX_ACC: return yaw ? launch_deal_t<DIM, 2, true>(P, d_nodes, n_nodes, o, st, rounds) : launch_deal_t<DIM, 2, false>(P, d_nodes, n_nodes, o, st, rounds);
-    case MPLX_JRK: return yaw ? launch_deal_t<DIM, 3, true>(P, d_nodes, n_nodes, o, st, rounds) : launch_deal_t<DIM, 3, false>(P, d_nodes, n_nodes, o, st, rounds);
-    case MPLX_SNP: return yaw ? launch_deal_t<DIM, 4, true>(P, d_nodes, n_nodes, o, st, rounds) : launch_deal_t<DIM, 4, false>(P, d_nodes, n_nodes, o, st, rounds);
-  }
-  return cudaErrorInvalidValue;
-}
-
 // rounds: batches of 256 items per CTA.  More rounds = better lane use in phase C but fewer,
 // longer CTAs; keep at least ~8 CTAs per resident slot (SMs x 4 CTAs) so the grid tail stays small.
-cudaError_t launch_expand_deal(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &o,
+cudaError_t launch_expand_deal(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const OutPtrs &o,
                                cudaStream_t st, int rounds) {
-  if (n_nodes <= 0) return cudaSuccess;
   const int npb = kThreads / P.nU;
   if (rounds <= 0) {
     const long ctas1 = ((long)n_nodes + npb - 1) / npb;  // CTAs at one round each
@@ -207,7 +167,31 @@ cudaError_t launch_expand_deal(const EnvParams &P, const mplx_waypoint *d_nodes,
     rounds = rounds < 1 ? 1 : (rounds > kDealMaxRounds ? kDealMaxRounds : rounds);
   }
   if (rounds > kDealMaxRounds) rounds = kDealMaxRounds;
-  return P.dim == 2 ? launch_deal_d<2>(P, d_nodes, n_nodes, o, st, rounds) : launch_deal_d<3>(P, d_nodes, n_nodes, o, st, rounds);
+  const int per_cta = npb * rounds;
+  const int grid = (n_nodes + per_cta - 1) / per_cta;
+  const size_t smem = (size_t)rounds * kThreads * sizeof(Ticket);
+  const bool yaw = (P.control & 16) != 0;
+  const bool vel = need_vel(P, yaw);
+  static const int unr_env = [] { const char *v = getenv("MPLX_DEAL_UNR"); return v ? atoi(v) : 0; }();  // tuning
+  // groups of 2 samples when per-sample cost terms are summed (yaw alignment, gradient): groups of 4 spill
+  // ~220 B per thread there (cfg4: 2.00 -> 1.68 ms per 262 144 nodes), and for short loops
+  const bool short_loops = unr_env ? unr_env == 2 : (P.maxn <= 15 || vel);
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      return with_bool(yaw, [&](auto YAW) {
+        return with_bool(vel, [&](auto V) {
+          return with_bool(short_loops, [&](auto SHORT) {
+            return with_bool(o.lattice != nullptr, [&](auto LAT) {
+              // vel is always true with yaw: no VEL = false instantiation for it
+              expand_deal_kernel<DIM, ORD, YAW, YAW || V, SHORT ? 2 : 4, 4, LAT>
+                  <<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, o, rounds);
+              return cudaGetLastError();
+            });
+          });
+        });
+      });
+    });
+  });
 }
 
 }  // namespace mplx

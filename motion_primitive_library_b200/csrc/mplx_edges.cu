@@ -20,6 +20,7 @@
 #include <limits.h>
 #include <math.h>
 
+#include "mplx_dispatch.h"
 #include "mplx_internal.h"
 #include "mplx_prim.cuh"
 
@@ -143,31 +144,27 @@ edges_cells_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__r
   if (!WRITE) count[e] = k_out;
 }
 
-template <int DIM>
 static cudaError_t launch_free(const EnvParams &P, const mplx_waypoint *parents, const int32_t *actions, int n,
                                uint8_t *out_free, double *out_cost, cudaStream_t st) {
-  const int grid = (n + 127) / 128;
-  switch (__builtin_popcount(P.control & 15)) {
-    case 1: edges_free_kernel<DIM, 1><<<grid, 128, 0, st>>>(P, parents, actions, n, out_free, out_cost); break;
-    case 2: edges_free_kernel<DIM, 2><<<grid, 128, 0, st>>>(P, parents, actions, n, out_free, out_cost); break;
-    case 3: edges_free_kernel<DIM, 3><<<grid, 128, 0, st>>>(P, parents, actions, n, out_free, out_cost); break;
-    default: edges_free_kernel<DIM, 4><<<grid, 128, 0, st>>>(P, parents, actions, n, out_free, out_cost); break;
-  }
-  return cudaGetLastError();
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      edges_free_kernel<DIM, ORD><<<(n + 127) / 128, 128, 0, st>>>(P, parents, actions, n, out_free, out_cost);
+      return cudaGetLastError();
+    });
+  });
 }
 
-template <int DIM, bool WRITE>
+template <bool WRITE>
 static cudaError_t launch_cells(const EnvParams &P, const mplx_waypoint *parents, const int32_t *actions, int n,
                                 long long *count, const long long *offset, int32_t *cells, int32_t *ids, int32_t *owner,
                                 cudaStream_t st) {
-  const int grid = (n + 127) / 128;
-  switch (__builtin_popcount(P.control & 15)) {
-    case 1: edges_cells_kernel<DIM, 1, WRITE><<<grid, 128, 0, st>>>(P, parents, actions, n, count, offset, cells, ids, owner); break;
-    case 2: edges_cells_kernel<DIM, 2, WRITE><<<grid, 128, 0, st>>>(P, parents, actions, n, count, offset, cells, ids, owner); break;
-    case 3: edges_cells_kernel<DIM, 3, WRITE><<<grid, 128, 0, st>>>(P, parents, actions, n, count, offset, cells, ids, owner); break;
-    default: edges_cells_kernel<DIM, 4, WRITE><<<grid, 128, 0, st>>>(P, parents, actions, n, count, offset, cells, ids, owner); break;
-  }
-  return cudaGetLastError();
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      edges_cells_kernel<DIM, ORD, WRITE>
+          <<<(n + 127) / 128, 128, 0, st>>>(P, parents, actions, n, count, offset, cells, ids, owner);
+      return cudaGetLastError();
+    });
+  });
 }
 
 }  // namespace mplx
@@ -193,10 +190,7 @@ extern "C" int mplx_edges_is_free(mplx_ctx *c, const mplx_waypoint *parents, con
   cudaStream_t st = c->stream;
   CU(cudaMemcpyAsync(B.parents.p, parents, sizeof(mplx_waypoint) * n_edges, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(B.actions.p, actions, sizeof(int32_t) * n_edges, cudaMemcpyHostToDevice, st));
-  if (c->dim == 2)
-    CU(mplx::launch_free<2>(c->P, B.parents.p, B.actions.p, n_edges, B.free_.p, out_cost ? B.cost.p : nullptr, st));
-  else
-    CU(mplx::launch_free<3>(c->P, B.parents.p, B.actions.p, n_edges, B.free_.p, out_cost ? B.cost.p : nullptr, st));
+  CU(mplx::launch_free(c->P, B.parents.p, B.actions.p, n_edges, B.free_.p, out_cost ? B.cost.p : nullptr, st));
   c->launches += 1;
   CU(cudaMemcpyAsync(out_free, B.free_.p, n_edges, cudaMemcpyDeviceToHost, st));
   if (out_cost) CU(cudaMemcpyAsync(out_cost, B.cost.p, sizeof(double) * n_edges, cudaMemcpyDeviceToHost, st));
@@ -223,10 +217,7 @@ extern "C" int mplx_edges_cells(mplx_ctx *c, const mplx_waypoint *parents, const
   CU(cudaMemcpyAsync(B.parents.p, parents, sizeof(mplx_waypoint) * n_edges, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(B.actions.p, actions, sizeof(int32_t) * n_edges, cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(B.count.p + n_edges, 0, sizeof(long long), st));
-  if (dim == 2)
-    CU((mplx::launch_cells<2, false>(c->P, B.parents.p, B.actions.p, n_edges, B.count.p, nullptr, nullptr, nullptr, nullptr, st)));
-  else
-    CU((mplx::launch_cells<3, false>(c->P, B.parents.p, B.actions.p, n_edges, B.count.p, nullptr, nullptr, nullptr, nullptr, st)));
+  CU(mplx::launch_cells<false>(c->P, B.parents.p, B.actions.p, n_edges, B.count.p, nullptr, nullptr, nullptr, nullptr, st));
   // exclusive scan over n_edges+1 counts: offset[n_edges] = total
   size_t tmp_bytes = 0;
   CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, B.count.p, B.offset.p, n_edges + 1, st));
@@ -248,10 +239,7 @@ extern "C" int mplx_edges_cells(mplx_ctx *c, const mplx_waypoint *parents, const
     CU(B.ids.reserve(total)); CU(B.owner.reserve(total)); CU(B.ids_sorted.reserve(total)); CU(B.owner_sorted.reserve(total));
   }
   int32_t *ids = table ? B.ids.p : nullptr, *own = table ? B.owner.p : nullptr;
-  if (dim == 2)
-    CU((mplx::launch_cells<2, true>(c->P, B.parents.p, B.actions.p, n_edges, nullptr, B.offset.p, B.cells.p, ids, own, st)));
-  else
-    CU((mplx::launch_cells<3, true>(c->P, B.parents.p, B.actions.p, n_edges, nullptr, B.offset.p, B.cells.p, ids, own, st)));
+  CU(mplx::launch_cells<true>(c->P, B.parents.p, B.actions.p, n_edges, nullptr, B.offset.p, B.cells.p, ids, own, st));
   c->launches += 1;
   CU(cudaMemcpyAsync(out_cells, B.cells.p, sizeof(int32_t) * (size_t)total * dim, cudaMemcpyDeviceToHost, st));
   if (table) {

@@ -126,6 +126,11 @@ __device__ __forceinline__ double grad_term(const EnvParams &P, const double (&v
   return P.grad_w * sqrt(n2);
 }
 
+// Whether the sample loop evaluates velocities: the yaw term and the gradient term read them.
+__host__ __device__ __forceinline__ bool need_vel(const EnvParams &P, bool yaw) {
+  return yaw || (P.pot != nullptr && P.grad_w != 0.0);
+}
+
 // traverse_primitive, literal per-primitive loop: include/mpl_planner/env/env_map.h:90-132.
 // max_v is the caller's max_i pr.max_vel(i) (the reference recomputes it at :91-94).
 template <int DIM, int ORD, bool YAW>

@@ -28,6 +28,7 @@
 //
 // Results are bit-identical to the other kernels: every decision is either proven equal to the
 // reference's (certain), independent of it (all candidates free), or made by the exact chain.
+#include "mplx_dispatch.h"
 #include "mplx_fx.cuh"
 #include "mplx_pack.cuh"
 
@@ -275,66 +276,46 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
   __syncthreads();  // B3: the queue is complete; the helper warp takes it from here
 }
 
-template <int DIM, int ORD>
-static cudaError_t launch_fx_t(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes,
-                               const mplx_succ_out &so, cudaStream_t st, int unr) {
-  const OutPtrs o{so.count, so.succ, so.cost, so.action, so.key, so.lattice};
-  const int npb = kThreads / P.nU;
-  const int grid = (n_nodes + npb - 1) / npb;
-  const bool lat = o.lattice != nullptr;
-  const bool region = P.region_bits != nullptr;
-  const int inv_nU = ((1 << 20) + P.nU - 1) / P.nU;
-#define MPLX_LAUNCH_FX_B(UNR, MINB, LAT, REGION) \
-  expand_fx_kernel<DIM, ORD, UNR, MINB, LAT, REGION><<<grid, kFxThreads, 0, st>>>(P, d_nodes, n_nodes, npb, inv_nU, o)
-#define MPLX_LAUNCH_FX(UNR, LAT, REGION) MPLX_LAUNCH_FX_B(UNR, 4, LAT, REGION)
-  static const int minb_env = [] {
-    const char *e = getenv("MPLX_FX_MINB");  // tuning: resident CTAs per SM the register budget is cut for
-    return e ? atoi(e) : 0;
-  }();
-  if (!lat && !region && (minb_env == 5 || minb_env == 6) && DIM == 3 && ORD == 2) {
-    if (minb_env == 5) { if (unr == 4) MPLX_LAUNCH_FX_B(4, 5, false, false); else MPLX_LAUNCH_FX_B(8, 5, false, false); }
-    else { if (unr == 4) MPLX_LAUNCH_FX_B(4, 6, false, false); else MPLX_LAUNCH_FX_B(8, 6, false, false); }
-    return cudaGetLastError();
-  }
-  if (unr == 4) {
-    if (region) { if (lat) MPLX_LAUNCH_FX(4, true, true); else MPLX_LAUNCH_FX(4, false, true); }
-    else { if (lat) MPLX_LAUNCH_FX(4, true, false); else MPLX_LAUNCH_FX(4, false, false); }
-  } else {
-    if (region) { if (lat) MPLX_LAUNCH_FX(8, true, true); else MPLX_LAUNCH_FX(8, false, true); }
-    else { if (lat) MPLX_LAUNCH_FX(8, true, false); else MPLX_LAUNCH_FX(8, false, false); }
-  }
-#undef MPLX_LAUNCH_FX
-#undef MPLX_LAUNCH_FX_B
-  return cudaGetLastError();
-}
-
 // Occupancy planning only (no potential map, no yaw control), |U| <= 128 (hcurr slots), stats off.
 bool fx_supported(const EnvParams &P) {
   return P.occ2 != nullptr && P.pot == nullptr && (P.control & 16) == 0 && P.nU <= kThreads && P.stats == nullptr;
 }
 
-cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes,
-                             const mplx_succ_out &o, cudaStream_t st) {
-  if (n_nodes <= 0) return cudaSuccess;
+cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const OutPtrs &o,
+                             cudaStream_t st) {
   static const int unr_env = [] {
     const char *e = getenv("MPLX_FX_UNR");  // tuning override: 4 or 8 samples per group
     return e ? atoi(e) : 0;
   }();
+  static const int minb_env = [] {
+    const char *e = getenv("MPLX_FX_MINB");  // tuning: resident CTAs per SM the register budget is cut for
+    return e ? atoi(e) : 0;
+  }();
   const int unr = unr_env == 4 || unr_env == 8 ? unr_env : (P.maxn <= 15 ? 4 : 8);
-#define MPLX_FX_ORD(DIM)                                                                  \
-  switch (P.control & 15) {                                                               \
-    case MPLX_VEL: return launch_fx_t<DIM, 1>(P, d_nodes, n_nodes, o, st, unr);      \
-    case MPLX_ACC: return launch_fx_t<DIM, 2>(P, d_nodes, n_nodes, o, st, unr);      \
-    case MPLX_JRK: return launch_fx_t<DIM, 3>(P, d_nodes, n_nodes, o, st, unr);      \
-    case MPLX_SNP: return launch_fx_t<DIM, 4>(P, d_nodes, n_nodes, o, st, unr);      \
-  }
-  if (P.dim == 2) {
-    MPLX_FX_ORD(2)
-  } else {
-    MPLX_FX_ORD(3)
-  }
-#undef MPLX_FX_ORD
-  return cudaErrorInvalidValue;
+  const int npb = kThreads / P.nU;
+  const int grid = (n_nodes + npb - 1) / npb;
+  const int inv_nU = ((1 << 20) + P.nU - 1) / P.nU;
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      return with_bool(unr == 8, [&](auto UNR8) {
+        return with_bool(o.lattice != nullptr, [&](auto LAT) {
+          return with_bool(P.region_bits != nullptr, [&](auto REGION) {
+            auto launch = [&](auto MINB) {
+              expand_fx_kernel<DIM, ORD, UNR8 ? 8 : 4, MINB, LAT, REGION>
+                  <<<grid, kFxThreads, 0, st>>>(P, d_nodes, n_nodes, npb, inv_nU, o);
+              return cudaGetLastError();
+            };
+            // MPLX_FX_MINB = 5 or 6 is for the plain 3-D ACC plan
+            if constexpr (DIM == 3 && ORD == 2 && !LAT && !REGION) {
+              if (minb_env == 5) return launch(Int<5>());
+              if (minb_env == 6) return launch(Int<6>());
+            }
+            return launch(Int<4>());
+          });
+        });
+      });
+    });
+  });
 }
 
 // {occupancy word, candidate-summary word} per 32 voxels (the summary rule: occ2_summary_word).

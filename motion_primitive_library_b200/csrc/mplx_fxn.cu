@@ -19,6 +19,7 @@
 // in global memory and re-evaluated with the exact FP64 chain by fx_resolve_kernel afterwards.
 #include <string.h>
 
+#include "mplx_dispatch.h"
 #include "mplx_fx.cuh"
 
 namespace mplx {
@@ -539,27 +540,29 @@ fx_resolve_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
   }
 }
 
-template <int DIM, int ORD>
-static cudaError_t launch_fxn_t(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &so,
-                                cudaStream_t st, FxAmbRec *amb_q, unsigned *amb_n, unsigned amb_cap) {
-  const OutPtrs o{so.count, so.succ, so.cost, so.action, so.key, so.lattice};
+// The rows must pay against Dim evaluations per control, everything must fit shared memory, and the
+// batch must be worth two launches.
+bool fxn_supported(const EnvParams &P, int n_nodes) {
+  if (!fx_supported(P) || P.n_rows <= 0 || P.nU > kThreads) return false;
+  if (P.n_rows * 2 > P.dim * P.nU) return false;
+  const int npb = kThreads / P.nU;
+  if (npb * P.n_rows > 255 || npb > kMaxNpb) return false;  // row indices are bytes; node tables of FxnShared
+  const size_t smem = (size_t)npb * P.n_rows * 128;
+  if (smem > 64 * 1024) return false;
+  return (long)n_nodes * P.nU >= 64L * kThreads;
+}
+
+cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const OutPtrs &o,
+                              cudaStream_t st, void *amb_q, unsigned *amb_n, unsigned amb_cap) {
+  FxAmbRec *q = static_cast<FxAmbRec *>(amb_q);
   const int npb = kThreads / P.nU;
   const int grid = (n_nodes + npb - 1) / npb;
   const bool lat = o.lattice != nullptr;
   const bool region = P.region_bits != nullptr;
   const int inv_nU = ((1 << 20) + P.nU - 1) / P.nU;
   const int inv_rows = ((1 << 20) + P.n_rows - 1) / P.n_rows;
-  const int rows_bytes = (int)(((size_t)npb * P.n_rows * sizeof(FxnRow<ORD>) + 15) & ~(size_t)15);
   static const int sort_env = [] { const char *v = getenv("MPLX_FXN_SORT"); return v ? atoi(v) : -1; }();  // tuning
-  const bool sort = sort_env >= 0 ? sort_env != 0 : ORD >= 3;
-  // staging of the successor records for the bulk copies (expand_fxn_kernel): destination 16-byte aligned
-  // The sorted path (JRK-125 with the CTA sort) keeps the per-lane stores: on that workload the bulk copies
-  // were measured slower.
   static const int bulk_env = [] { const char *v = getenv("MPLX_FXN_BULK"); return v ? atoi(v) : -1; }();  // tuning / A-B
-  const bool bulk = (bulk_env >= 0 ? bulk_env != 0 : !sort) && o.succ != nullptr &&
-                    (reinterpret_cast<uintptr_t>(o.succ) & 15u) == 0;
-  const int stage_off = bulk ? rows_bytes : -1;
-  const size_t smem = (size_t)rows_bytes + (bulk ? (size_t)kWarps * kStageBytes : 0);
   cudaError_t e = cudaMemsetAsync(amb_n, 0, sizeof(unsigned) * kFxSegments, st);
   if (e != cudaSuccess) return e;
   // Keep the voxel bitmaps in the L2's persisting carve-out: every CTA of every launch re-reads them while
@@ -581,75 +584,49 @@ static cudaError_t launch_fxn_t(const EnvParams &P, const mplx_waypoint *d_nodes
   const int pf_ahead = pf_env >= 0 ? pf_env : 2 * 4 * sm_count();
   static const int unr_env = [] { const char *v = getenv("MPLX_FXN_UNR"); return v ? atoi(v) : 0; }();    // tuning
   static const int minb_env = [] { const char *v = getenv("MPLX_FXN_MINB"); return v ? atoi(v) : 0; }();  // tuning
-#define MPLX_LAUNCH_FXN_S(UNR, MINB, LAT, REGION, SORT)                                                         \
-  do {                                                                                                          \
-    if (smem > 32 * 1024) { /* static + dynamic may pass the 48 KB default */                                   \
-      e = cudaFuncSetAttribute(expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT>,                       \
-                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                         \
-      if (e != cudaSuccess) return e;                                                                           \
-    }                                                                                                           \
-    if (carve >= 0) {                                                                                           \
-      e = cudaFuncSetAttribute(expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT>,                       \
-                               cudaFuncAttributePreferredSharedMemoryCarveout, carve);                          \
-      if (e != cudaSuccess) return e;                                                                           \
-    }                                                                                                           \
-    expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT><<<grid, kThreads, smem, st>>>(                    \
-        P, d_nodes, n_nodes, npb, inv_nU, inv_rows, amb_q, amb_n, amb_cap, o, pf_ahead, stage_off);                        \
-  } while (0)
-#define MPLX_LAUNCH_FXN(UNR, MINB, LAT, REGION)                     \
-  do {                                                              \
-    if (sort) MPLX_LAUNCH_FXN_S(UNR, MINB, LAT, REGION, true);      \
-    else MPLX_LAUNCH_FXN_S(UNR, MINB, LAT, REGION, false);          \
-  } while (0)
-  if (region) { if (lat) MPLX_LAUNCH_FXN(4, 4, true, true); else MPLX_LAUNCH_FXN(4, 4, false, true); }
-  else if (lat) MPLX_LAUNCH_FXN(4, 4, true, false);
-  else if (unr_env == 8 && minb_env == 3) MPLX_LAUNCH_FXN(8, 3, false, false);
-  else if (unr_env == 4 && minb_env == 3) MPLX_LAUNCH_FXN(4, 3, false, false);
-  else if (unr_env == 8) MPLX_LAUNCH_FXN(8, 4, false, false);
-  else if (minb_env == 5) MPLX_LAUNCH_FXN(4, 5, false, false);
-  else MPLX_LAUNCH_FXN(4, 4, false, false);
-#undef MPLX_LAUNCH_FXN
-#undef MPLX_LAUNCH_FXN_S
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  const int rgrid = kFxSegments * 8;
-  if (region)
-    fx_resolve_kernel<DIM, ORD, true><<<rgrid, 128, 0, st>>>(P, d_nodes, amb_q, amb_n, amb_cap, o.cost);
-  else
-    fx_resolve_kernel<DIM, ORD, false><<<rgrid, 128, 0, st>>>(P, d_nodes, amb_q, amb_n, amb_cap, o.cost);
-  return cudaGetLastError();
-}
-
-// The rows must pay against Dim evaluations per control, everything must fit shared memory, and the
-// batch must be worth two launches.
-bool fxn_supported(const EnvParams &P, int n_nodes) {
-  if (!fx_supported(P) || P.n_rows <= 0 || P.nU > kThreads) return false;
-  if (P.n_rows * 2 > P.dim * P.nU) return false;
-  const int npb = kThreads / P.nU;
-  if (npb * P.n_rows > 255 || npb > kMaxNpb) return false;  // row indices are bytes; node tables of FxnShared
-  const size_t smem = (size_t)npb * P.n_rows * 128;
-  if (smem > 64 * 1024) return false;
-  return (long)n_nodes * P.nU >= 64L * kThreads;
-}
-
-cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &o,
-                              cudaStream_t st, void *amb_q, unsigned *amb_n, unsigned amb_cap) {
-  if (n_nodes <= 0) return cudaSuccess;
-  FxAmbRec *q = static_cast<FxAmbRec *>(amb_q);
-#define MPLX_FXN_ORD(DIM)                                                                         \
-  switch (P.control & 15) {                                                                       \
-    case MPLX_VEL: return launch_fxn_t<DIM, 1>(P, d_nodes, n_nodes, o, st, q, amb_n, amb_cap);     \
-    case MPLX_ACC: return launch_fxn_t<DIM, 2>(P, d_nodes, n_nodes, o, st, q, amb_n, amb_cap);     \
-    case MPLX_JRK: return launch_fxn_t<DIM, 3>(P, d_nodes, n_nodes, o, st, q, amb_n, amb_cap);     \
-    case MPLX_SNP: return launch_fxn_t<DIM, 4>(P, d_nodes, n_nodes, o, st, q, amb_n, amb_cap);     \
-  }
-  if (P.dim == 2) {
-    MPLX_FXN_ORD(2)
-  } else {
-    MPLX_FXN_ORD(3)
-  }
-#undef MPLX_FXN_ORD
-  return cudaErrorInvalidValue;
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      const int rows_bytes = (int)(((size_t)npb * P.n_rows * sizeof(FxnRow<ORD>) + 15) & ~(size_t)15);
+      const bool sort = sort_env >= 0 ? sort_env != 0 : ORD >= 3;
+      // staging of the successor records for the bulk copies (expand_fxn_kernel): destination 16-byte aligned
+      // The sorted path (JRK-125 with the CTA sort) keeps the per-lane stores: on that workload the bulk copies
+      // were measured slower.
+      const bool bulk = (bulk_env >= 0 ? bulk_env != 0 : !sort) && o.succ != nullptr &&
+                        (reinterpret_cast<uintptr_t>(o.succ) & 15u) == 0;
+      const int stage_off = bulk ? rows_bytes : -1;
+      const size_t smem = (size_t)rows_bytes + (bulk ? (size_t)kWarps * kStageBytes : 0);
+      auto launch = [&](auto UNR, auto MINB, auto LAT, auto REGION) {
+        return with_bool(sort, [&](auto SORT) {
+          const auto kernel = expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT>;
+          if (smem > 32 * 1024) {  // static + dynamic may pass the 48 KB default
+            const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (r != cudaSuccess) return r;
+          }
+          if (carve >= 0) {
+            const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
+            if (r != cudaSuccess) return r;
+          }
+          kernel<<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, inv_nU, inv_rows, q, amb_n, amb_cap, o,
+                                                pf_ahead, stage_off);
+          return cudaGetLastError();
+        });
+      };
+      const std::true_type yes{};
+      const std::false_type no{};
+      if (region) e = with_bool(lat, [&](auto LAT) { return launch(Int<4>(), Int<4>(), LAT, yes); });
+      else if (lat) e = launch(Int<4>(), Int<4>(), yes, no);
+      else if (unr_env == 8 && minb_env == 3) e = launch(Int<8>(), Int<3>(), no, no);
+      else if (unr_env == 4 && minb_env == 3) e = launch(Int<4>(), Int<3>(), no, no);
+      else if (unr_env == 8) e = launch(Int<8>(), Int<4>(), no, no);
+      else if (minb_env == 5) e = launch(Int<4>(), Int<5>(), no, no);
+      else e = launch(Int<4>(), Int<4>(), no, no);
+      if (e != cudaSuccess) return e;
+      return with_bool(region, [&](auto REGION) {
+        fx_resolve_kernel<DIM, ORD, REGION><<<kFxSegments * 8, 128, 0, st>>>(P, d_nodes, q, amb_n, amb_cap, o.cost);
+        return cudaGetLastError();
+      });
+    });
+  });
 }
 
 size_t fx_amb_record_bytes() { return sizeof(FxAmbRec); }

@@ -197,7 +197,7 @@ struct mplx_ctx {
   size_t occ2_window = 0;  // bytes of occ2 covered by the L2 access-policy window (0 = none)  // {occupancy, candidate summary} words of the fixed-point kernel
   DevBuf<double> U, ttab, tdt;
   DevBuf<int> tcount;
-  int force_seq = 0;
+  int kernel = 0;  // mplx_set_kernel
   DevBuf<unsigned long long> stats;
   bool has_map = false, has_pot = false, has_region = false, has_params = false, stats_on = false;
   size_t nvox = 0;

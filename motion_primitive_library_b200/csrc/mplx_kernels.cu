@@ -26,6 +26,7 @@
 
 #include "../../include/mplx.h"
 #include "mplx_device.cuh"
+#include "mplx_dispatch.h"
 #include "mplx_expand.cuh"
 #include "mplx_pack.cuh"
 
@@ -36,7 +37,7 @@ template <int DIM, int ORD, bool YAW>
 __global__ void __launch_bounds__(kThreads)
 expand_seq_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__restrict__ nodes, int n_nodes,
                   int npb, const __grid_constant__ OutPtrs o) {
-  const bool need_vel = YAW || (P.pot != nullptr && P.grad_w != 0.0);
+  const bool vel = need_vel(P, YAW);
   __shared__ uint32_t vbits[kMaxU / 32 + 9];
   __shared__ unsigned long long s_stats[2];
   const int nU = P.nU;
@@ -54,8 +55,8 @@ expand_seq_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
     unsigned n_samples = 0;
     if (emit) {
       double cf[CoefLayout<DIM, ORD, YAW>::NCMAX];
-      fill_coef<DIM, ORD, YAW>(pr, need_vel, cf);
-      double cost = same ? 0.0 : traverse_loop<DIM, ORD, YAW>(P, cf, need_vel, max_v, n_samples);
+      fill_coef<DIM, ORD, YAW>(pr, vel, cf);
+      double cost = same ? 0.0 : traverse_loop<DIM, ORD, YAW>(P, cf, vel, max_v, n_samples);
       if (!isinf(cost)) cost += intrinsic_cost<DIM, ORD, YAW>(P, pr);
       if (o.cost) o.cost[slot] = cost;
     }
@@ -272,81 +273,72 @@ expand_flat_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__r
 }
 
 template <int DIM, int ORD, bool YAW>
-static cudaError_t launch_t(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes,
-                            const mplx_succ_out &so, cudaStream_t st, int force_seq) {
-  const OutPtrs o{so.count, so.succ, so.cost, so.action, so.key, so.lattice};
+static cudaError_t launch_t(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const OutPtrs &o,
+                            cudaStream_t st, int kernel) {
   const int npb = P.nU >= kThreads ? 1 : kThreads / P.nU;
   const int grid = (n_nodes + npb - 1) / npb;
-  if (P.nU > kThreads || force_seq == 1) {
+  if (P.nU > kThreads || kernel == 1) {
     expand_seq_kernel<DIM, ORD, YAW><<<grid, kThreads, 0, st>>>(P, d_nodes, n_nodes, npb, o);
     return cudaGetLastError();
   }
-  const bool nv = YAW || (P.pot != nullptr && P.grad_w != 0.0);
-  if (force_seq != 3) {  // register kernel (default)
-    // samples in flight per lane: 4, or 2 when every primitive of the plan has a short loop
-    // (n <= 15: a group of 4 would mostly run past the end of the loop)
-    const bool short_loops = P.maxn <= 15;
-    const bool lat = o.lattice != nullptr;
+  const bool vel = need_vel(P, YAW);
+  if (kernel != 3) {  // register kernel (default)
     // groups of 8 samples for plain long-loop planning (measured 0.810 vs 0.828 ms on 512^3 ACC-27, no
     // change on 256^3); MPLX_UNR4=1 restores groups of 4
     static const bool unr8 = getenv("MPLX_UNR4") == nullptr;
-#define MPLX_LAUNCH_REG(VEL, UNR, LAT) \
-  expand_reg_kernel<DIM, ORD, YAW, VEL, UNR, 4, LAT><<<grid, kThreads, 0, st>>>(P, d_nodes, n_nodes, npb, o)
-    if (nv) {
-      if (short_loops) { if (lat) MPLX_LAUNCH_REG(true, 2, true); else MPLX_LAUNCH_REG(true, 2, false); }
-      else { if (lat) MPLX_LAUNCH_REG(true, 4, true); else MPLX_LAUNCH_REG(true, 4, false); }
-    } else {
-      if (short_loops) { if (lat) MPLX_LAUNCH_REG(YAW, 2, true); else MPLX_LAUNCH_REG(YAW, 2, false); }
-      else { if (lat) MPLX_LAUNCH_REG(YAW, 4, true); else if (unr8) MPLX_LAUNCH_REG(YAW, 8, false); else MPLX_LAUNCH_REG(YAW, 4, false); }
-    }
-#undef MPLX_LAUNCH_REG
-    return cudaGetLastError();
+    return with_bool(vel, [&](auto V) {
+      constexpr bool VEL = YAW || V;  // vel is always true with yaw: no VEL = false instantiation for it
+      return with_bool(o.lattice != nullptr, [&](auto LAT) {
+        auto launch = [&](auto UNR) {
+          expand_reg_kernel<DIM, ORD, YAW, VEL, UNR, 4, LAT><<<grid, kThreads, 0, st>>>(P, d_nodes, n_nodes, npb, o);
+          return cudaGetLastError();
+        };
+        // samples in flight per lane: 4, or 2 when every primitive of the plan has a short loop
+        // (n <= 15: a group of 4 would mostly run past the end of the loop)
+        if (P.maxn <= 15) return launch(Int<2>());
+        if constexpr (!VEL && !LAT) {
+          if (unr8) return launch(Int<8>());
+        }
+        return launch(Int<4>());
+      });
+    });
   }
   using L = FlatLayout<DIM, ORD, YAW>;
-  const bool need_vel = YAW || (P.pot != nullptr && P.grad_w != 0.0);
   const int maxns = P.maxn + 1;
-  const size_t smem = kWarps * L::warp_bytes(need_vel, maxns);
+  const size_t smem = kWarps * L::warp_bytes(vel, maxns);
+  const auto flat = expand_flat_kernel<DIM, ORD, YAW>;
   if (smem > 48 * 1024) {  // the attribute is per device: set it on every such launch (a host-side call)
-    cudaError_t e = cudaFuncSetAttribute(expand_flat_kernel<DIM, ORD, YAW>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(flat, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
   }
-  expand_flat_kernel<DIM, ORD, YAW><<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, o, maxns,
-                                                                   need_vel ? 1 : 0);
+  flat<<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, o, maxns, vel ? 1 : 0);
   return cudaGetLastError();
 }
 
-template <int DIM>
-static cudaError_t launch_d(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes,
-                            const mplx_succ_out &o, cudaStream_t st, int fs) {
-  const bool yaw = (P.control & 16) != 0;
-  switch (P.control & 15) {
-    case MPLX_VEL: return yaw ? launch_t<DIM, 1, true>(P, d_nodes, n_nodes, o, st, fs) : launch_t<DIM, 1, false>(P, d_nodes, n_nodes, o, st, fs);
-    case MPLX_ACC: return yaw ? launch_t<DIM, 2, true>(P, d_nodes, n_nodes, o, st, fs) : launch_t<DIM, 2, false>(P, d_nodes, n_nodes, o, st, fs);
-    case MPLX_JRK: return yaw ? launch_t<DIM, 3, true>(P, d_nodes, n_nodes, o, st, fs) : launch_t<DIM, 3, false>(P, d_nodes, n_nodes, o, st, fs);
-    case MPLX_SNP: return yaw ? launch_t<DIM, 4, true>(P, d_nodes, n_nodes, o, st, fs) : launch_t<DIM, 4, false>(P, d_nodes, n_nodes, o, st, fs);
-  }
-  return cudaErrorInvalidValue;
-}
-
-cudaError_t launch_expand(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes,
-                          const mplx_succ_out &o, cudaStream_t st, int force_seq, const FxScratch *fs) {
+cudaError_t launch_expand(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const mplx_succ_out &so,
+                          cudaStream_t st, int kernel, const FxScratch *fs, int *launches) {
+  *launches = 0;
   if (n_nodes <= 0) return cudaSuccess;
-  // large occupancy-planning batches: node-cooperative rows + flat sample items (mplx_fxn.cu)
+  const OutPtrs o{so.count, so.succ, so.cost, so.action, so.key, so.lattice};
+  // large occupancy-planning batches: node-cooperative rows + flat sample items, then the re-evaluation of
+  // the ambiguous primitives (mplx_fxn.cu)
   static const bool fxn_off = getenv("MPLX_FX_NOROWS") != nullptr;
-  if (force_seq == 0 && !fxn_off && fs && fs->q && fxn_supported(P, n_nodes))
+  if (kernel == 0 && !fxn_off && fs && fs->q && fxn_supported(P, n_nodes)) {
+    *launches = 2;
     return launch_expand_fxn(P, d_nodes, n_nodes, o, st, fs->q, fs->n, fs->cap);
+  }
+  *launches = 1;
   // auto (0): the dealing kernel where lanes of the register kernel idle most — controls whose
   // dynamic limits reject many primitives (JRK/SNP) and sample loops with per-sample work beyond the
   // voxel bit (potential field, yaw) — once the batch is large enough for multi-round CTAs; the register kernel otherwise
   // (measured: 512^3 JRK-125 +21 %, ACCxYAW-81 with potential +35 %, plain ACC-27 -3 %).
   // occupancy planning (no potential field, no yaw): the fixed-point kernel (mplx_fx.cu)
-  if ((force_seq == 0 || force_seq == 5) && fx_supported(P)) return launch_expand_fx(P, d_nodes, n_nodes, o, st);
-  if (force_seq == 5) force_seq = 0;  // not applicable to this plan: the auto rule below
+  if ((kernel == 0 || kernel == 5) && fx_supported(P)) return launch_expand_fx(P, d_nodes, n_nodes, o, st);
+  if (kernel == 5) kernel = 0;  // not applicable to this plan: the auto rule below
   const bool heavy = (P.control & 15) >= MPLX_JRK || (P.control & 16) != 0 || P.pot != nullptr;
   // (at one round per CTA the dealing kernel only adds overhead: 4096-node JRK launches of the lock-step
   // multi-query driver run 0.37 ms faster on the register kernel, so auto needs >= 2 rounds' worth of CTAs)
-  const bool deal = force_seq == 4 || (force_seq == 0 && heavy && (long)n_nodes * P.nU >= 2L * 256 * sm_count() * 4 * 8);
+  const bool deal = kernel == 4 || (kernel == 0 && heavy && (long)n_nodes * P.nU >= 2L * 256 * sm_count() * 4 * 8);
   if (deal && P.nU <= kThreads) {
     static const int rounds_env = [] {
       const char *e = getenv("MPLX_DEAL_ROUNDS");  // tuning override
@@ -354,8 +346,11 @@ cudaError_t launch_expand(const EnvParams &P, const mplx_waypoint *d_nodes, int 
     }();
     return launch_expand_deal(P, d_nodes, n_nodes, o, st, rounds_env);
   }
-  return P.dim == 2 ? launch_d<2>(P, d_nodes, n_nodes, o, st, force_seq)
-                    : launch_d<3>(P, d_nodes, n_nodes, o, st, force_seq);
+  return with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      return with_bool(P.control & 16, [&](auto YAW) { return launch_t<DIM, ORD, YAW>(P, d_nodes, n_nodes, o, st, kernel); });
+    });
+  });
 }
 
 int sm_count() {

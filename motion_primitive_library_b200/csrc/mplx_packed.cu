@@ -169,14 +169,15 @@ extern "C" int mplx_expand_packed(mplx_ctx *c, const mplx_waypoint *nodes, int n
     CU(cudaMemcpyAsync(B.nodes.p, nodes + off, sizeof(mplx_waypoint) * m, cudaMemcpyHostToDevice, st));
     mplx_succ_out d{B.count.p, out->state ? B.succ.p : nullptr, B.cost.p, B.action.p, B.key.p, nullptr};
     CU(B.fxq.reserve((size_t)m * nU));
-    CU(mplx::launch_expand(c->P, B.nodes.p, m, d, st, c->force_seq, &B.fxq.view));
+    int launches = 0;
+    CU(mplx::launch_expand(c->P, B.nodes.p, m, d, st, c->kernel, &B.fxq.view, &launches));
     CU(cudaMemsetAsync(B.total.p, 0, sizeof(long long), st));
     mplx::pack_kernel<<<(m + 7) / 8, 256, 0, st>>>(m, nU, dim, control, drop_inf, B.count.p,
                                                    out->state ? B.succ.p : nullptr, B.cost.p, B.action.p, B.key.p, B.total.p, B.kcount.p, B.offset.p,
                                                    out->state ? B.pstate.p : nullptr, out->cost ? B.pcost.p : nullptr,
                                                    out->action ? B.paction.p : nullptr, out->key ? B.pkey.p : nullptr);
     CU(cudaGetLastError());
-    c->launches += 2;
+    c->launches += launches + 1;
     CU(cudaMemcpyAsync(B.h_total.p, B.total.p, sizeof(long long), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(B.ready, st));
     if (k >= ahead)

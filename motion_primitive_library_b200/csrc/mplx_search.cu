@@ -16,6 +16,7 @@
 #include <chrono>
 #include <vector>
 
+#include "mplx_dispatch.h"
 #include "mplx_expand.cuh"
 #include "mplx_fx.cuh"
 #include "mplx_internal.h"
@@ -145,34 +146,18 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
   }
 }
 
-template <int DIM>
-cudaError_t launch_dim(const EnvParams &P, const Job &J, int grid, int block, cudaStream_t st) {
-  switch (P.control & 15) {
-    case MPLX_VEL: search_kernel<DIM, 1><<<grid, block, 0, st>>>(P, J); break;
-    case MPLX_ACC: search_kernel<DIM, 2><<<grid, block, 0, st>>>(P, J); break;
-    case MPLX_JRK: search_kernel<DIM, 3><<<grid, block, 0, st>>>(P, J); break;
-    case MPLX_SNP: search_kernel<DIM, 4><<<grid, block, 0, st>>>(P, J); break;
-    default: return cudaErrorInvalidValue;
-  }
-  return cudaGetLastError();
-}
-
-template <int DIM, int ORD>
-int max_resident(int block) {
+int resident_ctas(const EnvParams &P, int block) {
   int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, search_kernel<DIM, ORD>, block, 0) != cudaSuccess) {
+  const cudaError_t e = with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, search_kernel<DIM, ORD>, block, 0);
+    });
+  });
+  if (e != cudaSuccess) {
     cudaGetLastError();
     per_sm = 1;
   }
   return std::max(1, per_sm) * sm_count();
-}
-int resident_ctas(const EnvParams &P, int block) {
-  const int o = P.control & 15;
-  if (P.dim == 2)
-    return o == MPLX_VEL ? max_resident<2, 1>(block) : o == MPLX_ACC ? max_resident<2, 2>(block)
-         : o == MPLX_JRK ? max_resident<2, 3>(block) : max_resident<2, 4>(block);
-  return o == MPLX_VEL ? max_resident<3, 1>(block) : o == MPLX_ACC ? max_resident<3, 2>(block)
-       : o == MPLX_JRK ? max_resident<3, 3>(block) : max_resident<3, 4>(block);
 }
 
 }  // namespace
@@ -330,8 +315,12 @@ extern "C" int mplx_plan_batch(mplx_ctx *c, const mplx_waypoint *starts, const m
   CU(cudaEventCreate(&e0));
   CU(cudaEventCreate(&e1));
   cudaEventRecord(e0, c->stream);
-  cudaError_t le = c->dim == 2 ? launch_dim<2>(P, J, (int)slots, block, c->stream)
-                               : launch_dim<3>(P, J, (int)slots, block, c->stream);
+  cudaError_t le = with_dim(P.dim, [&](auto DIM) {
+    return with_order(P.control, [&](auto ORD) {
+      search_kernel<DIM, ORD><<<(int)slots, block, 0, c->stream>>>(P, J);
+      return cudaGetLastError();
+    });
+  });
   cudaEventRecord(e1, c->stream);
   if (le != cudaSuccess) {
     cudaEventDestroy(e0);

@@ -38,7 +38,7 @@ WIDTHS = (1, 2, 31, 32, 33, 64, 65, 243, 255, 256)
 
 # ---- restatements of the launcher and the sizing rules ------------------------------------------------
 def search_instantiation(dim, control):
-    """launch_dim<DIM> (csrc/mplx_search.cu): the search_kernel<DIM, ORD> a plan runs, from control & 15."""
+    """mplx_plan_batch (csrc/mplx_search.cu): the search_kernel<DIM, ORD> a plan runs, from control & 15."""
     order = ORDER.get(control & 15)
     if order is None:
         raise ValueError(f"control {control:#x} has no search kernel")
