@@ -14,6 +14,7 @@
 
 #include "../../include/mplx.h"
 #include "mplx_internal.h"
+#include "mplx_pack.cuh"
 
 namespace mplx {
 thread_local char g_err[512] = "";
@@ -141,12 +142,14 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
   CU(cudaMemcpyAsync(c->map.p, data, nvox, cudaMemcpyHostToDevice, c->stream));
   CU(c->occ.reserve((nvox + 31) / 32));
   CU(mplx::launch_pack_bits(c->map.p, nvox, c->occ.p, true, c->stream));
-  CU(c->occ2.reserve((nvox + 31) / 32));
-  CU(mplx::launch_pack_occ2(c->occ.p, nvox, c->dim, dim[0], dim[1], c->occ2.p, c->stream));
+  const int nz = c->dim == 3 ? dim[2] : 1;
+  const size_t npairs = mplx::occ2_pair_count(c->dim, dim[0], dim[1], nz);
+  CU(c->occ2.reserve(npairs));
+  CU(mplx::launch_pack_occ2(c->occ.p, nvox, c->dim, dim[0], dim[1], nz, c->occ2.p, c->stream));
   c->launches += 2;
   {
-    // L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_fxn_t
-    const size_t bytes = ((nvox + 31) / 32) * sizeof(uint2);
+    // L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_expand_fxn
+    const size_t bytes = npairs * sizeof(uint2);
     int maxp = 0, maxw = 0;
     cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
     cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
@@ -166,6 +169,8 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
     c->P.origin[k] = k < c->dim ? origin[k] : 0.0;
     c->P.dimd[k] = (double)c->P.mdim[k];
   }
+  c->P.occ2_nb[0] = mplx::occ2_bricks_x(c->dim, dim[0]);
+  c->P.occ2_nb[1] = mplx::occ2_bricks_y(c->dim, dim[1]);
   c->P.res = res;
   c->P.rinv = 1.0 / res;
   c->has_map = true;

@@ -35,9 +35,11 @@ struct EnvParams {
   const int *tcount;           // [kNMax+1]
   const double *tdt;           // [kNMax+1]  T/n (env_map.h:98)
   int maxn;                    // largest n the flat sample phase accepts (<= kNMax)
-  // {occupancy word, candidate-summary word} per 32 voxels for the fixed-point kernel (mplx_fx.cu)
+  // {occupancy word, candidate-summary word} pairs of the fixed-point kernels (mplx_fx.cu), in bricks
+  // (layout: mplx_pack.cuh)
   const uint2 *occ2;
   size_t occ2_bytes;  // size of occ2 when an L2 persisting carve-out was granted for it, else 0
+  int occ2_nb[2];     // bricks of occ2 along x and y (occ2_bricks_x, occ2_bricks_y)
   // Per-axis value tables of U for the node-cooperative kernel (mplx_fx.cu): the distinct values of
   // U[.][a] (bitwise) of all axes listed one after the other as "rows"; U[i][a] == row_u[prow[3*i+a]].
   const unsigned char *prow;      // [nU*3]

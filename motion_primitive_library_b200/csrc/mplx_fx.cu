@@ -318,21 +318,24 @@ cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, i
   });
 }
 
-// {occupancy word, candidate-summary word} per 32 voxels (the summary rule: occ2_summary_word).
-__global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, int dim, int nx, int ny,
+// The {occupancy word, candidate-summary word} pairs in bricks (layout and bits: occ2_brick_pair).
+__global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, int dim, int nx, int ny, int nz,
                                  uint2 *__restrict__ out) {
-  const size_t nwords = (nvox + 31) >> 5;
-  for (size_t wd = (size_t)blockIdx.x * blockDim.x + threadIdx.x; wd < nwords;
-       wd += (size_t)gridDim.x * blockDim.x)
-    out[wd] = make_uint2(occ[wd], occ2_summary_word(occ, wd, nvox, dim, nx, ny));
+  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < npairs; p += (size_t)gridDim.x * blockDim.x) {
+    uint32_t o, s;
+    occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
+    out[p] = make_uint2(o, s);
+  }
 }
 
-cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, uint2 *d_out, cudaStream_t st) {
-  const size_t nwords = (nvox + 31) >> 5;
-  int grid = (int)((nwords + 255) / 256);
+cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint2 *d_out,
+                             cudaStream_t st) {
+  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
+  int grid = (int)((npairs + 255) / 256);
   if (grid > sm_count() * 16) grid = sm_count() * 16;
   if (grid < 1) grid = 1;
-  pack_occ2_kernel<<<grid, 256, 0, st>>>(d_occ, nvox, dim, nx, ny, d_out);
+  pack_occ2_kernel<<<grid, 256, 0, st>>>(d_occ, nvox, dim, nx, ny, nz, d_out);
   return cudaGetLastError();
 }
 

@@ -208,7 +208,7 @@ extern "C" int mplx_update_potential_map(mplx_ctx *c, const double *radius, doub
   // map_util_->setMap(.., dmap, ..) and ENV_->set_potential_map(dmap): map_planner.cpp:387-388
   if (e == cudaSuccess) e = cudaMemcpyAsync(c->map.p, c->pot.p, nvox, cudaMemcpyDeviceToDevice, st);
   if (e == cudaSuccess) e = launch_pack_bits(c->map.p, nvox, c->occ.p, true, st);
-  if (e == cudaSuccess) e = launch_pack_occ2(c->occ.p, nvox, c->dim, nx, ny, c->occ2.p, st);
+  if (e == cudaSuccess) e = launch_pack_occ2(c->occ.p, nvox, c->dim, nx, ny, nz, c->occ2.p, st);
   if (e == cudaSuccess && out_map) e = cudaMemcpyAsync(out_map, c->pot.p, nvox, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   src.release();

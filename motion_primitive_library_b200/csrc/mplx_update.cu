@@ -7,11 +7,12 @@
 //      finds them already in order), so the last write of a voxel ends its run of equal indices;
 //   2. scatter: the last entry of each run writes its byte into the grid;
 //   3. every occupancy word holding an edited voxel is re-packed from its 32 bytes (pack_word);
-//   4. every occ2 pair whose summary can read such a word is recomputed (occ2_summary_word).
-// Steps 3 and 4 run one thread per distinct word (the first entry of each word in sorted order) and
-// use the rules of the full packs on the final grid and occupancy, so the result is bit-identical to
-// mplx_set_map of the edited grid.  Step 4 may recompute a pair none of whose summary bits changed
-// (a neighbour across a row or plane end); recomputing it rewrites the value it already has.
+//   4. every occ2 brick pair holding a voxel whose summary an edited voxel reaches is recomputed
+//      (occ2_brick_pair, from the occupancy words of step 3 and occ2_summary_word).
+// Step 3 runs one thread per distinct word (the first entry of each word in sorted order), step 4 one
+// thread per edited voxel that reaches a pair its predecessor does not.  Both use the rules of the full
+// packs on the final grid and occupancy, so the result is bit-identical to mplx_set_map of the edited
+// grid.  Two threads may recompute the same pair; they write the same value.
 #include <cub/device/device_radix_sort.cuh>
 #include <cuda_runtime.h>
 #include <string.h>
@@ -39,20 +40,61 @@ __global__ void repack_occ_kernel(const uint32_t *__restrict__ idx, int n, const
     if (first_of_word(idx, k)) occ[idx[k] >> 5] = pack_word<true>(map, idx[k] >> 5, nvox);
 }
 
-// step 4: the summary of voxel j reads the occupancy of j - {0,1} - {0,nx} (- {0,nx*ny}), so a change in
-// word w reaches the voxels 32w + [0, 32] + dy*nx (+ dz*nx*ny): two words per (dy, dz).
+// step 4: the summary of voxel (x,y,z) reads the occupancy of {x-1,x} x {y-1,y} (x {z-1,z}), so an edit of
+// voxel v reaches the summaries of v + {0,1}^dim: the pairs of those cells are recomputed.  A voxel whose
+// predecessor in the sorted list is the voxel before it in x within the same brick row (not at either end
+// of the row) reaches no pair the predecessor does not, and is skipped; duplicates are skipped too.
 __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, const uint32_t *__restrict__ occ, size_t nvox,
-                                   int dim, int nx, int ny, uint2 *__restrict__ occ2) {
-  const size_t nwords = (nvox + 31) >> 5, sxy = (size_t)nx * ny;
+                                   int dim, int nx, int ny, int nz, uint2 *__restrict__ occ2) {
+  const size_t sxy = (size_t)nx * ny;
+  const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
+  const int xmask = dim == 3 ? 7 : 31;  // x extent of a brick row - 1
   for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    if (!first_of_word(idx, k)) continue;
-    const size_t w = idx[k] >> 5;
+    const uint32_t v = idx[k];
+    const int x = (int)(v % nx), y = (int)(v / nx % ny), z = (int)(v / sxy);
+    if (k > 0 && (idx[k - 1] == v || (idx[k - 1] == v - 1 && (x & xmask) != 0 && (x & xmask) != xmask))) continue;
+    unsigned done[8];
+    int nd = 0;
     for (int dz = 0; dz <= (dim == 3 ? 1 : 0); dz++)
-      for (int dy = 0; dy <= 1; dy++) {
-        const size_t w0 = w + ((dy * (size_t)nx + dz * sxy) >> 5);
-        for (size_t t = w0; t <= w0 + 1 && t < nwords; t++)
-          occ2[t] = make_uint2(occ[t], occ2_summary_word(occ, t, nvox, dim, nx, ny));
+      for (int dy = 0; dy <= 1; dy++)
+        for (int dx = 0; dx <= 1; dx++) {
+          if (x + dx >= nx || y + dy >= ny || z + dz >= nz) continue;
+          const unsigned p = dim == 3 ? occ2_pair<3>(x + dx, y + dy, z + dz, nbx, nby)
+                                      : occ2_pair<2>(x + dx, y + dy, 0, nbx, nby);
+          bool seen = false;
+          for (int i = 0; i < nd; i++) seen = seen || done[i] == p;
+          if (seen) continue;
+          done[nd++] = p;
+          uint32_t o, s;
+          occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
+          occ2[p] = make_uint2(o, s);
+        }
+  }
+}
+
+// The pairs in voxel order, as mplx_read_map returns them: pair w holds the occupancy word w and the summary
+// bits of voxels 32w..32w+31, gathered from the bricks; bits at i >= nvox read as they did in voxel order
+// (occupancy 0, summary 1).
+__global__ void unbrick_occ2_kernel(const uint2 *__restrict__ occ2, size_t nvox, int dim, int nx, int ny,
+                                    uint2 *__restrict__ out) {
+  const size_t nwords = (nvox + 31) >> 5, sxy = (size_t)nx * ny;
+  const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
+  for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < nwords; w += (size_t)gridDim.x * blockDim.x) {
+    uint32_t o = 0, s = 0;
+    for (int b = 0; b < 32; b++) {
+      const size_t i = (w << 5) + b;
+      if (i >= nvox) {
+        s |= 1u << b;
+        continue;
       }
+      const int x = (int)(i % nx), y = (int)(i / nx % ny), z = (int)(i / sxy);
+      const unsigned p = dim == 3 ? occ2_pair<3>(x, y, z, nbx, nby) : occ2_pair<2>(x, y, 0, nbx, nby);
+      const unsigned bit = dim == 3 ? occ2_bit<3>(x, y) : occ2_bit<2>(x, y);
+      const uint2 q = occ2[p];
+      o |= ((q.x >> bit) & 1u) << b;
+      s |= ((q.y >> bit) & 1u) << b;
+    }
+    out[w] = make_uint2(o, s);
   }
 }
 
@@ -105,10 +147,10 @@ extern "C" int mplx_update_cells(mplx_ctx *c, const int32_t *idx, const int8_t *
     d_val = B.val_sorted.p;
   }
   const int grid = grid_for_entries(n);
-  const int nx = c->P.mdim[0], ny = c->P.mdim[1];
+  const int nx = c->P.mdim[0], ny = c->P.mdim[1], nz = c->dim == 3 ? c->P.mdim[2] : 1;
   scatter_last_kernel<<<grid, 256, 0, st>>>(d_idx, d_val, n, c->map.p);
   repack_occ_kernel<<<grid, 256, 0, st>>>(d_idx, n, c->map.p, c->nvox, c->occ.p);
-  repack_occ2_kernel<<<grid, 256, 0, st>>>(d_idx, n, c->occ.p, c->nvox, c->dim, nx, ny, c->occ2.p);
+  repack_occ2_kernel<<<grid, 256, 0, st>>>(d_idx, n, c->occ.p, c->nvox, c->dim, nx, ny, nz, c->occ2.p);
   CU(cudaGetLastError());
   c->launches += 3;
   CU(cudaStreamSynchronize(st));
@@ -122,7 +164,16 @@ extern "C" int mplx_read_map(mplx_ctx *c, int8_t *grid, uint32_t *occ, uint32_t 
   cudaStream_t st = c->stream;
   if (grid) CU(cudaMemcpyAsync(grid, c->map.p, c->nvox, cudaMemcpyDeviceToHost, st));
   if (occ) CU(cudaMemcpyAsync(occ, c->occ.p, nwords * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  if (occ2) CU(cudaMemcpyAsync(occ2, c->occ2.p, nwords * sizeof(uint2), cudaMemcpyDeviceToHost, st));
+  if (occ2) {
+    ScopedDevBuf<uint2> tmp;
+    CU(tmp.reserve(nwords));
+    const int grid = grid_for_entries(nwords < (1u << 30) ? (int)nwords : 1 << 30);
+    unbrick_occ2_kernel<<<grid, 256, 0, st>>>(c->occ2.p, c->nvox, c->dim, c->P.mdim[0], c->P.mdim[1], tmp.p);
+    CU(cudaGetLastError());
+    c->launches += 1;
+    CU(cudaMemcpyAsync(occ2, tmp.p, nwords * sizeof(uint2), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));  // before tmp is freed
+  }
   CU(cudaStreamSynchronize(st));
   return MPLX_OK;
 }
