@@ -219,7 +219,7 @@ int mplx_edges_cells(mplx_ctx *ctx, const mplx_waypoint *parents, const int32_t 
                      int64_t *out_offset, int32_t *out_cells, int64_t capacity, int64_t *out_total,
                      int32_t *out_table_voxel, int32_t *out_table_edge);
 
-/* ---- batched A* on the device (occupancy planning) ----------------------------------------- */
+/* ---- batched A* on the device ---------------------------------------------------------------- */
 
 /* Results of mplx_plan_batch (HOST arrays).  Query q's trajectory is actions[action_offset[q],
  * action_offset[q+1]) (action ids from start to goal; recoverTraj, graph_search.h:369-455); its closed
@@ -246,11 +246,12 @@ typedef struct {
  * what the host planner (MPL::AstarStepper with env_map's goal test and heuristic) gives, bit for bit.
  * The goal test is env_map::is_goal with tolerances tol_pos / tol_vel / tol_acc / tol_yaw (< 0 = off).
  * start_free[q] != 0 says the start is free (planner_base.h:283-287); NULL = is_free(start.pos) on the
- * device grid.  Occupancy planning only: the call fails with MPLX_ERR_ARG, and does nothing, when a
- * potential map is installed, the control carries yaw, max_expand <= 0, nU > 256, or the map or the
- * parameters are missing, and with MPLX_ERR_ALLOC, also doing nothing, when one worst-case arena does not fit the
- * budget (mplx_plan_batch_fits).  Every query slot owns an arena for the worst case (1 + max_expand*nU
- * states), so no query can overflow; the arenas stay in the ctx for the next call.  Synchronous. */
+ * device grid.  Occupancy planning only (mplx_plan_batch_cost_terms serves the rest): the call fails
+ * with MPLX_ERR_ARG, and does nothing, when a potential map is installed, the control carries yaw,
+ * max_expand <= 0, nU > 256, or the map or the parameters are missing, and with MPLX_ERR_ALLOC, also
+ * doing nothing, when one worst-case arena does not fit the budget (mplx_plan_batch_fits).  Every query
+ * slot owns an arena for the worst case (1 + max_expand*nU states), so no query can overflow; the arenas
+ * stay in the ctx for the next call.  Synchronous. */
 int mplx_plan_batch(mplx_ctx *ctx, const mplx_waypoint *starts, const mplx_waypoint *goals, const uint8_t *start_free,
                     int n_q, double eps, int max_expand, double tol_pos, double tol_vel, double tol_acc,
                     double tol_yaw, mplx_batch_out *out);
@@ -262,6 +263,26 @@ int mplx_plan_batch(mplx_ctx *ctx, const mplx_waypoint *starts, const mplx_waypo
  * mplx_plan_batch refuses.  Allocates and changes nothing.  slots / arena_bytes may be NULL. */
 int mplx_plan_batch_fits(mplx_ctx *ctx, int n_q, int max_expand, int with_closed, int32_t *slots,
                          int64_t *arena_bytes);
+
+/* mplx_plan_batch for every plan the ctx can hold: besides occupancy planning, potential-field planning
+ * (mplx_set_potential or mplx_update_potential_map, with or without a gradient weight), yaw controls
+ * (with wyaw and yaw_max) and search regions.  The sample loop sums the potential, gradient and
+ * yaw-alignment terms per sample in the reference's loop order, so each query again gives what the host
+ * planner gives, cost bit for bit.  The goal test and the start-is-free test read the ctx's grid, as the
+ * host planner reads its map: after mplx_update_potential_map that grid is the field, after
+ * mplx_set_potential it stays the occupancy map.  Same arguments, outputs, memory budget and refusals as
+ * mplx_plan_batch, except that a potential map or a yaw control is not refused: MPLX_ERR_ARG when
+ * max_expand <= 0, nU > 256, or the map or the parameters are missing, MPLX_ERR_ALLOC when one worst-case
+ * arena does not fit; either leaves outputs and ctx untouched.  Occupancy plans give the same results as
+ * through mplx_plan_batch, whose kernel skips the cost-term code.  Synchronous. */
+int mplx_plan_batch_cost_terms(mplx_ctx *ctx, const mplx_waypoint *starts, const mplx_waypoint *goals,
+                               const uint8_t *start_free, int n_q, double eps, int max_expand, double tol_pos,
+                               double tol_vel, double tol_acc, double tol_yaw, mplx_batch_out *out);
+
+/* mplx_plan_batch_fits for mplx_plan_batch_cost_terms: the slots and bytes per slot that call would use,
+ * MPLX_ERR_ALLOC / MPLX_ERR_ARG as it would refuse.  Allocates and changes nothing. */
+int mplx_plan_batch_cost_terms_fits(mplx_ctx *ctx, int n_q, int max_expand, int with_closed, int32_t *slots,
+                                    int64_t *arena_bytes);
 
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field

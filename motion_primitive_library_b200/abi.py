@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = (
     "mplx_edges_cells",
     "mplx_plan_batch",
     "mplx_plan_batch_fits",
+    "mplx_plan_batch_cost_terms",
+    "mplx_plan_batch_cost_terms_fits",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -172,6 +174,10 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch.restype = i32
     lib.mplx_plan_batch_fits.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
     lib.mplx_plan_batch_fits.restype = i32
+    lib.mplx_plan_batch_cost_terms.argtypes = [vp, vp, vp, vp, i32, f64, i32, f64, f64, f64, f64, C.POINTER(BatchOut)]
+    lib.mplx_plan_batch_cost_terms.restype = i32
+    lib.mplx_plan_batch_cost_terms_fits.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+    lib.mplx_plan_batch_cost_terms_fits.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

@@ -369,9 +369,24 @@ class env_map:
 
     def plan_batch(self, starts, goals, eps=1.0, max_expand=1000, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
                    tol_yaw=-1.0, start_free=None, closed=True):
-        """mplx_plan_batch: the A* searches of n (start, goal) queries on the device (occupancy planning).
-        Returns a dict: valid, cost, expanded, n_closed (arrays), actions / closed (one array per query),
-        slots, arena_bytes, seconds.  Raises MplxError (code MPLX_ERR_ARG) for the plans it refuses."""
+        """mplx_plan_batch: the A* searches of n (start, goal) queries on the device (occupancy planning;
+        plan_batch_cost_terms serves potential-field and yaw planning).  Returns a dict: valid, cost, expanded,
+        n_closed (arrays), actions / closed (one array per query), slots, arena_bytes, seconds.  Raises
+        MplxError (code MPLX_ERR_ARG) for the plans it refuses."""
+        return self._plan_batch(self._lib.mplx_plan_batch, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc,
+                                tol_yaw, start_free, closed)
+
+    def plan_batch_cost_terms(self, starts, goals, eps=1.0, max_expand=1000, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
+                              tol_yaw=-1.0, start_free=None, closed=True):
+        """mplx_plan_batch_cost_terms: plan_batch for every plan, including a potential map (with or without a
+        gradient weight), a yaw control and a search region; the sample loop sums the potential, gradient and
+        yaw-alignment terms.  tol_yaw >= 0 adds |yaw - goal yaw| <= tol_yaw to the goal test.  Same results dict;
+        raises MplxError for max_expand <= 0, more than 256 primitives, a missing map or parameters
+        (MPLX_ERR_ARG) and search memory beyond the budget (MPLX_ERR_ALLOC)."""
+        return self._plan_batch(self._lib.mplx_plan_batch_cost_terms, starts, goals, eps, max_expand, tol_pos, tol_vel,
+                                tol_acc, tol_yaw, start_free, closed)
+
+    def _plan_batch(self, fn, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc, tol_yaw, start_free, closed):
         self._sync_params()
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)
         goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE).reshape(-1)
@@ -386,9 +401,8 @@ class env_map:
         out = abi.BatchOut(valid.ctypes.data, cost.ctypes.data, expanded.ctypes.data, n_closed.ctypes.data,
                            aoff.ctypes.data, acts.ctypes.data, cap, coff.ctypes.data, abi.ptr(keys), cap if closed else 0,
                            0, 0, 0.0)
-        abi.check(self._lib.mplx_plan_batch(self._h, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps),
-                                            int(max_expand), float(tol_pos), float(tol_vel), float(tol_acc),
-                                            float(tol_yaw), C.byref(out)))
+        abi.check(fn(self._h, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps), int(max_expand),
+                     float(tol_pos), float(tol_vel), float(tol_acc), float(tol_yaw), C.byref(out)))
         return dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
                     actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
                     closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,

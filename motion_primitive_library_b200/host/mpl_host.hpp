@@ -2047,16 +2047,25 @@ class MultiQueryPlanner {
     std::vector<int> actions;
     std::vector<uint64_t> closed_keys;  // sorted; only with setCollectClosed(true)
   };
-  /// Which loop plan() runs: AUTO picks the device search (mplx_plan_batch) for occupancy planning with
-  /// max_expand > 0 and |U| <= 256 once the batch has kDeviceSearchMinQueries queries and its worst-case
-  /// search memory fits the device-memory budget (mplx_plan_batch_fits), else the lock-step loop;
-  /// LOCKSTEP always runs the lock-step loop; DEVICE takes the device search whenever the control and
-  /// the cap allow it, whatever the batch size, and fails when the memory does not fit.  Both loops give
-  /// every query the same result.
-  enum Path { AUTO = 0, LOCKSTEP = 1, DEVICE = 2 };
+  /// Which loop plan() runs.  AUTO picks, for max_expand > 0 and |U| <= 256 when the batch's worst-case
+  /// search memory fits the device-memory budget:
+  ///   - occupancy planning: the device search (mplx_plan_batch) once the batch has
+  ///     kDeviceSearchMinQueries queries;
+  ///   - plans with per-sample cost terms (a potential map or a yaw control): the device search that sums
+  ///     them (mplx_plan_batch_cost_terms) once the batch has kDeviceCostTermsMinQueries queries;
+  /// and the lock-step loop otherwise.  LOCKSTEP always runs the lock-step loop.  DEVICE takes
+  /// mplx_plan_batch whenever the plan, the control and the cap allow it, whatever the batch size;
+  /// DEVICE_COST_TERMS takes mplx_plan_batch_cost_terms for every plan the cap and |U| allow.  The two
+  /// forced paths run the lock-step loop for the plans they cannot take, and fail when the memory does
+  /// not fit.  Every loop gives every query the same result.
+  enum Path { AUTO = 0, LOCKSTEP = 1, DEVICE = 2, DEVICE_COST_TERMS = 3 };
   /// Smallest batch AUTO sends to the device search.  search_bench.py, one H100 80GB HBM3 (the
   /// measurements are cited in DESIGN.md §7): the device search was faster at every measured batch size.
   static constexpr std::size_t kDeviceSearchMinQueries = 16;
+  /// Smallest cost-term batch AUTO sends to mplx_plan_batch_cost_terms.  search_bench.py --workload cfg4,
+  /// one H100 80GB HBM3 at 400 W (DESIGN.md §7): the device search was faster at every measured batch size,
+  /// 2.1x at 16 queries (0.059 s against 0.125 s) and 4.8x at 4 096.
+  static constexpr std::size_t kDeviceCostTermsMinQueries = 16;
   explicit MultiQueryPlanner(const std::shared_ptr<MapUtil<Dim>> &map_util, int device = 0)
       : map_util_(map_util), gpu_(new env_map_gpu<Dim>(map_util, device)) {}
   /// the shared env: set U, limits, weights, control, tolerances on it
@@ -2078,8 +2087,10 @@ class MultiQueryPlanner {
   void setPath(int p) { path_ = p; }
   /// also return each query's closed set (sorted lattice keys) in Result::closed_keys
   void setCollectClosed(bool on) { collect_closed_ = on; }
-  /// the path the last plan() ran: true = device search
-  bool lastPlanOnDevice() const { return last_device_; }
+  /// the path the last plan() ran: true = a device search
+  bool lastPlanOnDevice() const { return last_device_ != 0; }
+  /// the path the last plan() ran: 0 = lock-step, 1 = mplx_plan_batch, 2 = mplx_plan_batch_cost_terms
+  int lastDevicePath() const { return last_device_; }
   /// device search of the last plan(): arena slots and bytes per slot (0 after a lock-step plan)
   int searchSlots() const { return slots_; }
   long long searchArenaBytes() const { return arena_bytes_; }
@@ -2088,18 +2099,25 @@ class MultiQueryPlanner {
   bool deviceSearchPossible(int max_expand) const {
     return gpu_->keys_only_possible() && max_expand > 0 && gpu_->U_.size() <= 256;
   }
+  /// the cost-term device search serves this plan: a bounded search, |U| within one CTA (any plan)
+  bool costTermsSearchPossible(int max_expand) const { return max_expand > 0 && gpu_->U_.size() <= 256; }
 
   std::vector<Result> plan(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
                            int max_expand) {
-    last_device_ = false;
+    last_device_ = 0;
     slots_ = 0;
     arena_bytes_ = 0;
-    if (path_ != LOCKSTEP && deviceSearchPossible(max_expand) &&
+    if ((path_ == AUTO || path_ == DEVICE) && deviceSearchPossible(max_expand) &&
         (path_ == DEVICE || starts.size() >= kDeviceSearchMinQueries)) {
       std::vector<Result> res;
-      if (plan_device(starts, goals, eps, max_expand, res)) return res;
+      if (plan_device(starts, goals, eps, max_expand, false, res)) return res;
+    } else if (costTermsSearchPossible(max_expand) &&
+               (path_ == DEVICE_COST_TERMS ||
+                (path_ == AUTO && !gpu_->keys_only_possible() && starts.size() >= kDeviceCostTermsMinQueries))) {
+      std::vector<Result> res;
+      if (plan_device(starts, goals, eps, max_expand, true, res)) return res;
     }
-    last_device_ = false;
+    last_device_ = 0;
     // the search states of the previous plan() are recycled, not freed: a planner that answers batch
     // after batch allocates (and page-faults) its state memory once
     if (ss_.size() != starts.size()) release();
@@ -2181,22 +2199,24 @@ class MultiQueryPlanner {
     return res;
   }
 
-  /// plan() on the device: every query's whole A* in one mplx_plan_batch call.  The start-is-free test
-  /// runs here on the host map, as in the lock-step loop.  Returns false, with nothing planned, when the
-  /// worst-case search memory does not fit the device-memory budget (MPLX_ERR_ALLOC) under AUTO: the
-  /// caller then runs the lock-step loop, which served such plans before.  DEVICE reports it as an error.
+  /// plan() on the device: every query's whole A* in one mplx_plan_batch call (cost_terms:
+  /// mplx_plan_batch_cost_terms).  The start-is-free test runs here on the host map, as in the lock-step
+  /// loop.  Returns false, with nothing planned, when the worst-case search memory does not fit the
+  /// device-memory budget (MPLX_ERR_ALLOC) under AUTO: the caller then runs the lock-step loop, which
+  /// served such plans before.  DEVICE and DEVICE_COST_TERMS report it as an error.
   bool plan_device(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
-                   int max_expand, std::vector<Result> &res) {
+                   int max_expand, bool cost_terms, std::vector<Result> &res) {
     const std::size_t Q = starts.size();
     res.assign(Q, Result());
     iterations_ = nodes_ = 0;
     t_pop_ = t_dev_ = t_relax_ = 0;
     gpu_->prepare_device();
     // sized before any result buffer exists: the host arrays below are as large as the device's
-    const int fit = mplx_plan_batch_fits(gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
+    const int fit = (cost_terms ? mplx_plan_batch_cost_terms_fits : mplx_plan_batch_fits)(
+        gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
     if (fit == MPLX_ERR_ALLOC && path_ == AUTO) return false;
     if (fit != MPLX_OK) throw std::runtime_error(mplx_last_error());
-    last_device_ = true;
+    last_device_ = cost_terms ? 2 : 1;
     if (Q == 0) return true;
     std::vector<mplx_waypoint> S(Q), G(Q);
     std::vector<uint8_t> fr(Q);
@@ -2213,11 +2233,12 @@ class MultiQueryPlanner {
                        (int64_t)acts.size(), collect_closed_ ? coff.data() : nullptr,
                        collect_closed_ ? keys.data() : nullptr, (int64_t)keys.size(), 0, 0, 0.0};
     const auto t0 = std::chrono::steady_clock::now();
-    const int rc = mplx_plan_batch(gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_,
-                                   gpu_->tol_vel_, gpu_->tol_acc_, gpu_->tol_yaw_, &out);
+    const int rc = (cost_terms ? mplx_plan_batch_cost_terms : mplx_plan_batch)(
+        gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_,
+        gpu_->tol_acc_, gpu_->tol_yaw_, &out);
     // the device allocation itself can still fail when other users of the card took memory in between
     if (rc == MPLX_ERR_ALLOC && path_ == AUTO) {
-      last_device_ = false;
+      last_device_ = 0;
       return false;
     }
     if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
@@ -2266,7 +2287,8 @@ class MultiQueryPlanner {
   int host_threads_ = 0;
   bool keys_only_ = true;
   int path_ = AUTO;
-  bool collect_closed_ = false, last_device_ = false;
+  bool collect_closed_ = false;
+  int last_device_ = 0;  // lastDevicePath()
   int slots_ = 0;
   long long arena_bytes_ = 0;
   static constexpr int kMaxSucc = 1024;  // |U| upper bound of libmplx

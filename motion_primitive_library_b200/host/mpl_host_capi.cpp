@@ -285,13 +285,14 @@ int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
   return 0;
 }
 
-/* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (the device search for
- * occupancy planning with a bounded search once the batch is large enough), 1 = always lock-step,
- * 2 = the device search whenever the plan allows it. */
+/* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (a device search for a
+ * bounded search once the batch is large enough: mplx_plan_batch for occupancy planning,
+ * mplx_plan_batch_cost_terms for potential-field and yaw planning), 1 = always lock-step, 2 = the
+ * occupancy device search whenever the plan allows it, 3 = the cost-term device search for every plan. */
 int mplh_batch_set_path(void *session, int path) {
   BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq || path < 0 || path > 2) {
-    g_err = "null session or path not in 0..2";
+  if (!s || !s->mq || path < 0 || path > 3) {
+    g_err = "null session or path not in 0..3";
     return 1;
   }
   if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setPath(path);
@@ -299,8 +300,9 @@ int mplh_batch_set_path(void *session, int path) {
   return 0;
 }
 
-/* The last plan of the session: *device = 1 when it ran the device search (then *slots and *arena_bytes
- * describe its arenas), 0 when it ran the lock-step loop. */
+/* The last plan of the session: *device = 1 when it ran the occupancy device search, 2 when it ran the
+ * cost-term device search (then *slots and *arena_bytes describe its arenas), 0 when it ran the lock-step
+ * loop. */
 int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t *arena_bytes) {
   BatchSession *s = (BatchSession *)session;
   if (!s || !s->mq) {
@@ -308,7 +310,7 @@ int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t
     return 1;
   }
   auto put = [&](const auto *mq) {
-    if (device) *device = mq->lastPlanOnDevice() ? 1 : 0;
+    if (device) *device = mq->lastDevicePath();
     if (slots) *slots = mq->searchSlots();
     if (arena_bytes) *arena_bytes = mq->searchArenaBytes();
   };

@@ -292,9 +292,9 @@ def plan_trace(args, cap=1 << 20):
 
 def plan_batch(args, starts, goals, path="auto"):
     """MPL::MultiQueryPlanner over many (start, goal) pairs, one session opened and closed around the call.
-    path: "auto" (the device search for occupancy planning with a bounded search once the batch is large
-    enough, else the lock-step loop: one device launch per iteration expands the current node of every live
-    query), "lockstep" or "device" (see BatchPlanner).  starts/goals: WAYPOINT_DTYPE arrays."""
+    path: "auto" (a device search for a bounded search once the batch is large enough, else the lock-step
+    loop: one device launch per iteration expands the current node of every live query), "lockstep",
+    "device" or "device_cost_terms" (see BatchPlanner).  starts/goals: WAYPOINT_DTYPE arrays."""
     s = BatchPlanner(args, path=path)
     try:
         res, tot = s.plan(starts, goals)
@@ -312,13 +312,16 @@ class BatchPlanner:
     are recycled for the next (a planner that answers batch after batch allocates its state memory once).
     `args` supplies the map, the controls and the limits (its start/goal are ignored).
 
-    path: "auto" runs each query's whole A* on the device (mplx_plan_batch) for occupancy planning (no
-    potential map, no yaw control) with max_num > 0 once the batch is large enough, and the lock-step loop
-    otherwise; "lockstep" always runs the lock-step loop, "device" the device search whenever the plan allows
-    it.  Every path gives each query the same result; the choice is a diagnostic.  The totals of plan()
-    say which ran ("path")."""
+    path: "auto" runs each query's whole A* on the device for max_num > 0 and at most 256 primitives once the
+    batch is large enough: occupancy planning (no potential map, no yaw control) with mplx_plan_batch, potential-
+    field and yaw planning with mplx_plan_batch_cost_terms; otherwise the lock-step loop.  "lockstep" always
+    runs the lock-step loop, "device" mplx_plan_batch whenever the plan allows it, "device_cost_terms"
+    mplx_plan_batch_cost_terms for every plan the cap and the control set allow.  Every path gives each query
+    the same result; the choice is a diagnostic.  The totals of plan() say which ran ("path": "device",
+    "device_cost_terms" or "lockstep")."""
 
-    PATHS = {"auto": 0, "lockstep": 1, "device": 2}
+    PATHS = {"auto": 0, "lockstep": 1, "device": 2, "device_cost_terms": 3}
+    _RAN = {0: "lockstep", 1: "device", 2: "device_cost_terms"}
 
     def __init__(self, args, path="auto"):
         self._lib, _ = _host()
@@ -338,7 +341,7 @@ class BatchPlanner:
         dev, slots, nbytes = C.c_int32(0), C.c_int32(0), C.c_int64(0)
         if self._lib.mplh_batch_last_path(self._h, C.byref(dev), C.byref(slots), C.byref(nbytes)) != 0:
             raise RuntimeError(self._lib.mplh_last_error().decode())
-        return dict(path="device" if dev.value else "lockstep", slots=int(slots.value), arena_bytes=int(nbytes.value))
+        return dict(path=self._RAN[dev.value], slots=int(slots.value), arena_bytes=int(nbytes.value))
 
     def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True):
         """plan() that also returns every query's trajectory (action ids) and closed set (sorted lattice keys):
