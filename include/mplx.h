@@ -64,7 +64,10 @@ typedef struct mplx_ctx mplx_ctx;
  * !(tn == curr) && validate_primitive(...) (env_map.h:158-160); cost may be +inf
  * (colliding but dynamically valid — LPA* keeps those, graph_search.h:284-311).
  * Any pointer except `count` may be NULL to skip that field.  All pointers are HOST
- * pointers for mplx_expand and DEVICE pointers for mplx_expand_device. */
+ * pointers for mplx_expand and DEVICE pointers for mplx_expand_device.
+ * mplx_expand and mplx_expand_device may also write the slots [i*nU + count[i], (i+1)*nU)
+ * of every non-NULL array; what they hold there is unspecified.  Nothing outside
+ * [0, n_nodes*nU) is written. */
 typedef struct {
   int32_t *count;      /* [n_nodes]                                                       */
   mplx_waypoint *succ; /* [n_nodes*nU]   succ      (vec_E<Waypoint<Dim>>&, env_map.h:147)   */

@@ -21,6 +21,7 @@
 
 #include "mplx_dispatch.h"
 #include "mplx_fx.cuh"
+#include "mplx_span.cuh"
 
 namespace mplx {
 
@@ -57,13 +58,46 @@ struct FxnShared {
   unsigned short cnt[kWarps][33], start[kWarps][33];
 };
 constexpr unsigned kNoWork = 0xffffffffu;
-constexpr int kStageBytes = 32 * (int)sizeof(mplx_waypoint);  // one warp's successor records
 
-template <int DIM, int ORD, int UNR, int MINB, bool LAT, bool REGION, bool SORT>
+// Shared-memory staging of the CTA's output span (mplx_span.cuh): byte offsets into the dynamic buffer, 16-byte
+// aligned, -1 where the array is written per lane.  An array is staged at its offset + (global address of its
+// span & 15), so that shared and global addresses agree mod 16 as the bulk copies require.
+struct FxnStage {
+  int succ, key, action, cost;
+};
+// staged outputs of the unsorted path by default (bits 1 succ, 2 key + action, 4 cost), measured on the headline
+// and cfg2 (DESIGN §4.2); keys, actions and costs only where the sample loops run long enough to hide their copies
+// and barriers: the plan bounds them at maxn = ceil(v_max T / res) samples (headline 30: staged, cfg2 12: not)
+constexpr int kSpanUnsorted = 7, kSpanMinLoop = 20;
+
+__device__ __forceinline__ void bulk_copy(void *g, const unsigned char *s, unsigned bytes) {
+  const unsigned sa = (unsigned)__cvta_generic_to_shared(s);
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(g), "r"(sa), "r"(bytes) : "memory");
+}
+
+// One thread writes a staged span of n elements to g: 4-byte stores for the lead and trail, bulk copies for the
+// head, the whole lines and the tail.  The caller commits the bulk group.
+__device__ __forceinline__ void span_out(void *g, const unsigned char *s, unsigned elem, unsigned n) {
+  const SpanCopy c = span_copy(reinterpret_cast<uintptr_t>(g), elem, n);
+  unsigned char *d = static_cast<unsigned char *>(g);
+  const unsigned end = elem * n, trail0 = end - c.trail;
+  for (unsigned i = 0; i < c.lead; i += 4) *reinterpret_cast<uint32_t *>(d + i) = *reinterpret_cast<const uint32_t *>(s + i);
+  for (unsigned i = trail0; i < end; i += 4) *reinterpret_cast<uint32_t *>(d + i) = *reinterpret_cast<const uint32_t *>(s + i);
+  unsigned at = c.lead;
+  if (c.head) bulk_copy(d + at, s + at, c.head);
+  at += c.head;
+  if (c.body) bulk_copy(d + at, s + at, c.body);
+  at += c.body;
+  if (c.tail) bulk_copy(d + at, s + at, c.tail);
+}
+
+// STAGE: the outputs leave through the CTA-span staging (unsorted path with a 16-byte aligned succ array only; the
+// instantiations without it carry none of its code).
+template <int DIM, int ORD, int UNR, int MINB, bool LAT, bool REGION, bool SORT, bool STAGE>
 __global__ void __launch_bounds__(kThreads, MINB)
 expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__restrict__ nodes, int n_nodes, int npb,
                   int inv_nU, int inv_rows, FxAmbRec *__restrict__ amb_q, unsigned *__restrict__ amb_n,
-                  unsigned amb_cap, const __grid_constant__ OutPtrs o, int pf_ahead, int stage_off) {
+                  unsigned amb_cap, const __grid_constant__ OutPtrs o, int pf_ahead, const FxnStage sg) {
   extern __shared__ __align__(16) unsigned char fx_dyn[];
   FxnRow<ORD> *rows = reinterpret_cast<FxnRow<ORD> *>(fx_dyn);
   __shared__ FxnShared S;
@@ -282,6 +316,11 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
     }
     __syncthreads();  // B2b: sorted positions are known
   }
+  static_assert(!(SORT && STAGE), "the sorted path writes its outputs per lane");
+  // the CTA's span of output slots, [span0, span0 + span_n), and where array x of it is staged (STAGE)
+  const size_t span0 = (size_t)node0 * nU;
+  const unsigned span_n = (unsigned)((n_nodes - node0 < npb ? n_nodes - node0 : npb) * nU);
+  auto staged = [&](int off, const void *gptr) { return fx_dyn + off + (reinterpret_cast<uintptr_t>(gptr) & 15u); };
   size_t slot = 0;
   double intrinsic = 0.0;
   if (active) {
@@ -305,7 +344,34 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
       }
     }
     if (ci == nU - 1) o.count[ni] = rank + (emit ? 1 : 0);
-    if (o.succ && emit) {
+    if constexpr (STAGE) {
+      // My slot in the CTA's span: the node's emitted successors first, in control order, then its holes past
+      // count, filled from the end, so that every slot of the span is written exactly once.
+      const int sl = s + (emit ? rank : nU - 1 - (ci - rank));
+      mplx_waypoint tn = {};  // a hole is a zero record
+      if (emit) {
+#pragma unroll
+        for (int k = 0; k < DIM; k++) {
+          const FxnRow<ORD> &Rw = rows[ra[k]];
+          tn.pos[k] = Rw.st[0];
+          tn.vel[k] = Rw.st[1];
+          tn.acc[k] = Rw.st[2];
+          tn.jrk[k] = Rw.st[3];
+        }
+        tn.t = S.tcurr[nl] + P.T;  // env_map.h:161
+      }
+      double2 *sp = reinterpret_cast<double2 *>(fx_dyn + sg.succ + sl * (int)sizeof(mplx_waypoint));
+      sp[0] = make_double2(tn.pos[0], tn.pos[1]);
+      sp[1] = make_double2(tn.pos[2], tn.vel[0]);
+      sp[2] = make_double2(tn.vel[1], tn.vel[2]);
+      sp[3] = make_double2(tn.acc[0], tn.acc[1]);
+      sp[4] = make_double2(tn.acc[2], tn.jrk[0]);
+      sp[5] = make_double2(tn.jrk[1], tn.jrk[2]);
+      sp[6] = make_double2(tn.yaw, tn.t);
+      if (sg.key >= 0) reinterpret_cast<uint64_t *>(staged(sg.key, o.key + span0))[sl] = emit ? key : 0;
+      if (sg.action >= 0) reinterpret_cast<int32_t *>(staged(sg.action, o.action + span0))[sl] = emit ? ci : 0;
+      if (sg.cost >= 0 && !emit) reinterpret_cast<double *>(staged(sg.cost, o.cost + span0))[sl] = 0.0;
+    } else if (o.succ && emit) {
       mplx_waypoint tn;
 #pragma unroll
       for (int k = 0; k < 3; k++) {
@@ -321,27 +387,13 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
       }
       tn.yaw = 0.0;
       tn.t = S.tcurr[nl] + P.T;  // env_map.h:161
-      if (stage_off >= 0) {
-        // the warp's records, compacted in lane order (= slot order), wait in shared memory for the bulk copies below
-        double2 *sp = reinterpret_cast<double2 *>(fx_dyn + stage_off + warp * kStageBytes +
-                                                  __popc(bal & ((1u << lane) - 1u)) * (int)sizeof(mplx_waypoint));
-        sp[0] = make_double2(tn.pos[0], tn.pos[1]);
-        sp[1] = make_double2(tn.pos[2], tn.vel[0]);
-        sp[2] = make_double2(tn.vel[1], tn.vel[2]);
-        sp[3] = make_double2(tn.acc[0], tn.acc[1]);
-        sp[4] = make_double2(tn.acc[2], tn.jrk[0]);
-        sp[5] = make_double2(tn.jrk[1], tn.jrk[2]);
-        sp[6] = make_double2(tn.yaw, tn.t);
-      } else {
-        // 128-bit stores (store_waypoint).  (Staging the CTA's records in shared memory for a coalesced copy-out
-        // by the threads themselves was measured: slower — the extra pass and barrier cost more than it saves.)
-        store_waypoint(o.succ + (size_t)ni * nU + rank, tn);
-      }
+      store_waypoint(o.succ + (size_t)ni * nU + rank, tn);  // 128-bit stores
     }
     if (emit) {
       slot = (size_t)ni * nU + rank;
-      if (o.action) __stcs(o.action + slot, ci);
-      if (o.key) __stcs(reinterpret_cast<unsigned long long *>(o.key + slot), (unsigned long long)key);
+      if (o.action && !(STAGE && sg.action >= 0)) __stcs(o.action + slot, ci);
+      if (o.key && !(STAGE && sg.key >= 0))
+        __stcs(reinterpret_cast<unsigned long long *>(o.key + slot), (unsigned long long)key);
       if (LAT && o.lattice) {
         int q = 0;
 #pragma unroll
@@ -357,26 +409,6 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
 #pragma unroll
       for (int a = 1; a < DIM; a++) J += rows[ra[a]].J;
       intrinsic = J + P.w * P.T;
-    }
-  }
-
-  // The records leave through the bulk-copy engine (cp.async.bulk, shared -> global): the emitting lanes of one
-  // node hold consecutive slots, so each node's part of the warp is ONE contiguous copy issued by its first
-  // lane, and the 112-byte records never pass the L1's tag stage (as per-lane stores they cost it as many
-  // look-ups as all voxel loads of the kernel).
-  bool bulk_issued = false;
-  if (stage_off >= 0 && o.succ) {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // my generic-proxy writes, before the async reads
-    __syncwarp();
-    const unsigned peers = __match_any_sync(0xffffffffu, nl) & bal;  // emitting lanes of my node in this warp
-    if (emit && lane == __ffs(peers) - 1) {
-      const unsigned bytes = (unsigned)__popc(peers) * (unsigned)sizeof(mplx_waypoint);
-      const unsigned src = (unsigned)__cvta_generic_to_shared(
-          fx_dyn + stage_off + warp * kStageBytes + __popc(bal & ((1u << lane) - 1u)) * (int)sizeof(mplx_waypoint));
-      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(o.succ + slot), "r"(src), "r"(bytes)
-                   : "memory");
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      bulk_issued = true;
     }
   }
 
@@ -405,12 +437,31 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
       unsigned ns = 0;
       v = isinf(traverse_loop<DIM, ORD, false>(P, cf, false, max_v, ns)) ? 1 : 0;
     }
-    if (o.cost) o.cost[slot] = v == 1 ? (double)INFINITY : 0.0 + intrinsic;
+    const double c = v == 1 ? (double)INFINITY : 0.0 + intrinsic;
+    if (STAGE && sg.cost >= 0) reinterpret_cast<double *>(staged(sg.cost, o.cost + span0))[slot - span0] = c;
+    else if (o.cost) o.cost[slot] = c;
   }
   if (SORT) {
     __syncthreads();  // B3: the sorted work list is complete
     wk = S.work[threadIdx.x];
     wowner = S.owner[threadIdx.x];
+  }
+
+  // The staged spans leave through the bulk-copy engine (cp.async.bulk, shared -> global), while the sample loop
+  // runs: the CTA's records, keys and actions are each one contiguous range of the output arrays, so the copies
+  // write whole 128-byte lines except at the span's two ends, and the 112-byte records never pass the L1's tag
+  // stage (as per-lane stores they cost it as many look-ups as all voxel loads of the kernel).
+  bool bulk_issued = false;
+  if constexpr (STAGE) {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes, before the async reads
+    __syncthreads();                                                // B3: the staged span is complete
+    if (threadIdx.x == 0) {
+      span_out(o.succ + span0, fx_dyn + sg.succ, (unsigned)sizeof(mplx_waypoint), span_n);
+      if (sg.key >= 0) span_out(o.key + span0, staged(sg.key, o.key + span0), 8u, span_n);
+      if (sg.action >= 0) span_out(o.action + span0, staged(sg.action, o.action + span0), 4u, span_n);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      bulk_issued = true;
+    }
   }
 
   // ---- phase C (thread = work item): the fixed-point sample loop, two groups in flight ----
@@ -485,7 +536,22 @@ expand_fxn_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__re
     unsigned ns = 0;
     verdict = isinf(traverse_loop<DIM, ORD, false>(P, cf, false, mv, ns)) ? 1 : 0;
   }
-  if ((verdict == 0 || verdict == 1) && o.cost) __stcs(o.cost + wslot, verdict == 1 ? (double)INFINITY : 0.0 + wintr);
+  if (STAGE && sg.cost >= 0) {
+    // Queued primitives (verdict 2) get a finite placeholder: fx_resolve_kernel runs behind this kernel on the
+    // same stream and overwrites their slots.
+    if (verdict >= 0)
+      reinterpret_cast<double *>(staged(sg.cost, o.cost + span0))[wslot - (unsigned)span0] =
+          verdict == 1 ? (double)INFINITY : (verdict == 2 ? 0.0 : 0.0 + wintr);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();  // B4: every cost of the span is staged
+    if (threadIdx.x == 0) {
+      span_out(o.cost + span0, staged(sg.cost, o.cost + span0), 8u, span_n);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      bulk_issued = true;
+    }
+  } else if ((verdict == 0 || verdict == 1) && o.cost) {
+    __stcs(o.cost + wslot, verdict == 1 ? (double)INFINITY : 0.0 + wintr);
+  }
   // the staging buffer must outlive the copies that read it
   if (bulk_issued) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
@@ -562,7 +628,9 @@ cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, 
   const int inv_nU = ((1 << 20) + P.nU - 1) / P.nU;
   const int inv_rows = ((1 << 20) + P.n_rows - 1) / P.n_rows;
   static const int sort_env = [] { const char *v = getenv("MPLX_FXN_SORT"); return v ? atoi(v) : -1; }();  // tuning
-  static const int bulk_env = [] { const char *v = getenv("MPLX_FXN_BULK"); return v ? atoi(v) : -1; }();  // tuning / A-B
+  // tuning / A-B: which outputs of the unsorted path go through the CTA-span staging (bits 1 succ, 2 key + action,
+  // 4 cost)
+  static const int span_env = [] { const char *v = getenv("MPLX_FXN_SPAN"); return v ? atoi(v) : -1; }();
   cudaError_t e = cudaMemsetAsync(amb_n, 0, sizeof(unsigned) * kFxSegments, st);
   if (e != cudaSuccess) return e;
   // Keep the voxel bitmaps in the L2's persisting carve-out: every CTA of every launch re-reads them while
@@ -588,16 +656,34 @@ cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, 
     return with_order(P.control, [&](auto ORD) {
       const int rows_bytes = (int)(((size_t)npb * P.n_rows * sizeof(FxnRow<ORD>) + 15) & ~(size_t)15);
       const bool sort = sort_env >= 0 ? sort_env != 0 : ORD >= 3;
-      // staging of the successor records for the bulk copies (expand_fxn_kernel): destination 16-byte aligned
-      // The sorted path (JRK-125 with the CTA sort) keeps the per-lane stores: on that workload the bulk copies
-      // were measured slower.
-      const bool bulk = (bulk_env >= 0 ? bulk_env != 0 : !sort) && o.succ != nullptr &&
-                        (reinterpret_cast<uintptr_t>(o.succ) & 15u) == 0;
-      const int stage_off = bulk ? rows_bytes : -1;
-      const size_t smem = (size_t)rows_bytes + (bulk ? (size_t)kWarps * kStageBytes : 0);
+      // Staging of the CTA's output span for the bulk copies (expand_fxn_kernel, STAGE).  The sorted path (JRK-125
+      // with the CTA sort) keeps the per-lane stores: on cfg3 the staged span was measured slower.  The records
+      // need a 16-byte aligned array.  Keys, actions and costs are staged with the records only (without them, as
+      // in mplx_expand_packed, or with short sample loops, the barriers cost more than the copies save) and only
+      // while the CTA stays within 48 KB of shared memory: 4 CTAs per SM then fit the 196 KB carve-out step (1 KB
+      // of each CTA is reserved by the system) and leave 60 KB of L1 to the voxel lines.
+      const int mask = sort ? 0 : span_env >= 0 ? span_env : P.maxn >= kSpanMinLoop ? kSpanUnsorted : 1;
+      const size_t span_slots = (size_t)npb * P.nU;
+      FxnStage sg = {-1, -1, -1, -1};
+      size_t smem = (size_t)rows_bytes;
+      auto take = [&](size_t bytes) {
+        const int off = (int)smem;
+        smem += (bytes + 16 + 15) & ~(size_t)15;  // + the shift that matches the global address mod 16
+        return off;
+      };
+      if ((mask & 1) && o.succ && (reinterpret_cast<uintptr_t>(o.succ) & 15u) == 0)
+        sg.succ = take(span_slots * sizeof(mplx_waypoint));
+      constexpr size_t kCtaSmem = 48 * 1024;
+      const size_t ka = (o.key ? span_slots * 8 + 32 : 0) + (o.action ? span_slots * 4 + 32 : 0);
+      if ((mask & 2) && sg.succ >= 0 && ka > 0 && smem + ka + sizeof(FxnShared) <= kCtaSmem) {
+        if (o.key) sg.key = take(span_slots * 8);
+        if (o.action) sg.action = take(span_slots * 4);
+      }
+      if ((mask & 4) && sg.succ >= 0 && o.cost && smem + span_slots * 8 + 32 + sizeof(FxnShared) <= kCtaSmem)
+        sg.cost = take(span_slots * 8);
       auto launch = [&](auto UNR, auto MINB, auto LAT, auto REGION) {
-        return with_bool(sort, [&](auto SORT) {
-          const auto kernel = expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT>;
+        auto go = [&](auto SORT, auto STAGE) {
+          const auto kernel = expand_fxn_kernel<DIM, ORD, UNR, MINB, LAT, REGION, SORT, STAGE>;
           if (smem > 32 * 1024) {  // static + dynamic may pass the 48 KB default
             const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (r != cudaSuccess) return r;
@@ -607,9 +693,11 @@ cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, 
             if (r != cudaSuccess) return r;
           }
           kernel<<<grid, kThreads, smem, st>>>(P, d_nodes, n_nodes, npb, inv_nU, inv_rows, q, amb_n, amb_cap, o,
-                                                pf_ahead, stage_off);
+                                                pf_ahead, sg);
           return cudaGetLastError();
-        });
+        };
+        if (sort) return go(std::true_type{}, std::false_type{});
+        return with_bool(sg.succ >= 0, [&](auto STAGE) { return go(std::false_type{}, STAGE); });
       };
       const std::true_type yes{};
       const std::false_type no{};
