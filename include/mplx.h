@@ -287,6 +287,77 @@ int mplx_plan_batch_cost_terms(mplx_ctx *ctx, const mplx_waypoint *starts, const
 int mplx_plan_batch_cost_terms_fits(mplx_ctx *ctx, int n_q, int max_expand, int with_closed, int32_t *slots,
                                     int64_t *arena_bytes);
 
+/* Results of mplx_plan_batch_grow (HOST arrays of n_q entries, all required).  The trajectories and closed
+ * keys follow with mplx_plan_batch_grow_results. */
+typedef struct {
+  int32_t *valid;     /* [n_q] as mplx_batch_out                                                    */
+  double *cost;       /* [n_q]                                                                      */
+  int32_t *expanded;  /* [n_q]                                                                      */
+  int32_t *n_closed;  /* [n_q]                                                                      */
+  int32_t *n_actions; /* [n_q] trajectory length                                                    */
+  int32_t *searched;  /* [n_q] 1: the fields above are the query's result; 0: its search needed more than
+                         the largest capacity (its fields are 0 / +inf)                              */
+  int32_t rounds;     /* out: kernel launches this call made                                        */
+  int32_t slots;      /* out: slots (arenas) of the first round                                     */
+  int64_t first_cap, last_cap; /* out: records per arena in the first and the last round            */
+  int64_t arena_bytes; /* out: bytes of one first-round arena                                       */
+  int64_t reruns;     /* out: query searches abandoned and searched again (arena or result pool full) */
+  double seconds;     /* out: device time of all rounds (CUDA events)                               */
+} mplx_grow_out;
+
+/* Graph search A* for n_q queries as mplx_plan_batch (cost_terms = 0: the occupancy search, with its
+ * refusals) or mplx_plan_batch_cost_terms (cost_terms = 1, with its refusals) runs it, with arenas sized
+ * for the batch rather than for the worst case, so that unbounded searches (max_expand <= 0, the
+ * reference's default setMaxNum(-1)) and caps whose worst case does not fit run on the device too.  Each
+ * searched query gives exactly what the host planner gives: a query that outgrows its arena is abandoned
+ * and searched again from scratch, and a search's result does not depend on its arena's size.
+ *
+ * Capacity: an arena of cap records holds cap states and cap predecessor records.  A query's need is the
+ * larger of its final state and predecessor-record counts (the records, one per finite successor,
+ * normally bind); it finishes in an arena with cap >= need and is abandoned in one with cap < need.
+ *
+ * Budget: as mplx_plan_batch_fits (a quarter of the free device memory counting the search buffers the
+ * ctx holds, at most 8 GiB).  The per-query arrays (a few hundred bytes per query) and the automatic
+ * result pool (an eighth of the budget) come off it first; the arenas share the rest.
+ *
+ * Round schedule (each round is one kernel launch over the round's pending queries, each query with a
+ * fresh key-table epoch):
+ *   cap_max = the largest capacity at which one arena fits the rest of the budget, at most max_cap when
+ *             max_cap > 0, and at most 1 + max_expand*nU (the worst case) when max_expand > 0;
+ *   cap_0   = first_cap when first_cap > 0, else the largest capacity at which min(n_q, resident CTAs)
+ *             arenas fit the rest of the budget; then clipped to [1, cap_max].  A bounded plan whose worst
+ *             case fits therefore runs in one round.
+ *   Round r runs its pending queries in max(1, min(pending, resident CTAs, arenas that fit)) slots.  A query that
+ *   finishes takes its room in the result pool; one that finds the pool full stays pending at the same
+ *   capacity; one that overflows moves on.  The pool-full queries run again first, at the same capacity;
+ *   then the overflowed ones at min(4*cap, cap_max).  A query that overflows at cap_max gets searched = 0.
+ *   reruns counts every query that was queued again (pool full or overflowed below cap_max).
+ *
+ * Result pool: completed queries reserve room for their closed keys (with_closed) and action ids in one
+ * device pool, one atomicAdd per query; the pool is drained to the host after each round.  pool_bytes > 0
+ * sets its size (a diagnostic), 0 takes an eighth of the budget.  The rerun of queries that found the pool
+ * full gets a pool that holds the largest of them, so every round completes at least one query.  No result
+ * is truncated or written out of bounds.
+ *
+ * Refusals, each with the outputs and the ctx untouched and no launch: MPLX_ERR_ARG for cost_terms not 0
+ * or 1, a potential map or a yaw control with cost_terms = 0, nU > 256, a missing map or parameters, a NULL
+ * out or output array, missing query arrays, n_q < 0, or a negative first_cap, max_cap or pool_bytes;
+ * MPLX_ERR_ALLOC when not even an arena of one record fits next to the per-query arrays and the pool.
+ * The arenas stay in the ctx and are shared with mplx_plan_batch and mplx_plan_batch_cost_terms.
+ * Synchronous. */
+int mplx_plan_batch_grow(mplx_ctx *ctx, int cost_terms, const mplx_waypoint *starts, const mplx_waypoint *goals,
+                         const uint8_t *start_free, int n_q, double eps, int max_expand, double tol_pos,
+                         double tol_vel, double tol_acc, double tol_yaw, int with_closed, int64_t first_cap,
+                         int64_t max_cap, int64_t pool_bytes, mplx_grow_out *out);
+
+/* The trajectories (action ids from start to goal) and the closed keys (sorted ascending; with_closed) of
+ * the last mplx_plan_batch_grow call on this ctx: query q's at actions[action_offset[q], action_offset[q+1])
+ * and closed_keys[closed_offset[q], closed_offset[q+1]) (offsets have n_q+1 entries; closed_keys NULL skips
+ * them, and a call without with_closed has none).  MPLX_ERR_ARG, writing nothing, when no call was made,
+ * an array is missing, or a capacity is below the sum of n_actions / n_closed. */
+int mplx_plan_batch_grow_results(mplx_ctx *ctx, int64_t *action_offset, int32_t *actions, int64_t action_capacity,
+                                 int64_t *closed_offset, uint64_t *closed_keys, int64_t closed_capacity);
+
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field
  * planning once a batch fills the GPU, else the register kernel),

@@ -49,6 +49,8 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_fits",
     "mplx_plan_batch_cost_terms",
     "mplx_plan_batch_cost_terms_fits",
+    "mplx_plan_batch_grow",
+    "mplx_plan_batch_grow_results",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -109,6 +111,26 @@ class BatchOut(C.Structure):
         ("closed_capacity", C.c_int64),
         ("slots", C.c_int32),
         ("arena_bytes", C.c_int64),
+        ("seconds", C.c_double),
+    ]
+
+
+class GrowOut(C.Structure):
+    """mplx_grow_out"""
+
+    _fields_ = [
+        ("valid", C.c_void_p),
+        ("cost", C.c_void_p),
+        ("expanded", C.c_void_p),
+        ("n_closed", C.c_void_p),
+        ("n_actions", C.c_void_p),
+        ("searched", C.c_void_p),
+        ("rounds", C.c_int32),
+        ("slots", C.c_int32),
+        ("first_cap", C.c_int64),
+        ("last_cap", C.c_int64),
+        ("arena_bytes", C.c_int64),
+        ("reruns", C.c_int64),
         ("seconds", C.c_double),
     ]
 
@@ -178,6 +200,12 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch_cost_terms.restype = i32
     lib.mplx_plan_batch_cost_terms_fits.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
     lib.mplx_plan_batch_cost_terms_fits.restype = i32
+    i64 = C.c_int64
+    lib.mplx_plan_batch_grow.argtypes = [vp, i32, vp, vp, vp, i32, f64, i32, f64, f64, f64, f64, i32, i64, i64, i64,
+                                         C.POINTER(GrowOut)]
+    lib.mplx_plan_batch_grow.restype = i32
+    lib.mplx_plan_batch_grow_results.argtypes = [vp, vp, vp, i64, vp, vp, i64]
+    lib.mplx_plan_batch_grow_results.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

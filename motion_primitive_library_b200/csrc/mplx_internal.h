@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <vector>
 #include "../../include/mplx.h"
 #include "mplx_device.cuh"
 #include "mplx_kernels.h"
@@ -175,9 +176,16 @@ struct SearchBufs {
   DevBuf<uint64_t> key, closed;
   DevBuf<int32_t> action, count, ires, actions;
   DevBuf<uint8_t> free_;
+  DevBuf<unsigned long long> offs;  // mplx_plan_batch_grow: each query's place in the result pool (closed)
+  // what mplx_plan_batch_grow_results copies: the last mplx_plan_batch_grow call's trajectories and
+  // sorted closed keys, query q's at [offset[q], offset[q+1])
+  std::vector<int64_t> grow_aoff, grow_coff;
+  std::vector<int32_t> grow_actions;
+  std::vector<uint64_t> grow_closed;
   void release() {
     arena.release(); succ.release(); queries.release(); cost.release(); dres.release(); key.release();
     closed.release(); action.release(); count.release(); ires.release(); actions.release(); free_.release();
+    offs.release();
     layout_bytes = 0;
     cleared = 0;
     next_epoch = 1;

@@ -26,7 +26,9 @@ namespace mplx {
 namespace search {
 
 enum : uint32_t { kOpened = 1u, kClosed = 2u };
-enum Status : int { kIdle = 0, kRunning = 1, kTrivial = 2, kGoal = 3, kFailed = 4 };
+// kOverflow: the query needed more states or predecessor records than its arena holds (only with the
+// capacity check, consume<true>); the search is abandoned and nothing of it is a result.
+enum Status : int { kIdle = 0, kRunning = 1, kTrivial = 2, kGoal = 3, kFailed = 4, kOverflow = 5 };
 
 // State<Dim> (mpl_host.hpp:1017-1043) without the LPA* members: rhs is never set by A*, so the
 // comparator's min(g, rhs) is g.
@@ -52,16 +54,16 @@ struct SSlot {
   uint32_t state, epoch;
 };
 
-// Worst case of one query: 1 + max_expand*nU states, as many predecessor records and heap
-// entries, and a power-of-two key table at most half full.
+// An arena of cap states, as many predecessor records and heap entries, and a power-of-two key table
+// at most half full.
 struct Layout {
   int64_t cap;  // states = predecessor records = heap entries
   int64_t tab;  // key table entries (power of two >= 2*cap)
   int64_t off_pred, off_heap, off_tab, bytes;
 };
-MPLX_HD Layout layout_for(int max_expand, int nU) {
+MPLX_HD Layout layout_cap(int64_t cap) {
   Layout L;
-  L.cap = 1 + (int64_t)max_expand * nU;
+  L.cap = cap;
   L.tab = 1;
   while (L.tab < 2 * L.cap) L.tab <<= 1;
   const int64_t st = (L.cap * (int64_t)sizeof(SState) + 255) & ~(int64_t)255;
@@ -73,6 +75,9 @@ MPLX_HD Layout layout_for(int max_expand, int nU) {
   L.bytes = L.off_tab + L.tab * (int64_t)sizeof(SSlot);
   return L;
 }
+// The worst case of one query: 1 + max_expand*nU states (one per finite successor and the start), so no
+// query of a search capped at max_expand expansions can overflow it.
+MPLX_HD Layout layout_for(int max_expand, int nU) { return layout_cap(1 + (int64_t)max_expand * nU); }
 
 struct Arena {
   SState *st;
@@ -81,6 +86,7 @@ struct Arena {
   SSlot *tab;
   uint32_t tmask, epoch;
   int32_t n_states, n_preds, heap_n;
+  int32_t cap;  // states = predecessor records the arena holds (read by the capacity check only)
 };
 MPLX_HD Arena arena_at(unsigned char *base, const Layout &L, uint32_t epoch) {
   Arena A;
@@ -91,6 +97,7 @@ MPLX_HD Arena arena_at(unsigned char *base, const Layout &L, uint32_t epoch) {
   A.tmask = (uint32_t)(L.tab - 1);
   A.epoch = epoch;
   A.n_states = A.n_preds = A.heap_n = 0;
+  A.cap = (int32_t)L.cap;
   return A;
 }
 
@@ -152,11 +159,14 @@ MPLX_HD void heap_increase(Arena &A, int s, double f) {
 MPLX_HD uint32_t slot_of(const Arena &A, uint64_t k) {
   return (uint32_t)((k * 0x9e3779b97f4a7c15ULL) >> 20) & A.tmask;
 }
-// the state of key k, or a new one (coordinates left to the caller) when absent
+// the state of key k, or a new one (coordinates left to the caller) when absent.  CHECK: -1, with
+// nothing changed, when a new state would pass the arena's capacity.
+template <bool CHECK = false>
 MPLX_HD int get_or_make(Arena &A, uint64_t k, bool &created) {
   for (uint32_t i = slot_of(A, k);; i = (i + 1) & A.tmask) {
     SSlot &e = A.tab[i];
     if (e.epoch != A.epoch) {
+      if (CHECK && A.n_states >= A.cap) return -1;
       const int s = A.n_states++;
       e.key = k;
       e.state = (uint32_t)s;
@@ -305,7 +315,12 @@ MPLX_HD int pop(Arena &A, Query &S) {
 
 // AstarStepper::consume (mpl_host.hpp:1479-1508) for the n successors of the popped node:
 // key_at(s), cost_at(s), action_at(s), coord_at(s) describe successor s in control order.
-template <typename KeyAt, typename CostAt, typename ActAt, typename CoordAt>
+// CHECK: a new state or predecessor record that would pass the arena's capacity ends the query with
+// kOverflow.  States and records only ever grow, and the search never reads the capacity otherwise, so
+// with cap >= need (the larger of the final state and record counts of the query in an unbounded arena)
+// the query runs exactly as unchecked, and with cap < need it ends in kOverflow.  Heap entries never
+// outnumber states.
+template <bool CHECK = false, typename KeyAt, typename CostAt, typename ActAt, typename CoordAt>
 MPLX_HD void consume(Arena &A, Query &S, const Grid &G, const Goal &Q, int n, KeyAt key_at, CostAt cost_at,
                      ActAt action_at, CoordAt coord_at) {
   const int cur = S.cur;
@@ -314,7 +329,11 @@ MPLX_HD void consume(Arena &A, Query &S, const Grid &G, const Goal &Q, int n, Ke
     if (isinf(c)) continue;
     const uint64_t k = key_at(s);
     bool created;
-    const int sn = get_or_make(A, k, created);
+    const int sn = get_or_make<CHECK>(A, k, created);
+    if (CHECK && (sn < 0 || A.n_preds >= A.cap)) {
+      S.status = kOverflow;
+      return;
+    }
     if (created) {
       coord_at(s, A.st[sn].coord);
       A.st[sn].h = S.eps == 0 ? 0 : heur(G, Q, A.st[sn].coord, k);

@@ -386,6 +386,40 @@ class env_map:
         return self._plan_batch(self._lib.mplx_plan_batch_cost_terms, starts, goals, eps, max_expand, tol_pos, tol_vel,
                                 tol_acc, tol_yaw, start_free, closed)
 
+    def plan_batch_grow(self, starts, goals, eps=1.0, max_expand=-1, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
+                        tol_yaw=-1.0, start_free=None, closed=True, cost_terms=False, first_cap=0, max_cap=0,
+                        pool_bytes=0):
+        """mplx_plan_batch_grow: plan_batch (cost_terms=False) or plan_batch_cost_terms (cost_terms=True) with
+        arenas sized for the batch and grown for the queries that outgrow them, so max_expand <= 0 (unbounded)
+        is served too.  first_cap / max_cap / pool_bytes: 0 = automatic (include/mplx.h has the round schedule).
+        Returns plan_batch's dict plus searched (0: the query needed more than the largest arena; its fields are
+        0 / +inf and its lists empty), rounds, reruns, first_cap and last_cap."""
+        self._sync_params()
+        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)
+        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE).reshape(-1)
+        n = starts.size
+        valid, expanded, n_closed, n_actions, searched = (np.zeros(n, np.int32) for _ in range(5))
+        cost = np.zeros(n)
+        sf = None if start_free is None else np.ascontiguousarray(start_free, dtype=np.uint8)
+        out = abi.GrowOut(valid.ctypes.data, cost.ctypes.data, expanded.ctypes.data, n_closed.ctypes.data,
+                          n_actions.ctypes.data, searched.ctypes.data, 0, 0, 0, 0, 0, 0, 0.0)
+        abi.check(self._lib.mplx_plan_batch_grow(
+            self._h, 1 if cost_terms else 0, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps),
+            int(max_expand), float(tol_pos), float(tol_vel), float(tol_acc), float(tol_yaw), 1 if closed else 0,
+            int(first_cap), int(max_cap), int(pool_bytes), C.byref(out)))
+        na, nc = int(n_actions.sum()), int(n_closed.sum()) if closed else 0
+        aoff, coff = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+        acts, keys = np.zeros(max(na, 1), np.int32), np.zeros(max(nc, 1), np.uint64)
+        abi.check(self._lib.mplx_plan_batch_grow_results(self._h, aoff.ctypes.data, acts.ctypes.data, acts.size,
+                                                         coff.ctypes.data, keys.ctypes.data if closed else None,
+                                                         keys.size))
+        return dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
+                    actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
+                    closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
+                    searched=searched, slots=int(out.slots), arena_bytes=int(out.arena_bytes),
+                    seconds=float(out.seconds), rounds=int(out.rounds), reruns=int(out.reruns),
+                    first_cap=int(out.first_cap), last_cap=int(out.last_cap))
+
     def _plan_batch(self, fn, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc, tol_yaw, start_free, closed):
         self._sync_params()
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)

@@ -2053,12 +2053,16 @@ class MultiQueryPlanner {
   ///     kDeviceSearchMinQueries queries;
   ///   - plans with per-sample cost terms (a potential map or a yaw control): the device search that sums
   ///     them (mplx_plan_batch_cost_terms) once the batch has kDeviceCostTermsMinQueries queries;
-  /// and the lock-step loop otherwise.  LOCKSTEP always runs the lock-step loop.  DEVICE takes
-  /// mplx_plan_batch whenever the plan, the control and the cap allow it, whatever the batch size;
-  /// DEVICE_COST_TERMS takes mplx_plan_batch_cost_terms for every plan the cap and |U| allow.  The two
+  /// and the lock-step loop otherwise.  For an unbounded search (max_expand <= 0, the reference's default)
+  /// and |U| <= 256, AUTO takes the growing device search (mplx_plan_batch_grow, whose arenas are sized for
+  /// the batch and grow for the queries that outgrow them) from the same batch sizes.  LOCKSTEP always runs
+  /// the lock-step loop.  DEVICE takes mplx_plan_batch whenever the plan, the control and the cap allow it,
+  /// whatever the batch size; DEVICE_COST_TERMS takes mplx_plan_batch_cost_terms for every plan the cap and
+  /// |U| allow; DEVICE_GROW takes mplx_plan_batch_grow for every plan |U| allows, bounded or not.  The
   /// forced paths run the lock-step loop for the plans they cannot take, and fail when the memory does
-  /// not fit.  Every loop gives every query the same result.
-  enum Path { AUTO = 0, LOCKSTEP = 1, DEVICE = 2, DEVICE_COST_TERMS = 3 };
+  /// not fit.  Queries the growing search could not fit in its largest arena run through the lock-step
+  /// loop.  Every loop gives every query the same result.
+  enum Path { AUTO = 0, LOCKSTEP = 1, DEVICE = 2, DEVICE_COST_TERMS = 3, DEVICE_GROW = 4 };
   /// Smallest batch AUTO sends to the device search.  search_bench.py, one H100 80GB HBM3 (the
   /// measurements are cited in DESIGN.md §7): the device search was faster at every measured batch size.
   static constexpr std::size_t kDeviceSearchMinQueries = 16;
@@ -2085,15 +2089,31 @@ class MultiQueryPlanner {
   void setKeysOnly(bool on) { keys_only_ = on; }
   /// diagnostics: force a path (Path); AUTO is the default
   void setPath(int p) { path_ = p; }
+  /// diagnostics: the growing search's first and largest arena capacity (records; 0 = automatic, see
+  /// mplx_plan_batch_grow)
+  void setGrowCaps(long long first_cap, long long max_cap) {
+    grow_first_cap_set_ = first_cap;
+    grow_max_cap_set_ = max_cap;
+  }
   /// also return each query's closed set (sorted lattice keys) in Result::closed_keys
   void setCollectClosed(bool on) { collect_closed_ = on; }
   /// the path the last plan() ran: true = a device search
   bool lastPlanOnDevice() const { return last_device_ != 0; }
-  /// the path the last plan() ran: 0 = lock-step, 1 = mplx_plan_batch, 2 = mplx_plan_batch_cost_terms
+  /// the path the last plan() ran: 0 = lock-step, 1 = mplx_plan_batch, 2 = mplx_plan_batch_cost_terms,
+  /// 3 = mplx_plan_batch_grow
   int lastDevicePath() const { return last_device_; }
-  /// device search of the last plan(): arena slots and bytes per slot (0 after a lock-step plan)
+  /// device search of the last plan(): arena slots and bytes per slot (0 after a lock-step plan); for the
+  /// growing search those of its first round
   int searchSlots() const { return slots_; }
   long long searchArenaBytes() const { return arena_bytes_; }
+  /// growing search of the last plan() (0 otherwise): kernel launches, abandoned and repeated query
+  /// searches, records per arena in the first and the last round, and the queries it handed to the
+  /// lock-step loop because they outgrew its largest arena
+  int growRounds() const { return grow_rounds_; }
+  long long growReruns() const { return grow_reruns_; }
+  long long growFirstCap() const { return grow_first_cap_; }
+  long long growLastCap() const { return grow_last_cap_; }
+  int growLockstep() const { return grow_lockstep_; }
 
   /// the device search serves this plan: occupancy planning, a bounded search, |U| within one CTA
   bool deviceSearchPossible(int max_expand) const {
@@ -2107,7 +2127,15 @@ class MultiQueryPlanner {
     last_device_ = 0;
     slots_ = 0;
     arena_bytes_ = 0;
-    if ((path_ == AUTO || path_ == DEVICE) && deviceSearchPossible(max_expand) &&
+    grow_rounds_ = grow_lockstep_ = 0;
+    grow_reruns_ = grow_first_cap_ = grow_last_cap_ = 0;
+    const bool unbounded_auto =
+        path_ == AUTO && max_expand <= 0 &&
+        starts.size() >= (gpu_->keys_only_possible() ? kDeviceSearchMinQueries : kDeviceCostTermsMinQueries);
+    if ((path_ == DEVICE_GROW || unbounded_auto) && gpu_->U_.size() <= 256) {
+      std::vector<Result> res;
+      if (plan_grow(starts, goals, eps, max_expand, res)) return res;
+    } else if ((path_ == AUTO || path_ == DEVICE) && deviceSearchPossible(max_expand) &&
         (path_ == DEVICE || starts.size() >= kDeviceSearchMinQueries)) {
       std::vector<Result> res;
       if (plan_device(starts, goals, eps, max_expand, false, res)) return res;
@@ -2257,6 +2285,94 @@ class MultiQueryPlanner {
     }
     return true;
   }
+
+  /// plan() with the growing device search (mplx_plan_batch_grow; cost_terms for every plan that is not
+  /// occupancy planning).  The queries it could not fit in its largest arena (searched = 0) run through the
+  /// lock-step loop, and their results are merged.  Returns false, with nothing planned, when not even a
+  /// one-record arena fits the budget under AUTO; DEVICE_GROW reports that as an error.
+  bool plan_grow(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
+                 int max_expand, std::vector<Result> &res) {
+    const std::size_t Q = starts.size();
+    res.assign(Q, Result());
+    iterations_ = nodes_ = 0;
+    t_pop_ = t_dev_ = t_relax_ = 0;
+    gpu_->prepare_device();
+    std::vector<mplx_waypoint> S(Q), G(Q);
+    std::vector<uint8_t> fr(Q);
+    for (std::size_t q = 0; q < Q; q++) {
+      S[q] = env_map_gpu<Dim>::pod(starts[q]);
+      G[q] = env_map_gpu<Dim>::pod(goals[q]);
+      fr[q] = map_util_->isFree(map_util_->floatToInt(starts[q].pos)) ? 1 : 0;  // env_map.h:48-51
+    }
+    std::vector<int32_t> valid(Q), expd(Q), ncl(Q), nact(Q), searched(Q);
+    std::vector<double> cost(Q);
+    mplx_grow_out out{valid.data(), cost.data(), expd.data(), ncl.data(), nact.data(), searched.data(), 0, 0, 0, 0, 0,
+                      0, 0.0};
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc = mplx_plan_batch_grow(gpu_->ctx(), gpu_->keys_only_possible() ? 0 : 1, S.data(), G.data(), fr.data(),
+                                        (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_, gpu_->tol_acc_,
+                                        gpu_->tol_yaw_, collect_closed_ ? 1 : 0, grow_first_cap_set_, grow_max_cap_set_,
+                                        0, &out);
+    if (rc == MPLX_ERR_ALLOC && path_ == AUTO) return false;
+    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    int64_t na = 0, nc = 0;
+    for (std::size_t q = 0; q < Q; q++) {
+      na += nact[q];
+      nc += collect_closed_ ? ncl[q] : 0;
+    }
+    std::vector<int64_t> aoff(Q + 1), coff(Q + 1);
+    std::vector<int32_t> acts(std::max<int64_t>(na, 1));
+    std::vector<uint64_t> keys(std::max<int64_t>(nc, 1));
+    if (mplx_plan_batch_grow_results(gpu_->ctx(), aoff.data(), acts.data(), (int64_t)acts.size(), coff.data(),
+                                     collect_closed_ ? keys.data() : nullptr, (int64_t)keys.size()) != MPLX_OK)
+      throw std::runtime_error(mplx_last_error());
+    t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    vec_E<Waypoint<Dim>> restS, restG;
+    std::vector<std::size_t> rest;
+    for (std::size_t q = 0; q < Q; q++) {
+      if (!searched[q]) {
+        rest.push_back(q);
+        restS.push_back(starts[q]);
+        restG.push_back(goals[q]);
+        continue;
+      }
+      res[q].valid = valid[q] != 0;
+      res[q].cost = cost[q];
+      res[q].expanded = expd[q];
+      res[q].n_closed = (std::size_t)ncl[q];
+      res[q].actions.assign(acts.begin() + aoff[q], acts.begin() + aoff[q + 1]);
+      if (collect_closed_) res[q].closed_keys.assign(keys.begin() + coff[q], keys.begin() + coff[q + 1]);
+      iterations_ = std::max<long>(iterations_, expd[q]);
+      nodes_ += expd[q];
+    }
+    if (!rest.empty()) {
+      const int path = path_;
+      path_ = LOCKSTEP;
+      std::vector<Result> sub;
+      try {
+        sub = plan(restS, restG, eps, max_expand);
+      } catch (...) {
+        path_ = path;
+        throw;
+      }
+      path_ = path;
+      for (std::size_t i = 0; i < rest.size(); i++) res[rest[i]] = std::move(sub[i]);
+      iterations_ = nodes_ = 0;
+      for (const Result &r : res) {
+        iterations_ = std::max<long>(iterations_, r.expanded);
+        nodes_ += r.expanded;
+      }
+    }
+    last_device_ = 3;
+    slots_ = out.slots;
+    arena_bytes_ = out.arena_bytes;
+    grow_rounds_ = out.rounds;
+    grow_reruns_ = out.reruns;
+    grow_first_cap_ = out.first_cap;
+    grow_last_cap_ = out.last_cap;
+    grow_lockstep_ = (int)rest.size();
+    return true;
+  }
   /// Free the search states of the last plan() (tens of millions of states for a large batch), on
   /// the host cores.  Called by the next plan() and the destructor.
   void release() {
@@ -2291,6 +2407,9 @@ class MultiQueryPlanner {
   int last_device_ = 0;  // lastDevicePath()
   int slots_ = 0;
   long long arena_bytes_ = 0;
+  int grow_rounds_ = 0, grow_lockstep_ = 0;
+  long long grow_reruns_ = 0, grow_first_cap_ = 0, grow_last_cap_ = 0;
+  long long grow_first_cap_set_ = 0, grow_max_cap_set_ = 0;  // setGrowCaps
   static constexpr int kMaxSucc = 1024;  // |U| upper bound of libmplx
 };
 }  // namespace MPL

@@ -170,6 +170,10 @@ struct BatchSession {
   int dim = 0;
   int control = 0;
   void *mq = nullptr;  // MPL::MultiQueryPlanner<dim>*
+  // trajectories and closed sets of the last mplh_batch_plan_keep, query q's at [offset[q], offset[q+1])
+  std::vector<int64_t> aoff, coff;
+  std::vector<int32_t> actions;
+  std::vector<uint64_t> closed;
 };
 template <int Dim>
 MPL::MultiQueryPlanner<Dim> *open_mq(const mplh_plan_args *a) {
@@ -285,14 +289,15 @@ int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
   return 0;
 }
 
-/* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (a device search for a
- * bounded search once the batch is large enough: mplx_plan_batch for occupancy planning,
- * mplx_plan_batch_cost_terms for potential-field and yaw planning), 1 = always lock-step, 2 = the
- * occupancy device search whenever the plan allows it, 3 = the cost-term device search for every plan. */
+/* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (a device search once the
+ * batch is large enough: for a bounded search mplx_plan_batch for occupancy planning and
+ * mplx_plan_batch_cost_terms for potential-field and yaw planning, for an unbounded one
+ * mplx_plan_batch_grow), 1 = always lock-step, 2 = the occupancy device search whenever the plan allows it,
+ * 3 = the cost-term device search for every plan, 4 = the growing device search for every plan. */
 int mplh_batch_set_path(void *session, int path) {
   BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq || path < 0 || path > 3) {
-    g_err = "null session or path not in 0..3";
+  if (!s || !s->mq || path < 0 || path > 4) {
+    g_err = "null session or path not in 0..4";
     return 1;
   }
   if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setPath(path);
@@ -300,9 +305,44 @@ int mplh_batch_set_path(void *session, int path) {
   return 0;
 }
 
+/* Diagnostics: the first and the largest arena capacity (records) of the session's growing device searches;
+ * 0 = automatic (mplx_plan_batch_grow).  Negative values fail. */
+int mplh_batch_set_grow_caps(void *session, int64_t first_cap, int64_t max_cap) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq || first_cap < 0 || max_cap < 0) {
+    g_err = "null session or negative capacity";
+    return 1;
+  }
+  if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setGrowCaps(first_cap, max_cap);
+  else ((MPL::MultiQueryPlanner<3> *)s->mq)->setGrowCaps(first_cap, max_cap);
+  return 0;
+}
+
+/* The growing device search of the session's last plan (all 0 when it ran another path): kernel launches,
+ * query searches abandoned and repeated, records per arena in the first and the last round, and queries it
+ * handed to the lock-step loop.  Any pointer may be NULL. */
+int mplh_batch_grow_stats(void *session, int32_t *rounds, int64_t *reruns, int64_t *first_cap, int64_t *last_cap,
+                          int32_t *lockstep) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq) {
+    g_err = "null session";
+    return 1;
+  }
+  auto put = [&](const auto *mq) {
+    if (rounds) *rounds = mq->growRounds();
+    if (reruns) *reruns = mq->growReruns();
+    if (first_cap) *first_cap = mq->growFirstCap();
+    if (last_cap) *last_cap = mq->growLastCap();
+    if (lockstep) *lockstep = mq->growLockstep();
+  };
+  if (s->dim == 2) put((const MPL::MultiQueryPlanner<2> *)s->mq);
+  else put((const MPL::MultiQueryPlanner<3> *)s->mq);
+  return 0;
+}
+
 /* The last plan of the session: *device = 1 when it ran the occupancy device search, 2 when it ran the
- * cost-term device search (then *slots and *arena_bytes describe its arenas), 0 when it ran the lock-step
- * loop. */
+ * cost-term device search, 3 when it ran the growing device search (then *slots and *arena_bytes describe
+ * its (first round's) arenas), 0 when it ran the lock-step loop. */
 int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t *arena_bytes) {
   BatchSession *s = (BatchSession *)session;
   if (!s || !s->mq) {
@@ -319,19 +359,17 @@ int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t
   return 0;
 }
 
-/* mplh_batch_plan that also returns every query's trajectory (action ids, query q's at
- * actions[action_offset[q], action_offset[q+1])) and closed set (sorted lattice keys, likewise with
- * closed_offset; closed_keys NULL = skip).  A capacity that is too small fails the call. */
-int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
-                           int max_num, mplh_query_result *out, double *totals, int64_t *action_offset, int32_t *actions,
-                           int64_t cap_actions, int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
+/* mplh_batch_plan that keeps every query's trajectory (action ids) and, with collect_closed, closed set
+ * (sorted lattice keys) in the session for mplh_batch_kept; out[q].n_actions and out[q].n_closed size
+ * them, whatever max_num is. */
+int mplh_batch_plan_keep(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
+                         int max_num, int collect_closed, mplh_query_result *out, double *totals) {
   try {
     BatchSession *s = (BatchSession *)session;
     if (!s || !s->mq) throw std::runtime_error("null session");
-    if (!action_offset || !actions || (closed_keys && !closed_offset)) throw std::runtime_error("missing output array");
     auto go = [&](auto *mq, auto dimtag) {
       constexpr int Dim = decltype(dimtag)::value;
-      mq->setCollectClosed(closed_keys != nullptr);
+      mq->setCollectClosed(collect_closed != 0);
       // the session's later plans must not keep collecting, whatever plan() does
       struct Reset {
         decltype(mq) p;
@@ -345,23 +383,20 @@ int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mpl
       auto t0 = std::chrono::steady_clock::now();
       auto res = mq->plan(S, G, eps, max_num);
       const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      int64_t ao = 0, co = 0;
-      action_offset[0] = 0;
-      if (closed_offset) closed_offset[0] = 0;
+      s->aoff.assign((size_t)n_q + 1, 0);
+      s->coff.assign((size_t)n_q + 1, 0);
+      s->actions.clear();
+      s->closed.clear();
       for (int q = 0; q < n_q; q++) {
         out[q].valid = res[q].valid ? 1 : 0;
         out[q].cost = res[q].cost;
         out[q].expanded = res[q].expanded;
         out[q].n_closed = (int)res[q].n_closed;
         out[q].n_actions = (int)res[q].actions.size();
-        if (ao + (int64_t)res[q].actions.size() > cap_actions) throw std::runtime_error("action capacity too small");
-        for (int a : res[q].actions) actions[ao++] = a;
-        action_offset[q + 1] = ao;
-        if (closed_keys) {
-          if (co + (int64_t)res[q].closed_keys.size() > cap_closed) throw std::runtime_error("closed capacity too small");
-          for (uint64_t k : res[q].closed_keys) closed_keys[co++] = k;
-          closed_offset[q + 1] = co;
-        }
+        s->actions.insert(s->actions.end(), res[q].actions.begin(), res[q].actions.end());
+        s->closed.insert(s->closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
+        s->aoff[q + 1] = (int64_t)s->actions.size();
+        s->coff[q + 1] = (int64_t)s->closed.size();
       }
       if (totals) {
         totals[0] = (double)mq->iterations(); totals[1] = (double)mq->nodes_expanded(); totals[2] = secs;
@@ -375,6 +410,49 @@ int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mpl
     g_err = e.what();
     return 1;
   }
+}
+
+/* Copies what the last mplh_batch_plan_keep kept: query q's action ids at actions[action_offset[q],
+ * action_offset[q+1]) and closed keys likewise with closed_offset (closed_keys NULL = skip).  A capacity
+ * that is too small fails the call with nothing written. */
+int mplh_batch_kept(void *session, int64_t *action_offset, int32_t *actions, int64_t cap_actions,
+                    int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq) {
+    g_err = "null session";
+    return 1;
+  }
+  if (!action_offset || (!actions && !s->actions.empty()) || (closed_keys && !closed_offset)) {
+    g_err = "missing output array";
+    return 1;
+  }
+  if ((int64_t)s->actions.size() > cap_actions || (closed_keys && (int64_t)s->closed.size() > cap_closed)) {
+    g_err = (int64_t)s->actions.size() > cap_actions ? "action capacity too small" : "closed capacity too small";
+    return 1;
+  }
+  std::copy(s->aoff.begin(), s->aoff.end(), action_offset);
+  std::copy(s->actions.begin(), s->actions.end(), actions);
+  if (closed_keys) {
+    std::copy(s->coff.begin(), s->coff.end(), closed_offset);
+    std::copy(s->closed.begin(), s->closed.end(), closed_keys);
+  }
+  return 0;
+}
+
+/* mplh_batch_plan that also returns every query's trajectory (action ids, query q's at
+ * actions[action_offset[q], action_offset[q+1])) and closed set (sorted lattice keys, likewise with
+ * closed_offset; closed_keys NULL = skip).  A capacity that is too small fails the call. */
+int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
+                           int max_num, mplh_query_result *out, double *totals, int64_t *action_offset, int32_t *actions,
+                           int64_t cap_actions, int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq || !action_offset || !actions || (closed_keys && !closed_offset)) {
+    g_err = !s || !s->mq ? "null session" : "missing output array";
+    return 1;
+  }
+  const int rc = mplh_batch_plan_keep(session, starts, goals, n_q, eps, max_num, closed_keys != nullptr, out, totals);
+  if (rc) return rc;
+  return mplh_batch_kept(session, action_offset, actions, cap_actions, closed_offset, closed_keys, cap_closed);
 }
 
 /* Frees the session incl. the search states it kept; seconds spent are returned in *release_seconds. */

@@ -265,6 +265,16 @@ def _host():
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                            C.c_int64]
     lib.mplh_batch_plan_detail.restype = C.c_int
+    lib.mplh_batch_plan_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_int,
+                                         C.c_void_p, C.c_void_p]
+    lib.mplh_batch_plan_keep.restype = C.c_int
+    lib.mplh_batch_kept.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64]
+    lib.mplh_batch_kept.restype = C.c_int
+    lib.mplh_batch_grow_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                          C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
+    lib.mplh_batch_grow_stats.restype = C.c_int
+    lib.mplh_batch_set_grow_caps.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
+    lib.mplh_batch_set_grow_caps.restype = C.c_int
     return lib, fn
 
 
@@ -312,16 +322,19 @@ class BatchPlanner:
     are recycled for the next (a planner that answers batch after batch allocates its state memory once).
     `args` supplies the map, the controls and the limits (its start/goal are ignored).
 
-    path: "auto" runs each query's whole A* on the device for max_num > 0 and at most 256 primitives once the
-    batch is large enough: occupancy planning (no potential map, no yaw control) with mplx_plan_batch, potential-
-    field and yaw planning with mplx_plan_batch_cost_terms; otherwise the lock-step loop.  "lockstep" always
-    runs the lock-step loop, "device" mplx_plan_batch whenever the plan allows it, "device_cost_terms"
-    mplx_plan_batch_cost_terms for every plan the cap and the control set allow.  Every path gives each query
-    the same result; the choice is a diagnostic.  The totals of plan() say which ran ("path": "device",
-    "device_cost_terms" or "lockstep")."""
+    path: "auto" runs each query's whole A* on the device for at most 256 primitives once the batch is large
+    enough: for max_num > 0 occupancy planning (no potential map, no yaw control) with mplx_plan_batch, potential-
+    field and yaw planning with mplx_plan_batch_cost_terms; for max_num <= 0 (unbounded, the reference's default)
+    every plan with mplx_plan_batch_grow; otherwise the lock-step loop.  "lockstep" always runs the lock-step
+    loop, "device" mplx_plan_batch whenever the plan allows it, "device_cost_terms" mplx_plan_batch_cost_terms
+    for every plan the cap and the control set allow, "device_grow" mplx_plan_batch_grow for every plan the
+    control set allows (the queries that outgrow its largest arena go through the lock-step loop).  Every path
+    gives each query the same result; the choice is a diagnostic.  The totals of plan() say which ran ("path":
+    "device", "device_cost_terms", "device_grow" or "lockstep"; for "device_grow" also grow_rounds,
+    grow_reruns, grow_first_cap, grow_last_cap and grow_lockstep, the queries handed to the lock-step loop)."""
 
-    PATHS = {"auto": 0, "lockstep": 1, "device": 2, "device_cost_terms": 3}
-    _RAN = {0: "lockstep", 1: "device", 2: "device_cost_terms"}
+    PATHS = {"auto": 0, "lockstep": 1, "device": 2, "device_cost_terms": 3, "device_grow": 4}
+    _RAN = {0: "lockstep", 1: "device", 2: "device_cost_terms", 3: "device_grow"}
 
     def __init__(self, args, path="auto"):
         self._lib, _ = _host()
@@ -337,36 +350,50 @@ class BatchPlanner:
         if self._lib.mplh_batch_set_path(self._h, self.PATHS[path]) != 0:
             raise RuntimeError(self._lib.mplh_last_error().decode())
 
+    def set_grow_caps(self, first_cap=0, max_cap=0):
+        """Diagnostics: the growing device search's first and largest arena capacity in records (0 = automatic;
+        see mplx_plan_batch_grow).  Queries that outgrow max_cap run through the lock-step loop."""
+        if self._lib.mplh_batch_set_grow_caps(self._h, int(first_cap), int(max_cap)) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+
     def _last_path(self):
         dev, slots, nbytes = C.c_int32(0), C.c_int32(0), C.c_int64(0)
         if self._lib.mplh_batch_last_path(self._h, C.byref(dev), C.byref(slots), C.byref(nbytes)) != 0:
             raise RuntimeError(self._lib.mplh_last_error().decode())
-        return dict(path=self._RAN[dev.value], slots=int(slots.value), arena_bytes=int(nbytes.value))
+        d = dict(path=self._RAN[dev.value], slots=int(slots.value), arena_bytes=int(nbytes.value))
+        rounds, lockstep = C.c_int32(0), C.c_int32(0)
+        reruns, first_cap, last_cap = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        if self._lib.mplh_batch_grow_stats(self._h, C.byref(rounds), C.byref(reruns), C.byref(first_cap),
+                                           C.byref(last_cap), C.byref(lockstep)) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
+        d.update(grow_rounds=int(rounds.value), grow_reruns=int(reruns.value), grow_first_cap=int(first_cap.value),
+                 grow_last_cap=int(last_cap.value), grow_lockstep=int(lockstep.value))
+        return d
 
     def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True):
         """plan() that also returns every query's trajectory (action ids) and closed set (sorted lattice keys):
-        (res, totals, actions, closed) with one array per query in actions / closed."""
+        (res, totals, actions, closed) with one array per query in actions / closed.  Any max_num, including
+        max_num <= 0 (unbounded): the outputs are sized from the results."""
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
         goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
         nq = len(starts)
         mx = self._args.max_num if max_num is None else max_num
-        if mx <= 0:
-            raise ValueError("plan_detail needs max_num > 0 (it sizes the outputs)")
         out = (QueryResult * max(nq, 1))()
         totals = np.zeros(7)
-        cap = max(1, nq * mx)
-        aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
-        acts = np.zeros(cap, np.int32)
-        keys = np.zeros(cap, np.uint64) if closed else None
-        rc = self._lib.mplh_batch_plan_detail(self._h, starts.ctypes.data, goals.ctypes.data, nq,
-                                              self._args.eps if eps is None else eps, mx, out, totals.ctypes.data,
-                                              aoff.ctypes.data, acts.ctypes.data, cap, coff.ctypes.data,
-                                              None if keys is None else keys.ctypes.data, cap if closed else 0)
-        if rc != 0:
+        if self._lib.mplh_batch_plan_keep(self._h, starts.ctypes.data, goals.ctypes.data, nq,
+                                          self._args.eps if eps is None else eps, mx, 1 if closed else 0, out,
+                                          totals.ctypes.data) != 0:
             raise RuntimeError(self._lib.mplh_last_error().decode())
         res = np.zeros(nq, dtype=_QRES)
         for q in range(nq):
             res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        na, nc = int(res["n_actions"].sum()), int(res["n_closed"].sum()) if closed else 0
+        aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
+        acts = np.zeros(max(na, 1), np.int32)
+        keys = np.zeros(max(nc, 1), np.uint64) if closed else None
+        if self._lib.mplh_batch_kept(self._h, aoff.ctypes.data, acts.ctypes.data, acts.size, coff.ctypes.data,
+                                     None if keys is None else keys.ctypes.data, 0 if keys is None else keys.size) != 0:
+            raise RuntimeError(self._lib.mplh_last_error().decode())
         tot = self._totals(totals)
         return (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
                 [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
