@@ -55,17 +55,19 @@ __device__ __forceinline__ void edge_build(const EnvParams &P, const mplx_waypoi
   PrimState<DIM, ORD, false> pr;
   const double *u = P.U + (size_t)action * P.udim;
   double max_v = 0;
+  bool nan_v = false;  // a NaN speed compares false above and would otherwise read as max_v = 0, n = 0
   J = 0;
 #pragma unroll
   for (int k = 0; k < DIM; k++) {
     pr.ax[k].build(__ldg(u + k), w.pos[k], w.vel[k], w.acc[k], w.jrk[k]);
     const double mv = pr.ax[k].max_vel(P.T);
     if (mv > max_v) max_v = mv;
+    nan_v = nan_v || mv != mv;
     J += pr.ax[k].J(P.T);  // Primitive::J sums the axes left to right (primitive.h:403-407)
   }
   fill_coef<DIM, ORD, false>(pr, false, e.cf);
   const double nd = ceil(max_v * P.T / P.res);
-  e.n = !(nd <= (double)kEdgeNMax) ? -1 : (int)nd;  // -1: more samples than any real edge has
+  e.n = (nan_v || !(nd <= (double)kEdgeNMax)) ? -1 : (int)nd;  // -1: more samples than any real edge has
   e.dt = P.T / e.n;
 }
 

@@ -160,6 +160,7 @@ extern "C" int mplx_expand_packed(mplx_ctx *c, const mplx_waypoint *nodes, int n
   };
 
   const int ahead = 2;  // chunks queued before the host waits for a record count
+  auto pipeline = [&]() -> int {
   for (int k = 0; k < nchunks; k++) {
     ChunkBufs &B = c->cb[k % kPackBufs];
     cudaStream_t st = c->cb[k & 1].st;
@@ -185,9 +186,18 @@ extern "C" int mplx_expand_packed(mplx_ctx *c, const mplx_waypoint *nodes, int n
   }
   for (int k = nchunks - ahead < 0 ? 0 : nchunks - ahead; k < nchunks; k++)
     if (int r = drain(k)) return r;
-  CU(cudaStreamSynchronize(ds));
-  CU(cudaStreamSynchronize(c->cb[0].st));
-  CU(cudaStreamSynchronize(c->cb[1].st));
+  return MPLX_OK;
+  };
+  // Every exit waits for the three streams, a refusal included: when drain() finds the capacity too small,
+  // later chunks' kernels and earlier chunks' copies into the caller's arrays are still queued, and the
+  // caller may free those arrays as soon as the call returns.
+  const int rc = pipeline();
+  const cudaError_t e_ds = cudaStreamSynchronize(ds), e_s0 = cudaStreamSynchronize(c->cb[0].st),
+                    e_s1 = cudaStreamSynchronize(c->cb[1].st);
+  if (rc) return rc;
+  CU(e_ds);
+  CU(e_s0);
+  CU(e_s1);
   // offsets were reserved per chunk: make them global
   for (int k = 1; k < nchunks; k++) {
     const int off = k * chunk;

@@ -45,6 +45,7 @@ struct Planner : MPL::MapPlanner<Dim> {
   using MPL::MapPlanner<Dim>::ss_ptr_;
   using MPL::MapPlanner<Dim>::ENV_;
   using MPL::MapPlanner<Dim>::lhm_;
+  using MPL::MapPlanner<Dim>::pow_;  // createMask's exponent: protected, no setter in the reference
 };
 
 template <int Dim>
@@ -107,8 +108,10 @@ int plan(const mplh_plan_args *a, mplh_plan_result *r, uint64_t *closed_keys, in
 }
 
 template <int Dim>
-int potential(const mplh_plan_args *a, const double *radius, const double *range, const double *pos, int8_t *out) {
+int potential(const mplh_plan_args *a, const double *radius, double pow, const double *range, const double *pos,
+              int8_t *out) {
   Planner<Dim> planner(false);
+  planner.pow_ = pow;
   auto mu = make_map<Dim>(a);
   planner.setMapUtil(mu);
   Vecf<Dim> rad, rng, p;
@@ -468,7 +471,12 @@ int refp_plan(const mplh_plan_args *a, mplh_plan_result *r, uint64_t *closed_key
 }
 int refp_update_potential_map(const mplh_plan_args *a, const double *radius, const double *range, const double *pos,
                               int8_t *out) {
-  return a->dim == 2 ? potential<2>(a, radius, range, pos, out) : potential<3>(a, radius, range, pos, out);
+  return a->dim == 2 ? potential<2>(a, radius, 1.0, range, pos, out) : potential<3>(a, radius, 1.0, range, pos, out);
+}
+// the same with createMask's exponent pow_ (1.0 in the reference unless a subclass assigns it)
+int refp_update_potential_map_pow(const mplh_plan_args *a, const double *radius, double pow, const double *range,
+                                  const double *pos, int8_t *out) {
+  return a->dim == 2 ? potential<2>(a, radius, pow, range, pos, out) : potential<3>(a, radius, pow, range, pos, out);
 }
 int refp_set_search_region(const mplh_plan_args *a, const double *path, int n_path, const double *radius, int dense,
                            uint8_t *out) {

@@ -1,7 +1,8 @@
 """SURVEY.md §8f row 2 on the device: mplx_update_potential_map = MapPlanner::updatePotentialMap,
 mplx_set_search_region_path = MapPlanner::setSearchRegion.  Bit-exact against the REFERENCE's own
 functions (oracle/_ref planner library, built from the unmodified sources, or its recorded results where
-it is not built) and against the literal numpy restatement of the stamping rule."""
+it is not built) and against the literal numpy restatement of the stamping rule
+(tests/test_maps_inputs_restatement_vs_ref.py), unknown cells included."""
 import numpy as np
 import pytest
 
@@ -28,7 +29,7 @@ def ref_args(grid, dims, origin, res):
 
 
 def test_potential_map_3d_matches_reference():
-    import scenarios as S
+    from test_maps_inputs_restatement_vs_ref import restate_potential
 
     rng = np.random.default_rng(3)
     for dims, res, rad, powv in (((40, 36, 30), 0.1, (0.5, 0.5, 0.3), 1.0), ((33, 31, 29), 0.25, (1.0, 1.0, 0.5), 1.0),
@@ -37,8 +38,7 @@ def test_potential_map_3d_matches_reference():
         g[rng.integers(0, g.size, 50)] = -1  # unknown cells stay untouched unless stamped
         origin = (-1.0, 0.5, 0.0)
         got = gpu_env(g, dims, origin, res).update_potential_map(rad, powv)
-        np.testing.assert_array_equal(got, S.potential_from_map_stencil(np.where(g > 0, g, 0).astype(np.int8), dims, res, rad, powv)
-                                      if (g >= 0).all() else got)
+        np.testing.assert_array_equal(got, restate_potential(g, dims, origin, res, rad, powv))
         same_array(got, pb.reference_potential_map(ref_args(g, dims, origin, res), rad, g.size))
 
 
