@@ -92,7 +92,9 @@ const char *mplx_last_error(void);
 /* MapUtil<Dim>::setMap (include/mpl_collision/map_util.h:85-91).  `data` is the x-fastest
  * int8 grid (occupied 100 / free 0 / unknown -1, map_util.h:309-313); it is copied to HBM.
  * dim/origin have ctx-dim entries.  Clears any potential map and search region
- * (their sizes are tied to the grid).  Edits of a few voxels of the same grid: mplx_update_cells. */
+ * (their sizes are tied to the grid).  Edits of a few voxels of the same grid: mplx_update_cells.
+ * Ordered only against the ctx's own stream: it does not wait for an expansion that
+ * mplx_expand_device still runs on a caller's stream; synchronise that stream first. */
 int mplx_set_map(mplx_ctx *ctx, const int8_t *data, const int32_t *dim, const double *origin,
                  double res);
 
@@ -103,7 +105,9 @@ int mplx_set_map(mplx_ctx *ctx, const int8_t *data, const int32_t *dim, const do
  * the edited grid.  Unlike mplx_set_map, the potential map and the search region are kept (the
  * reference env holds its own copies of both: env_map.h:181-183,290; env_base.h:301-303).
  * Synchronous, like mplx_set_map.  n == 0 is a no-op.  Any invalid argument (n < 0, a NULL array
- * with n > 0, an index outside the grid) -> MPLX_ERR_ARG with nothing applied. */
+ * with n > 0, an index outside the grid) -> MPLX_ERR_ARG with nothing applied.  Like mplx_set_map,
+ * ordered only against the ctx's own stream: an expansion still running on a caller's stream from
+ * mplx_expand_device may read the grid while it changes; synchronise that stream first. */
 int mplx_update_cells(mplx_ctx *ctx, const int32_t *idx, const int8_t *values, int n);
 
 /* Diagnostics: copy the device grid (nvox bytes), the occupancy words and the occ2 pairs
