@@ -161,11 +161,13 @@ struct UpdateBufs {
   }
 };
 
-// Device memory one mplx_plan_batch call may take (arenas and results): a quarter of the free device
-// memory, at most this much.  The slot count follows from it (mplx_search.cu, size_batch).
+// Device memory one search call may take (arenas, per-query arrays and the result pool): a quarter of the
+// free device memory, at most this much.  The slot count follows from it (mplx_search.cu, search_budget).
 constexpr size_t kSearchArenaBudget = (size_t)8 << 30;
 
-// the device search (mplx_search.cu): per-slot arenas kept across calls, per-call staging
+// the device search (mplx_search.cu): per-slot arenas kept across calls; per-slot successor scratch
+// (succ, cost, key, action, count), the per-query arrays (queries, free_, ires, dres, offs) and the
+// result pool (closed), reused by every call and round
 struct SearchBufs {
   DevBuf<unsigned char> arena;
   int64_t layout_bytes = 0;  // bytes per slot of the layout the arena was cleared for
@@ -174,18 +176,17 @@ struct SearchBufs {
   DevBuf<mplx_waypoint> succ, queries;
   DevBuf<double> cost, dres;
   DevBuf<uint64_t> key, closed;
-  DevBuf<int32_t> action, count, ires, actions;
+  DevBuf<int32_t> action, count, ires;
   DevBuf<uint8_t> free_;
-  DevBuf<unsigned long long> offs;  // mplx_plan_batch_grow: each query's place in the result pool (closed)
+  DevBuf<unsigned long long> offs;  // each query's place in the result pool, then the pool's fill counter
   // what mplx_plan_batch_grow_results copies: the last mplx_plan_batch_grow call's trajectories and
-  // sorted closed keys, query q's at [offset[q], offset[q+1])
+  // sorted closed keys, query q's at [offset[q], offset[q+1]); the other entry points leave them alone
   std::vector<int64_t> grow_aoff, grow_coff;
   std::vector<int32_t> grow_actions;
   std::vector<uint64_t> grow_closed;
   void release() {
     arena.release(); succ.release(); queries.release(); cost.release(); dres.release(); key.release();
-    closed.release(); action.release(); count.release(); ires.release(); actions.release(); free_.release();
-    offs.release();
+    closed.release(); action.release(); count.release(); ires.release(); free_.release(); offs.release();
     layout_bytes = 0;
     cleared = 0;
     next_epoch = 1;

@@ -9,21 +9,26 @@
 //   thread 0     relaxes the successors, tests the goal and the limits (mplx_search.cuh).
 // So there is no launch, no PCIe transfer and no host work per iteration.
 //
-// Two entry points share the kernel.  mplx_plan_batch serves occupancy planning only (no potential map,
-// no yaw control) with search_kernel<DIM, ORD, false, false>: the sample loop never evaluates
-// velocities.  mplx_plan_batch_cost_terms serves every plan, including potential-field, gradient and
-// yaw planning, with search_kernel<DIM, ORD, YAW, true>: the sample loop sums the potential, gradient
-// and yaw-alignment terms per sample in loop order (sample_group), as the register and dealing kernels
-// do, so the edge costs equal theirs bit for bit.
+// The occupancy search (no potential map, no yaw control) runs search_kernel<DIM, ORD, false, false>: the
+// sample loop never evaluates velocities.  The cost-term search serves every plan, including
+// potential-field, gradient and yaw planning, with search_kernel<DIM, ORD, YAW, true>: the sample loop sums
+// the potential, gradient and yaw-alignment terms per sample in loop order (sample_group), as the register
+// and dealing kernels do, so the edge costs equal theirs bit for bit.
 //
-// mplx_plan_batch_grow runs either instantiation with GROW: arenas sized for the batch rather than the worst
-// case, a query that outgrows its arena abandoned (kOverflow) and searched again in a larger one in the next
-// round, and results gathered in a device pool that is drained between rounds (include/mplx.h).
+// Every entry point searches in rounds of one launch each (run_round).  A round searches a list of queries
+// in arenas of one capacity; a query that outgrows its arena ends in kOverflow (consume<true>), and one that
+// finishes reserves room for its closed keys and actions in a device result pool, drained after the round.
+// mplx_plan_batch and mplx_plan_batch_cost_terms run one round with worst-case arenas and a pool that holds
+// every query's worst case, so none of their queries can overflow or find the pool full.  A round in
+// worst-case arenas runs the kernel without the capacity check (CHECK false), which gives the same results
+// and spills less.
+// mplx_plan_batch_grow sizes arenas for the batch and searches overflowed queries again in larger arenas
+// (include/mplx.h states its round schedule).
 #include <cuda_runtime.h>
 #include <string.h>
 
 #include <algorithm>
-#include <chrono>
+#include <numeric>
 #include <vector>
 
 #include "mplx_dispatch.h"
@@ -40,7 +45,8 @@ using namespace search;
 struct Job {
   const mplx_waypoint *starts, *goals;
   const uint8_t *start_free;  // nullptr: is_free(start.pos) on the device grid
-  int n_q, max_expand, act_stride;
+  int n_q, max_expand;
+  bool closed;  // the closed keys are stored
   double eps, tol_pos, tol_vel, tol_acc, tol_yaw;
   unsigned char *arena;
   Layout L;
@@ -51,16 +57,13 @@ struct Job {
   double *s_cost;
   uint64_t *s_key;
   int *counter;
-  // per-query results
-  int32_t *valid, *expanded, *n_closed, *n_actions, *actions;
-  double *cost;
-  uint64_t *closed;  // nullptr: skip
-  // mplx_plan_batch_grow only: the round searches queries qlist[0, n_q); query qlist[i] writes
-  // state[qlist[i]] (kDone / kOverflowed / kPoolFull) and, when done, its closed keys (with `closed` set)
-  // and then its actions into pool[offs[q], ...), reserved with one atomicAdd on *pool_used; when the pool
-  // is full, offs[q] receives the units it needed
+  // per-query results: the launch searches queries qlist[0, n_q); query q = qlist[i] writes state[q]
+  // (kDone / kOverflowed / kPoolFull) and, when done, its results, its closed keys (with `closed`) and
+  // then its actions into pool[offs[q], ...), reserved with one atomicAdd on *pool_used; when the pool is
+  // full, offs[q] receives the units it needed
   const int32_t *qlist;
-  int32_t *state;
+  int32_t *valid, *expanded, *n_closed, *n_actions, *state;
+  double *cost;
   uint64_t *pool;
   unsigned long long *pool_used, *offs;
   unsigned long long pool_cap;  // in uint64 units
@@ -69,16 +72,18 @@ enum GrowState : int32_t { kDone = 1, kOverflowed = 2, kPoolFull = 3 };
 
 // Samples per group of the cost-term sample loop; the result does not depend on the group size.  Groups
 // of 4 spill with the cost terms (as in the dealing kernel, mplx_deal.cu).  Spill stores / loads in bytes
-// under -Xptxas -v (nvcc 12.9, sm_90a) of the instantiations that spill at 2 or 1, <DIM, ORD, YAW>:
+// under -Xptxas -v (nvcc 12.9, sm_90a) of the instantiations without the capacity check that spill at 2 or 1,
+// <DIM, ORD, YAW>:
 //                      groups of 2    groups of 1
 //   <2, JRK, yaw>        52 /  76        0 /   0
-//   <2, SNP, no yaw>    164 / 260      212 / 324
-//   <2, SNP, yaw>        84 / 196       84 / 204
+//   <2, SNP, no yaw>    148 / 252      180 / 292
+//   <2, SNP, yaw>        80 / 192       80 / 200
 //   <3, ACC, no yaw>     76 / 100       52 /  76
 //   <3, ACC, yaw>        32 /  56        0 /   0
-//   <3, JRK, no yaw>      0 /   0      308 / 364
-//   <3, JRK, yaw>       196 / 316      244 / 364
-// The other 9 spill at neither.  Groups of 2: 604 B of spill stores over the 16, against 900 B at 1.
+//   <3, JRK, no yaw>      0 /   0      312 / 368
+//   <3, JRK, yaw>       164 / 292      244 / 340
+// The other 9 spill at neither.  Groups of 2: 552 B of spill stores over the 16, against 868 B at 1.  With
+// the capacity check (CHECK): 760 B at 2, against 940 B at 1.
 constexpr int kCostUnr = 2;
 
 // hash_value(waypoint) (waypoint.h:93-125) as phase A computes it for `tn == curr`: the yaw lattice id
@@ -92,9 +97,9 @@ __device__ __forceinline__ uint64_t node_hash(const mplx_waypoint *w) {
 
 // COST: the sample loop sums per-sample cost terms (potential, gradient, yaw alignment); without it the
 // kernel is the occupancy search, whose code does not carry the velocity coefficients.
-// GROW: mplx_plan_batch_grow's kernel: the arena's capacity is checked (consume<true>), the queries come
-// from J.qlist, and results go to the result pool; without it the code is mplx_plan_batch's.
-template <int DIM, int ORD, bool YAW, bool COST, bool GROW>
+// CHECK: the arena's capacity is checked (consume<true>).  A launch whose arenas hold every query's worst
+// case (layout_for) runs without it, exactly as with it, and spills less in the sample loop.
+template <int DIM, int ORD, bool YAW, bool COST, bool CHECK>
 __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant__ EnvParams P, const __grid_constant__ Job J) {
   static_assert(COST || !YAW, "a yaw control always sums cost terms");
   __shared__ mplx_waypoint s_node;
@@ -122,7 +127,7 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
       s_q = atomicAdd(J.counter, 1);
       s_status = kIdle;
       if (s_q < J.n_q) {
-        const int q = GROW ? J.qlist[s_q] : s_q;
+        const int q = J.qlist[s_q];
         A = arena_at(J.arena + (size_t)slot * J.L.bytes, J.L, J.epoch0 + (uint32_t)s_q);
         Q.w = J.goals[q];
         Q.key = node_hash<DIM, ORD, YAW>(&J.goals[q]);
@@ -167,7 +172,7 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
       }
       __syncthreads();
       if (threadIdx.x == 0) {
-        consume<GROW>(
+        consume<CHECK>(
             A, S, G, Q, o.count[0], [&](int s) { return (uint64_t)o.key[s]; }, [&](int s) { return s_cost[s]; },
             [&](int s) { return (int)o.action[s]; }, [&](int s, mplx_waypoint &w) { w = o.succ[s]; });
         if (S.status == kRunning) s_node = A.st[pop(A, S)].coord;
@@ -175,7 +180,7 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
       }
       __syncthreads();
     }
-    if (GROW && threadIdx.x == 0) {
+    if (threadIdx.x == 0) {
       const int q = J.qlist[s_q];
       if (S.status == kOverflow) {
         J.state[q] = kOverflowed;
@@ -213,44 +218,27 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
         }
       }
     }
-    if (!GROW && threadIdx.x == 0) {
-      const int q = s_q;
-      int na = 0;
-      const double c = finish(A, S, J.actions + (size_t)q * J.act_stride, J.act_stride, &na);
-      J.cost[q] = c;
-      J.valid[q] = isinf(c) ? 0 : 1;
-      J.expanded[q] = S.expanded;
-      J.n_actions[q] = na;
-      int nc = 0;
-      if (S.status != kIdle && S.status != kTrivial) {
-        for (int s = 0; s < A.n_states; s++)
-          if (A.st[s].flags & kClosed) {
-            if (J.closed && nc < J.max_expand) J.closed[(size_t)q * J.max_expand + nc] = A.st[s].key;
-            nc++;
-          }
-      }
-      J.n_closed[q] = nc;
-    }
     __syncthreads();
   }
 }
 
-// The instantiation a plan runs: <DIM, ORD, false, false> for mplx_plan_batch, <DIM, ORD, yaw bit, true>
-// for mplx_plan_batch_cost_terms, each with GROW for mplx_plan_batch_grow.  f receives the kernel's address.
-template <bool GROW = false, class F>
-cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, F &&f) {
-  return with_dim(P.dim, [&](auto DIM) {
-    return with_order(P.control, [&](auto ORD) {
-      if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, GROW>);
-      return with_bool(P.control & 16, [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, GROW>); });
+// The instantiation a plan runs: <DIM, ORD, false, false> for the occupancy search, <DIM, ORD, yaw bit,
+// true> for the cost-term search, each with the capacity check or without.  f receives the kernel's address.
+template <class F>
+cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, bool check, F &&f) {
+  return with_bool(check, [&](auto CHECK) {
+    return with_dim(P.dim, [&](auto DIM) {
+      return with_order(P.control, [&](auto ORD) {
+        if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, CHECK>);
+        return with_bool(P.control & 16, [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, CHECK>); });
+      });
     });
   });
 }
 
-template <bool GROW = false>
-int resident_ctas(const EnvParams &P, bool cost_terms, int block) {
+int resident_ctas(const EnvParams &P, bool cost_terms, bool check, int block) {
   int per_sm = 0;
-  const cudaError_t e = with_search_kernel<GROW>(P, cost_terms, [&](auto kernel) {
+  const cudaError_t e = with_search_kernel(P, cost_terms, check, [&](auto kernel) {
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
   });
   if (e != cudaSuccess) {
@@ -267,24 +255,42 @@ using namespace mplx;
 using namespace mplx::search;
 
 namespace {
-// The device memory of one search call: per-query results (n_q*max_expand action ids, and as many
-// closed keys when asked for; the queries and the per-query counters) and as many worst-case arenas as fit
-// next to them.  The budget is a quarter of the device memory free at the call, counting the search
-// buffers the ctx already holds as free (they are reused or replaced), at most kSearchArenaBudget.
-// MPLX_ERR_ALLOC, with nothing changed, when not even one arena fits.
+// Bytes of the per-query arrays of one search call: start and goal, the start-is-free flag, valid, expanded,
+// n_closed, n_actions, state and the launch's query list, the cost and the place in the result pool.
+constexpr size_t kQueryBytes =
+    2 * sizeof(mplx_waypoint) + 1 + 6 * sizeof(int32_t) + sizeof(double) + sizeof(unsigned long long);
+
+// The device memory one search call may take: a quarter of the device memory free at the call, counting the
+// arenas and the result pool the ctx already holds as free (they are reused or replaced), at most
+// kSearchArenaBudget.
+int search_budget(const SearchBufs &B, size_t &budget) {
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  const size_t held = B.arena.cap + B.closed.cap * sizeof(uint64_t);
+  budget = std::min(kSearchArenaBudget, (free_b + held) / 4);
+  return MPLX_OK;
+}
+
+// The result pool (uint64 units) of a call whose every query may take its worst case: max_expand closed keys
+// (with_closed) and max_expand action ids, two to a unit.
+int64_t worst_pool_units(int n_q, int max_expand, bool with_closed) {
+  return (int64_t)n_q * ((with_closed ? max_expand : 0) + (max_expand + 1) / 2);
+}
+
+// mplx_plan_batch*'s device memory: the per-query arrays, a result pool for every query's worst case and as
+// many worst-case arenas as fit next to them in the budget (search_budget).  MPLX_ERR_ALLOC, with nothing
+// changed, when not even one arena fits.
 int size_batch(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, bool with_closed, Layout &L,
                int64_t &slots) {
   const int nU = c->P.nU;
   L = layout_for(max_expand, nU);
   const int block = ((nU + 31) / 32) * 32;
-  size_t free_b = 0, total_b = 0;
-  CU(cudaMemGetInfo(&free_b, &total_b));
-  const SearchBufs &B = c->sb;
-  const size_t held = B.arena.cap + B.actions.cap * sizeof(int32_t) + B.closed.cap * sizeof(uint64_t);
-  const size_t budget = std::min(kSearchArenaBudget, (free_b + held) / 4);
-  const size_t per_q = (size_t)max_expand * (sizeof(int32_t) + (with_closed ? sizeof(uint64_t) : 0));
-  const size_t results = (size_t)n_q * (per_q + 2 * sizeof(mplx_waypoint) + 1 + 4 * sizeof(int32_t) + sizeof(double));
-  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, block));
+  size_t budget = 0;
+  const int rc = search_budget(c->sb, budget);
+  if (rc) return rc;
+  const size_t results =
+      (size_t)n_q * kQueryBytes + (size_t)worst_pool_units(n_q, max_expand, with_closed) * sizeof(uint64_t);
+  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, block));
   const size_t left = results < budget ? budget - results : 0;
   slots = std::min<int64_t>(slots, (int64_t)(left / (size_t)L.bytes));
   if (slots < 1)
@@ -330,6 +336,136 @@ int prepare_arenas(mplx_ctx *c, const Layout &L, int64_t slots, int64_t n_epochs
   return MPLX_OK;
 }
 
+// One search call's queries and parameters.
+struct Batch {
+  int n_q, max_expand;
+  bool cost_terms, with_closed, start_free;
+  double eps, tol_pos, tol_vel, tol_acc, tol_yaw;
+};
+
+// The per-query arrays of a call, with the queries uploaded.
+int upload(mplx_ctx *c, const mplx_waypoint *starts, const mplx_waypoint *goals, const uint8_t *start_free, int n_q) {
+  SearchBufs &B = c->sb;
+  CU(B.queries.reserve(2 * (size_t)n_q));
+  CU(B.free_.reserve((size_t)n_q));
+  CU(B.ires.reserve(6 * (size_t)n_q));
+  CU(B.dres.reserve((size_t)n_q));
+  CU(B.offs.reserve((size_t)n_q + 1));
+  CU(cudaMemcpyAsync(B.queries.p, starts, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(B.queries.p + n_q, goals, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
+  if (start_free) CU(cudaMemcpyAsync(B.free_.p, start_free, n_q, cudaMemcpyHostToDevice, c->stream));
+  return MPLX_OK;
+}
+
+// What a round gives back, indexed by query id; only the round's queries' entries are from it.
+enum RoundField { kValid = 0, kExpanded = 1, kNClosed = 2, kNActions = 3, kState = 4 };
+struct Round {
+  std::vector<int32_t> ires;  // the RoundFields, n_q of each
+  std::vector<double> cost;
+  std::vector<unsigned long long> offs;  // kDone: the query's place in pool; kPoolFull: the units it needed
+  std::vector<uint64_t> pool;            // the result pool, drained
+  float ms = 0;
+  int32_t at(RoundField f, int q) const { return ires[(size_t)f * cost.size() + q]; }
+};
+
+// One launch over the queries `qlist` in `slots` arenas of layout L with a result pool of pool_units
+// uint64: reserves the per-slot scratch and the pool, launches, and copies the results and the pool back.
+int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, const Layout &L, int64_t slots,
+              int64_t pool_units, Round &R) {
+  SearchBufs &B = c->sb;
+  const int nU = c->P.nU;
+  const int n_q = b.n_q;
+  const int64_t n = (int64_t)qlist.size();
+  int rc = prepare_arenas(c, L, slots, n);
+  if (rc) return rc;
+  CU(B.succ.reserve((size_t)slots * nU));
+  CU(B.cost.reserve((size_t)slots * nU));
+  CU(B.key.reserve((size_t)slots * nU));
+  CU(B.action.reserve((size_t)slots * nU));
+  CU(B.count.reserve((size_t)slots + 1));
+  CU(B.closed.reserve((size_t)pool_units));
+  int32_t *ql = B.ires.p + 5 * (size_t)n_q;
+  CU(cudaMemcpyAsync(ql, qlist.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemsetAsync(B.count.p + slots, 0, sizeof(int32_t), c->stream));
+  CU(cudaMemsetAsync(B.offs.p + n_q, 0, sizeof(unsigned long long), c->stream));
+
+  Job J{};
+  J.starts = B.queries.p;
+  J.goals = B.queries.p + n_q;
+  J.start_free = b.start_free ? B.free_.p : nullptr;
+  J.n_q = (int)n;
+  J.max_expand = b.max_expand;
+  J.closed = b.with_closed;
+  J.eps = b.eps;
+  J.tol_pos = b.tol_pos;
+  J.tol_vel = b.tol_vel;
+  J.tol_acc = b.tol_acc;
+  J.tol_yaw = b.tol_yaw;
+  J.arena = B.arena.p;
+  J.L = L;
+  J.epoch0 = B.next_epoch;
+  J.s_succ = B.succ.p;
+  J.s_count = B.count.p;
+  J.s_action = B.action.p;
+  J.s_cost = B.cost.p;
+  J.s_key = B.key.p;
+  J.counter = B.count.p + slots;
+  J.qlist = ql;
+  J.valid = B.ires.p;
+  J.expanded = B.ires.p + n_q;
+  J.n_closed = B.ires.p + 2 * (size_t)n_q;
+  J.n_actions = B.ires.p + 3 * (size_t)n_q;
+  J.state = B.ires.p + 4 * (size_t)n_q;
+  J.cost = B.dres.p;
+  J.pool = B.closed.p;
+  J.pool_used = B.offs.p + n_q;
+  J.offs = B.offs.p;
+  J.pool_cap = (unsigned long long)pool_units;
+  B.next_epoch += (uint32_t)n;
+
+  EnvParams P = c->P;
+  P.stats = nullptr;
+  const int block = ((nU + 31) / 32) * 32;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  CU(cudaEventCreate(&e0));
+  CU(cudaEventCreate(&e1));
+  cudaEventRecord(e0, c->stream);
+  // worst-case arenas cannot overflow: the capacity check would change nothing
+  const bool check = b.max_expand <= 0 || L.cap < 1 + (int64_t)b.max_expand * nU;
+  cudaError_t le = with_search_kernel(P, b.cost_terms, check, [&](auto kernel) {
+    kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
+    return cudaGetLastError();
+  });
+  cudaEventRecord(e1, c->stream);
+  if (le != cudaSuccess) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    cudaGetLastError();
+    return fail(MPLX_ERR_CUDA, "search kernel launch failed: %s", cudaGetErrorString(le));
+  }
+  c->launches++;
+  R.ires.resize(5 * (size_t)n_q);
+  R.cost.resize(n_q);
+  R.offs.resize(n_q);
+  unsigned long long used = 0;
+  cudaError_t ce = cudaMemcpyAsync(R.ires.data(), B.ires.p, sizeof(int32_t) * R.ires.size(), cudaMemcpyDeviceToHost, c->stream);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(R.cost.data(), B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream);
+  if (ce == cudaSuccess)
+    ce = cudaMemcpyAsync(R.offs.data(), B.offs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost, c->stream);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(&used, B.offs.p + n_q, sizeof used, cudaMemcpyDeviceToHost, c->stream);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
+  R.ms = 0;
+  if (ce == cudaSuccess) ce = cudaEventElapsedTime(&R.ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  CU(ce);
+  // the pool is drained before the next round reuses it
+  R.pool.resize((size_t)std::min<unsigned long long>(used, (unsigned long long)pool_units));
+  if (!R.pool.empty())
+    CU(cudaMemcpy(R.pool.data(), B.closed.p, sizeof(uint64_t) * R.pool.size(), cudaMemcpyDeviceToHost));
+  return MPLX_OK;
+}
+
 int plan_batch_fits(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, int with_closed,
                     int32_t *slots, int64_t *arena_bytes) {
   int rc = check_plan(c, fn, cost_terms, max_expand);
@@ -361,12 +497,11 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
     return fail(MPLX_ERR_ARG, "%s: capacities below n_q*max_expand", fn);
   rc = mplx_bind(c);
   if (rc) return rc;
-  const int nU = c->P.nU;
+  const bool with_closed = out->closed_keys != nullptr;
   Layout L;
   int64_t slots = 0;
-  rc = size_batch(c, fn, cost_terms, n_q, max_expand, out->closed_keys != nullptr, L, slots);
+  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed, L, slots);
   if (rc) return rc;
-  const int block = ((nU + 31) / 32) * 32;
   out->slots = 0;
   out->arena_bytes = 0;
   out->seconds = 0;
@@ -374,115 +509,44 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
   if (out->closed_offset) out->closed_offset[0] = 0;
   if (n_q == 0) return MPLX_OK;
 
-  SearchBufs &B = c->sb;
-  rc = prepare_arenas(c, L, slots, n_q);
+  rc = upload(c, starts, goals, start_free, n_q);
   if (rc) return rc;
-  CU(B.succ.reserve((size_t)slots * nU));
-  CU(B.cost.reserve((size_t)slots * nU));
-  CU(B.key.reserve((size_t)slots * nU));
-  CU(B.action.reserve((size_t)slots * nU));
-  CU(B.count.reserve((size_t)slots + 1));
-  CU(B.queries.reserve(2 * (size_t)n_q));
-  CU(B.free_.reserve((size_t)n_q));
-  CU(B.ires.reserve(4 * (size_t)n_q));
-  CU(B.dres.reserve((size_t)n_q));
-  CU(B.actions.reserve((size_t)n_q * max_expand));
-  if (out->closed_keys) CU(B.closed.reserve((size_t)n_q * max_expand));
-  CU(cudaMemcpyAsync(B.queries.p, starts, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(B.queries.p + n_q, goals, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
-  if (start_free) CU(cudaMemcpyAsync(B.free_.p, start_free, n_q, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemsetAsync(B.count.p + slots, 0, sizeof(int32_t), c->stream));
-
-  Job J{};
-  J.starts = B.queries.p;
-  J.goals = B.queries.p + n_q;
-  J.start_free = start_free ? B.free_.p : nullptr;
-  J.n_q = n_q;
-  J.max_expand = max_expand;
-  J.act_stride = max_expand;
-  J.eps = eps;
-  J.tol_pos = tol_pos;
-  J.tol_vel = tol_vel;
-  J.tol_acc = tol_acc;
-  J.tol_yaw = tol_yaw;
-  J.arena = B.arena.p;
-  J.L = L;
-  J.epoch0 = B.next_epoch;
-  J.s_succ = B.succ.p;
-  J.s_count = B.count.p;
-  J.s_action = B.action.p;
-  J.s_cost = B.cost.p;
-  J.s_key = B.key.p;
-  J.counter = B.count.p + slots;
-  J.valid = B.ires.p;
-  J.expanded = B.ires.p + n_q;
-  J.n_closed = B.ires.p + 2 * n_q;
-  J.n_actions = B.ires.p + 3 * n_q;
-  J.actions = B.actions.p;
-  J.cost = B.dres.p;
-  J.closed = out->closed_keys ? B.closed.p : nullptr;
-  B.next_epoch += (uint32_t)n_q;
-
-  EnvParams P = c->P;
-  P.stats = nullptr;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  cudaEventRecord(e0, c->stream);
-  cudaError_t le = with_search_kernel(P, cost_terms, [&](auto kernel) {
-    kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
-    return cudaGetLastError();
-  });
-  cudaEventRecord(e1, c->stream);
-  if (le != cudaSuccess) {
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaGetLastError();
-    return fail(MPLX_ERR_CUDA, "search kernel launch failed: %s", cudaGetErrorString(le));
-  }
-  c->launches++;
-  std::vector<int32_t> ires(4 * (size_t)n_q);
-  std::vector<int32_t> acts((size_t)n_q * max_expand);
-  cudaError_t ce = cudaMemcpyAsync(ires.data(), B.ires.p, sizeof(int32_t) * 4 * n_q, cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess) ce = cudaMemcpyAsync(out->cost, B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess)
-    ce = cudaMemcpyAsync(acts.data(), B.actions.p, sizeof(int32_t) * acts.size(), cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess && out->closed_keys)
-    ce = cudaMemcpyAsync(out->closed_keys, B.closed.p, sizeof(uint64_t) * (size_t)n_q * max_expand,
-                         cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-  float ms = 0;
-  if (ce == cudaSuccess) ce = cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  CU(ce);
-  int64_t ao = 0;
+  const Batch b{n_q, max_expand, cost_terms, with_closed, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
+  std::vector<int32_t> all(n_q);
+  std::iota(all.begin(), all.end(), 0);
+  Round R;
+  rc = run_round(c, b, all, L, slots, worst_pool_units(n_q, max_expand, with_closed), R);
+  if (rc) return rc;
+  int64_t ao = 0, co = 0;
   for (int q = 0; q < n_q; q++) {
-    out->valid[q] = ires[q];
-    out->expanded[q] = ires[n_q + q];
-    out->n_closed[q] = ires[2 * n_q + q];
-    const int na = ires[3 * n_q + q];
-    if (na < 0) return fail(MPLX_ERR_ARG, "%s: query %d: trajectory longer than max_expand", fn, q);
-    // out->actions holds at least n_q*max_expand entries and ao <= q*max_expand, so compaction is in bounds
-    memcpy(out->actions + ao, acts.data() + (size_t)q * max_expand, sizeof(int32_t) * na);
+    // worst-case arenas and pool: no query can overflow or find the pool full
+    if (R.at(kState, q) != kDone)
+      return fail(MPLX_ERR_CUDA, "%s: query %d did not fit its worst-case arena and result pool", fn, q);
+    out->valid[q] = R.at(kValid, q);
+    out->cost[q] = R.cost[q];
+    out->expanded[q] = R.at(kExpanded, q);
+    const int nc = R.at(kNClosed, q);
+    out->n_closed[q] = nc;
+    const int na = R.at(kNActions, q);
+    if (na > max_expand) return fail(MPLX_ERR_ARG, "%s: query %d: trajectory longer than max_expand", fn, q);
+    // nc = expanded <= max_expand and na <= max_expand, so the compacted outputs stay within n_q*max_expand
+    const uint64_t *keys = R.pool.data() + R.offs[q];
+    const int nk = with_closed ? nc : 0;
+    const int32_t *a = reinterpret_cast<const int32_t *>(keys + nk);
+    std::copy(a, a + na, out->actions + ao);
     ao += na;
     out->action_offset[q + 1] = ao;
-  }
-  if (out->closed_keys) {
-    // the closed set's keys sorted ascending, as mplh_plan returns them (plan_capi.hpp export_result)
-    int64_t co = 0;
-    for (int q = 0; q < n_q; q++) {
-      uint64_t *src = out->closed_keys + (size_t)q * max_expand;
-      const int nc = out->n_closed[q];
-      std::sort(src, src + nc);
-      memmove(out->closed_keys + co, src, sizeof(uint64_t) * nc);
-      co += nc;
+    if (with_closed) {
+      // the closed set's keys sorted ascending, as mplh_plan returns them (plan_capi.hpp export_result)
+      std::copy(keys, keys + nk, out->closed_keys + co);
+      std::sort(out->closed_keys + co, out->closed_keys + co + nk);
+      co += nk;
       out->closed_offset[q + 1] = co;
     }
   }
   out->slots = (int32_t)slots;
   out->arena_bytes = L.bytes;
-  out->seconds = ms * 1e-3;
+  out->seconds = R.ms * 1e-3;
   return MPLX_OK;
 }
 
@@ -522,17 +586,15 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
   const int block = ((nU + 31) / 32) * 32;
   const bool ct = cost_terms != 0;
 
-  // the budget of size_batch; the per-query arrays and the pool's automatic size come off it first
-  size_t free_b = 0, total_b = 0;
-  CU(cudaMemGetInfo(&free_b, &total_b));
+  // the per-query arrays and the pool's automatic size come off the budget first
+  size_t budget = 0;
+  rc = search_budget(c->sb, budget);
+  if (rc) return rc;
   SearchBufs &B = c->sb;
-  const size_t held = B.arena.cap + B.actions.cap * sizeof(int32_t) + B.closed.cap * sizeof(uint64_t);
-  const size_t budget = std::min(kSearchArenaBudget, (free_b + held) / 4);
-  const size_t results = (size_t)n_q * (2 * sizeof(mplx_waypoint) + 1 + 6 * sizeof(int32_t) + sizeof(double) +
-                                        sizeof(unsigned long long));
+  const size_t results = (size_t)n_q * kQueryBytes;
   const size_t pool_auto = budget / 8;
   const size_t avail = results + pool_auto < budget ? budget - results - pool_auto : 0;
-  const int64_t resident = resident_ctas<true>(c->P, ct, block);
+  const int64_t resident = resident_ctas(c->P, ct, true, block);
   int64_t cap_max = cap_fitting(1, avail);
   if (cap_max < 1)
     return fail(MPLX_ERR_ALLOC, "%s: one search arena and the results (%lld bytes) exceed the budget of %lld bytes",
@@ -577,22 +639,12 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
     return MPLX_OK;
   }
 
-  CU(B.queries.reserve(2 * (size_t)n_q));
-  CU(B.free_.reserve((size_t)n_q));
-  CU(B.ires.reserve(6 * (size_t)n_q));
-  CU(B.dres.reserve((size_t)n_q));
-  CU(B.offs.reserve((size_t)n_q + 1));
-  CU(cudaMemcpyAsync(B.queries.p, starts, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(B.queries.p + n_q, goals, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
-  if (start_free) CU(cudaMemcpyAsync(B.free_.p, start_free, n_q, cudaMemcpyHostToDevice, c->stream));
-
-  EnvParams P = c->P;
-  P.stats = nullptr;
-  std::vector<int32_t> cur(n_q), next, ires(6 * (size_t)n_q);
-  for (int q = 0; q < n_q; q++) cur[q] = q;
-  std::vector<double> dres(n_q);
-  std::vector<unsigned long long> offs(n_q);
-  std::vector<uint64_t> pool;
+  rc = upload(c, starts, goals, start_free, n_q);
+  if (rc) return rc;
+  const Batch b{n_q, max_expand, ct, with_closed != 0, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
+  std::vector<int32_t> cur(n_q), next;
+  std::iota(cur.begin(), cur.end(), 0);
+  Round R;
   double seconds = 0;
   int32_t rounds = 0;
   int64_t reruns = 0;
@@ -603,88 +655,9 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
     const int64_t slots = std::max<int64_t>(1, std::min({n, resident, (int64_t)(avail / (size_t)L.bytes)}));
     // a pool that holds the largest query that found it full: the first of them to reserve fits, so every
     // round completes at least one query
-    const int64_t units = std::max(pool_units, again_units);
-    rc = prepare_arenas(c, L, slots, n);
+    rc = run_round(c, b, cur, L, slots, std::max(pool_units, again_units), R);
     if (rc) return rc;
-    CU(B.succ.reserve((size_t)slots * nU));
-    CU(B.cost.reserve((size_t)slots * nU));
-    CU(B.key.reserve((size_t)slots * nU));
-    CU(B.action.reserve((size_t)slots * nU));
-    CU(B.count.reserve((size_t)slots + 1));
-    CU(B.closed.reserve((size_t)units));
-    int32_t *qlist = B.ires.p + 5 * (size_t)n_q;
-    CU(cudaMemcpyAsync(qlist, cur.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemsetAsync(B.count.p + slots, 0, sizeof(int32_t), c->stream));
-    CU(cudaMemsetAsync(B.offs.p + n_q, 0, sizeof(unsigned long long), c->stream));
-
-    Job J{};
-    J.starts = B.queries.p;
-    J.goals = B.queries.p + n_q;
-    J.start_free = start_free ? B.free_.p : nullptr;
-    J.n_q = (int)n;
-    J.max_expand = max_expand;
-    J.eps = eps;
-    J.tol_pos = tol_pos;
-    J.tol_vel = tol_vel;
-    J.tol_acc = tol_acc;
-    J.tol_yaw = tol_yaw;
-    J.arena = B.arena.p;
-    J.L = L;
-    J.epoch0 = B.next_epoch;
-    J.s_succ = B.succ.p;
-    J.s_count = B.count.p;
-    J.s_action = B.action.p;
-    J.s_cost = B.cost.p;
-    J.s_key = B.key.p;
-    J.counter = B.count.p + slots;
-    J.valid = B.ires.p;
-    J.expanded = B.ires.p + n_q;
-    J.n_closed = B.ires.p + 2 * (size_t)n_q;
-    J.n_actions = B.ires.p + 3 * (size_t)n_q;
-    J.state = B.ires.p + 4 * (size_t)n_q;
-    J.cost = B.dres.p;
-    J.closed = with_closed ? B.closed.p : nullptr;  // only read as a flag here: keys go to the pool
-    J.qlist = qlist;
-    J.pool = B.closed.p;
-    J.pool_used = B.offs.p + n_q;
-    J.offs = B.offs.p;
-    J.pool_cap = (unsigned long long)units;
-    B.next_epoch += (uint32_t)n;
-
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    cudaEventRecord(e0, c->stream);
-    cudaError_t le = with_search_kernel<true>(P, ct, [&](auto kernel) {
-      kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
-      return cudaGetLastError();
-    });
-    cudaEventRecord(e1, c->stream);
-    if (le != cudaSuccess) {
-      cudaEventDestroy(e0);
-      cudaEventDestroy(e1);
-      cudaGetLastError();
-      return fail(MPLX_ERR_CUDA, "search kernel launch failed: %s", cudaGetErrorString(le));
-    }
-    c->launches++;
-    unsigned long long used = 0;
-    cudaError_t ce = cudaMemcpyAsync(ires.data(), B.ires.p, sizeof(int32_t) * 5 * n_q, cudaMemcpyDeviceToHost, c->stream);
-    if (ce == cudaSuccess) ce = cudaMemcpyAsync(dres.data(), B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream);
-    if (ce == cudaSuccess)
-      ce = cudaMemcpyAsync(offs.data(), B.offs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost, c->stream);
-    if (ce == cudaSuccess)
-      ce = cudaMemcpyAsync(&used, B.offs.p + n_q, sizeof used, cudaMemcpyDeviceToHost, c->stream);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-    float ms = 0;
-    if (ce == cudaSuccess) ce = cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    CU(ce);
-    // the pool is drained before the next round reuses it
-    pool.resize((size_t)std::min<unsigned long long>(used, (unsigned long long)units));
-    if (!pool.empty())
-      CU(cudaMemcpy(pool.data(), B.closed.p, sizeof(uint64_t) * pool.size(), cudaMemcpyDeviceToHost));
-    seconds += ms * 1e-3;
+    seconds += R.ms * 1e-3;
     if (rounds == 0) {
       out->slots = (int32_t)slots;
       out->arena_bytes = L.bytes;
@@ -695,22 +668,22 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
     std::vector<int32_t> again;  // the result pool was full: the same capacity again
     again_units = 0;
     for (const int32_t q : cur) {
-      const int32_t st = ires[4 * (size_t)n_q + q];
+      const int32_t st = R.at(kState, q);
       if (st == kDone) {
-        out->valid[q] = ires[q];
-        out->expanded[q] = ires[(size_t)n_q + q];
-        out->n_closed[q] = ires[2 * (size_t)n_q + q];
-        out->n_actions[q] = ires[3 * (size_t)n_q + q];
-        out->cost[q] = dres[q];
+        out->valid[q] = R.at(kValid, q);
+        out->expanded[q] = R.at(kExpanded, q);
+        out->n_closed[q] = R.at(kNClosed, q);
+        out->n_actions[q] = R.at(kNActions, q);
+        out->cost[q] = R.cost[q];
         out->searched[q] = 1;
-        const uint64_t *k = pool.data() + offs[q];
+        const uint64_t *k = R.pool.data() + R.offs[q];
         const size_t nk = with_closed ? (size_t)out->n_closed[q] : 0;
         keys[q].assign(k, k + nk);
         const int32_t *a = reinterpret_cast<const int32_t *>(k + nk);
         acts[q].assign(a, a + out->n_actions[q]);
       } else if (st == kPoolFull) {
         again.push_back(q);
-        again_units = std::max(again_units, (int64_t)offs[q]);
+        again_units = std::max(again_units, (int64_t)R.offs[q]);
       } else if (cap < cap_max) {
         next.push_back(q);
       }  // overflowed at the largest capacity: searched stays 0

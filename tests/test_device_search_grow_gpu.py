@@ -367,6 +367,38 @@ def test_one_ctx_alternating_entry_points_equals_fresh_ctx():
         e.close()
 
 
+def _grow_results(e, n, n_actions, n_closed):
+    aoff, coff = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+    acts, keys = np.zeros(max(n_actions, 1), np.int32), np.zeros(max(n_closed, 1), np.uint64)
+    abi.check(e._lib.mplx_plan_batch_grow_results(e._h, aoff.ctypes.data, acts.ctypes.data, acts.size,
+                                                  coff.ctypes.data, keys.ctypes.data, keys.size))
+    return aoff, acts, coff, keys
+
+
+def test_bounded_calls_leave_the_grow_results_alone():
+    """mplx_plan_batch and mplx_plan_batch_cost_terms search through the same device result pool as
+    mplx_plan_batch_grow, but mplx_plan_batch_grow_results keeps returning the last grow call's results."""
+    c = walled_corridor()
+    S, G = corridor_pairs(c, 10, seed=43, n_unreachable=1)
+    e = corridor_env(c)
+    try:
+        g = e.plan_batch_grow(S, G, first_cap=256)
+        na, nc = sum(map(len, g["actions"])), sum(map(len, g["closed"]))
+        before = _grow_results(e, len(S), na, nc)
+        assert np.array_equal(before[1][:na], np.concatenate(g["actions"]))
+        assert np.array_equal(before[3][:nc], np.concatenate(g["closed"]))
+        # other queries, so that the bounded calls fill the pool with other keys and actions
+        S2, G2 = corridor_pairs(c, 24, seed=44)
+        b = e.plan_batch(S2, G2, max_expand=400)
+        ct = e.plan_batch_cost_terms(S2[::-1], G2[::-1], max_expand=150)
+        assert b["n_closed"].sum() > 0 and ct["n_closed"].sum() > 0
+        after = _grow_results(e, len(S), na, nc)
+        for x, y in zip(before, after):
+            assert np.array_equal(x, y)
+    finally:
+        e.close()
+
+
 # ---- refusals ----------------------------------------------------------------------------------------------
 def _raw_out(n):
     arrs = dict(valid=np.full(n, -9, np.int32), cost=np.full(n, -9.0), expanded=np.full(n, -9, np.int32),

@@ -71,9 +71,11 @@ def layout_for(max_expand, nU):
 
 
 def results_bytes(n_q, max_expand, with_closed):
-    """size_batch: the per-query results a call holds next to its arenas."""
-    per_q = max_expand * (4 + (8 if with_closed else 0))
-    return n_q * (per_q + 2 * WAYPOINT_BYTES + 1 + 4 * 4 + 8)
+    """size_batch: the per-query arrays (start, goal, start-is-free flag, five int32 results and the query list,
+    the cost, the pool offset) and the result pool (every query's worst case: max_expand closed keys when asked
+    for, max_expand int32 action ids two to a uint64) a call holds next to its arenas."""
+    pool_units = n_q * ((max_expand if with_closed else 0) + (max_expand + 1) // 2)
+    return n_q * (2 * WAYPOINT_BYTES + 1 + 6 * 4 + 8 + 8) + 8 * pool_units
 
 
 class ArenaModel:
