@@ -362,6 +362,45 @@ int mplx_plan_batch_grow(mplx_ctx *ctx, int cost_terms, const mplx_waypoint *sta
 int mplx_plan_batch_grow_results(mplx_ctx *ctx, int64_t *action_offset, int32_t *actions, int64_t action_capacity,
                                  int64_t *closed_offset, uint64_t *closed_keys, int64_t closed_capacity);
 
+/* ---- trajectories through waypoints (TrajSolver) ----------------------------------------------- */
+
+/* Results of mplx_traj_solve (HOST arrays).  Path p owns the waypoint slots [offset[p], offset[p+1]); segment j
+ * of path p (j < n_wp(p) - 1) is at slot offset[p] + j, and the path's last slot holds zeros. */
+typedef struct {
+  int32_t *status;  /* [n_paths] 1: at least 2 waypoints and every coefficient finite; else 0                 */
+  double *seg_t;    /* [n_wp] segment duration (the given dts, or |p_j+1 - p_j|_inf / v)                     */
+  double *coeff;    /* [n_wp*(dim+1)*6] Primitive1D coefficients, highest order first, axes x, y, (z), yaw:
+                       what the segment's Primitive holds after TrajSolver::solve                           */
+  double *samples;  /* NULL, or [n_paths*(n_samples+1)*(4*dim+3)] Trajectory::sample(n_samples) rows
+                       {pos, vel, acc, jrk, yaw, yaw_dot, t}; zeros for status-0 paths                       */
+  double seconds;   /* out: device time of the kernels (CUDA events)                                        */
+} mplx_traj_out;
+
+/* TrajSolver<Dim>(control, yaw_control) (include/mpl_traj_solver/traj_solver.h) for n_paths independent paths
+ * on the device: the piecewise polynomial through each path's waypoints that minimises the integral of the
+ * squared velocity (VEL), acceleration (ACC) or jerk (JRK) — with or without YAW, the yaw axis from its own
+ * pass — for Dim = the ctx's dimension.  No map or parameters are needed.
+ *   wp_control NULL: setPath — only wps[].pos is read; the endpoints take `control`, the interior waypoints
+ *     VEL (position fixed), every other derivative and the yaw are 0.
+ *   wp_control given: setWaypoints — waypoint i fixes the derivatives its flags wp_control[i] name (use_pos,
+ *     use_vel, use_acc below the solver's order) at wps[i].pos / vel / acc; the yaw pass reads wps[i].yaw.
+ *   The yaw pass fixes the yaw at every waypoint, and at the endpoints also the derivatives yaw_control names
+ *     (as 0).
+ *   dts NULL: segment times |p_j+1 - p_j|_inf / v (TrajSolver::allocate_time); else dts[offset[p] + j] is
+ *     segment j's duration ([n_wp] slots as the outputs).
+ * Each path is what the host TrajSolver gives, within floating-point rounding: the reference's dense
+ * (S*N) x (S*N) formulation becomes one O(S) block-tridiagonal Cholesky sweep per path.  Two waypoints with
+ * free derivatives leave those at 0; a zero-length or non-finite segment time gives status 0.  The samples
+ * are the host Trajectory's sample(n_samples) of seg_t and coeff bit for bit.  Each path's outputs do not
+ * depend on the other paths of the batch.  Scratch is sized from the batch and kept in the ctx.
+ * Refusals, each with MPLX_ERR_ARG, the outputs untouched and no launch: control not VEL / ACC / JRK (with
+ * or without YAW; SNP has no solver in the reference), yaw_control not VEL / ACC / JRK, dts NULL with
+ * v <= 0, n_paths < 0, offset NULL, offset[0] != 0 or decreasing, out / status / seg_t / coeff NULL, wps NULL
+ * with waypoints, and samples given with n_samples <= 0.  Synchronous. */
+int mplx_traj_solve(mplx_ctx *ctx, int n_paths, const int64_t *offset, const mplx_waypoint *wps,
+                    const uint8_t *wp_control, const double *dts, double v, int control, int yaw_control,
+                    int n_samples, mplx_traj_out *out);
+
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field
  * planning once a batch fills the GPU, else the register kernel),

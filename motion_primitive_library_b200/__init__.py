@@ -6,5 +6,6 @@ path (benchmark input generators live in scenarios.py at the repository root).
 """
 from . import abi  # noqa: F401
 from .env import Expansion, MapUtil, env_map  # noqa: F401
+from .traj import TrajSolverBatch  # noqa: F401
 
-__all__ = ["abi", "env_map", "MapUtil", "Expansion"]
+__all__ = ["abi", "env_map", "MapUtil", "Expansion", "TrajSolverBatch"]

@@ -51,6 +51,7 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_cost_terms_fits",
     "mplx_plan_batch_grow",
     "mplx_plan_batch_grow_results",
+    "mplx_traj_solve",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -135,6 +136,18 @@ class GrowOut(C.Structure):
     ]
 
 
+class TrajOut(C.Structure):
+    """mplx_traj_out"""
+
+    _fields_ = [
+        ("status", C.c_void_p),
+        ("seg_t", C.c_void_p),
+        ("coeff", C.c_void_p),
+        ("samples", C.c_void_p),
+        ("seconds", C.c_double),
+    ]
+
+
 class MplxError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libmplx error {code}: {msg}")
@@ -206,6 +219,8 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch_grow.restype = i32
     lib.mplx_plan_batch_grow_results.argtypes = [vp, vp, vp, i64, vp, vp, i64]
     lib.mplx_plan_batch_grow_results.restype = i32
+    lib.mplx_traj_solve.argtypes = [vp, i32, vp, vp, vp, vp, f64, i32, i32, i32, C.POINTER(TrajOut)]
+    lib.mplx_traj_solve.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

@@ -161,6 +161,19 @@ struct UpdateBufs {
   }
 };
 
+// inputs, outputs and per-waypoint scratch of mplx_traj_solve (mplx_traj.cu), sized by the largest batch so far
+struct TrajBufs {
+  DevBuf<long long> offset;
+  DevBuf<mplx_waypoint> wps;
+  DevBuf<uint8_t> ctl, mono;
+  DevBuf<int32_t> status;
+  DevBuf<double> dts, seg_t, taus, coeff, samples, fac, dpos, dyaw;
+  void release() {
+    offset.release(); wps.release(); ctl.release(); mono.release(); status.release(); dts.release(); seg_t.release();
+    taus.release(); coeff.release(); samples.release(); fac.release(); dpos.release(); dyaw.release();
+  }
+};
+
 // Device memory one search call may take (arenas, per-query arrays and the result pool): a quarter of the
 // free device memory, at most this much.  The slot count follows from it (mplx_search.cu, search_budget).
 constexpr size_t kSearchArenaBudget = (size_t)8 << 30;
@@ -226,6 +239,7 @@ struct mplx_ctx {
   EdgeBufs eb;
   UpdateBufs ub;
   SearchBufs sb;
+  TrajBufs tb;
   int64_t launches = 0;
   unsigned long long last_stats[2] = {0, 0};
 };

@@ -1,0 +1,611 @@
+// mplx_traj.cu — TrajSolver for batches of paths (mplx_traj_solve, include/mplx.h).
+//
+// The reference (src/mpl_traj_solver/poly_solver.cpp) assembles dense (S*N) x (S*N) matrices for a path of S
+// segments and LU-factors them.  Here each path is solved in O(S): the cost of segment i in the derivatives at
+// its two end waypoints is H_i = tau^(1-2R) * Sc * Hbar * Sc, Sc = diag(tau^k), with Hbar a constant 2h x 2h
+// matrix per order (h = N/2 = R), so the system in the free derivatives is block-tridiagonal in waypoint order
+// with h x h blocks.  Fixed derivatives take a unit row and column, which keeps every block h x h; one block
+// Cholesky sweep per path solves it.
+//   traj_sweep_kernel   one thread per path: segment times, the running sum of them, the sweep (axes, then yaw)
+//   traj_coeff_kernel   one thread per segment: Primitive1D coefficients from the end-point derivatives
+//   traj_sample_kernel  one thread per sample: Trajectory::sample(N) of those coefficients, in the host's
+//                       operand order (include/mpl_basis/trajectory.h:100-137, primitive.h:128-145)
+#include <algorithm>
+
+#include "mplx_internal.h"
+
+namespace mplx {
+namespace {
+
+constexpr double kPi = 3.14159265358979323846;
+
+// Hbar for h = 1, 2, 3: the cost of a unit-duration segment in [start derivatives (h), end derivatives (h)]
+__constant__ double kHbar1[4] = {1, -1, -1, 1};
+__constant__ double kHbar2[16] = {12, 6, -12, 6, 6, 4, -6, 2, -12, -6, 12, -6, 6, 2, -6, 4};
+__constant__ double kHbar3[36] = {720,  360,  60,  -720, 360,  -60, 360,  192, 36, -360, 168, -24,
+                                  60,   36,   9,   -60,  24,   -3,  -720, -360, -60, 720, -360, 60,
+                                  360,  168,  24,  -360, 192,  -36, -60,  -24, -3, 60,   -36,  9};
+// inverse of B(k, m) = (h+m)! / (h+m-k)!: the top h coefficients (scaled by tau^(h+m)) from the end derivatives
+__constant__ double kBinv2[4] = {3, -1, -2, 1};
+__constant__ double kBinv3[9] = {10, -4, 0.5, -15, 7, -1, 6, -3, 0.5};
+
+template <int H>
+__device__ __forceinline__ double hbar(int a, int b) {
+  if (H == 1) return kHbar1[a * 2 + b];
+  if (H == 2) return kHbar2[a * 4 + b];
+  return kHbar3[a * 6 + b];
+}
+template <int H>
+__device__ __forceinline__ double binv(int a, int b) {
+  if (H == 1) return 1.0;
+  if (H == 2) return kBinv2[a * 2 + b];
+  return kBinv3[a * 3 + b];
+}
+
+// Which derivatives of waypoint j are fixed and their values, for the axes pass (YAW false) or the yaw pass.
+struct PathIn {
+  const mplx_waypoint *w;  // the path's waypoints
+  const uint8_t *ctl;      // per-waypoint control (setWaypoints), or NULL (setPath)
+  int end_ctl;             // the endpoints' control: `control` (axes, setPath) or `yaw_control` (yaw)
+  int W;
+  bool yaw;
+  __device__ int flags(int j, int H) const {
+    const bool end = j == 0 || j == W - 1;
+    const int c = (!yaw && ctl) ? ctl[j] : (end ? end_ctl : MPLX_VEL);
+    return c & ((1 << H) - 1);  // use_pos, use_vel, use_acc: bit k fixes derivative k
+  }
+  __device__ double val(int j, int k, int a) const {
+    if (yaw) return (k == 0 && ctl) ? w[j].yaw : 0.0;
+    if (k == 0) return w[j].pos[a];
+    if (!ctl) return 0.0;
+    return k == 1 ? w[j].vel[a] : w[j].acc[a];
+  }
+};
+
+// The blocks of H_i for duration tau: ss = [start, start], se = [start, end], ee = [end, end].
+template <int H>
+__device__ __forceinline__ void seg_blocks(double tau, double (&ss)[H][H], double (&se)[H][H], double (&ee)[H][H]) {
+  double tp[H];
+  tp[0] = 1.0;
+#pragma unroll
+  for (int k = 1; k < H; k++) tp[k] = tp[k - 1] * tau;
+  double t2r = tau;  // tau^(2R-1)
+#pragma unroll
+  for (int k = 1; k < 2 * H - 1; k++) t2r *= tau;
+#pragma unroll
+  for (int a = 0; a < H; a++)
+#pragma unroll
+    for (int b = 0; b < H; b++) {
+      const double s = tp[a] * tp[b] / t2r;
+      ss[a][b] = hbar<H>(a, b) * s;
+      se[a][b] = hbar<H>(a, H + b) * s;
+      ee[a][b] = hbar<H>(H + a, H + b) * s;
+    }
+}
+
+// Cholesky factor of an SPD H x H matrix, lower triangle packed row by row (H(H+1)/2 <= 6 entries).
+template <int H>
+__device__ __forceinline__ void chol(const double (&K)[H][H], double (&L)[6]) {
+#pragma unroll
+  for (int i = 0; i < H; i++)
+#pragma unroll
+    for (int j = 0; j <= i; j++) {
+      double s = K[i][j];
+#pragma unroll
+      for (int k = 0; k < j; k++) s -= L[i * (i + 1) / 2 + k] * L[j * (j + 1) / 2 + k];
+      L[i * (i + 1) / 2 + j] = i == j ? sqrt(s) : s / L[j * (j + 1) / 2 + j];
+    }
+}
+// x := (L L^T)^-1 x
+template <int H>
+__device__ __forceinline__ void chol_solve(const double (&L)[6], double (&x)[H]) {
+#pragma unroll
+  for (int i = 0; i < H; i++) {
+#pragma unroll
+    for (int k = 0; k < i; k++) x[i] -= L[i * (i + 1) / 2 + k] * x[k];
+    x[i] /= L[i * (i + 1) / 2 + i];
+  }
+#pragma unroll
+  for (int i = H - 1; i >= 0; i--) {
+#pragma unroll
+    for (int k = i + 1; k < H; k++) x[i] -= L[k * (k + 1) / 2 + i] * x[k];
+    x[i] /= L[i * (i + 1) / 2 + i];
+  }
+}
+
+// Minimises sum_i d_i^T H_i d_i over the free derivatives of one path (W >= 2) for NC columns (axes) and writes
+// every waypoint's derivatives to D[j*H*NC + k*NC + a]; fac holds W packed Cholesky factors.  Two waypoints
+// solve nothing: their free derivatives are 0 (PolySolver, poly_solver.cpp:205).
+template <int H, int NC>
+__device__ void sweep(const PathIn &in, const double *seg_t, double *fac, double *D) {
+  const int W = in.W;
+  constexpr int HN = H * NC;
+  if (W > 2) {
+    double yp[H][NC], Lp[6], sep[H][H], eep[H][H];
+    int fmp = 0;
+    for (int j = 0; j < W; j++) {
+      const int fm = in.flags(j, H);
+      double K[H][H], b[H][NC], ss[H][H], se[H][H], ee[H][H];
+#pragma unroll
+      for (int r = 0; r < H; r++) {
+#pragma unroll
+        for (int c = 0; c < H; c++) K[r][c] = j > 0 ? eep[r][c] : 0.0;
+#pragma unroll
+        for (int a = 0; a < NC; a++) b[r][a] = 0.0;
+      }
+      if (j < W - 1) {
+        seg_blocks<H>(seg_t[j], ss, se, ee);
+#pragma unroll
+        for (int r = 0; r < H; r++)
+#pragma unroll
+          for (int c = 0; c < H; c++) K[r][c] += ss[r][c];
+      }
+      // right-hand side: what the fixed derivatives of waypoints j-1, j, j+1 contribute to the free rows
+      const int fmn = j < W - 1 ? in.flags(j + 1, H) : 0;
+#pragma unroll
+      for (int c = 0; c < H; c++)
+#pragma unroll
+        for (int a = 0; a < NC; a++) {
+          if ((fm >> c) & 1) {
+            const double f = in.val(j, c, a);
+#pragma unroll
+            for (int r = 0; r < H; r++) b[r][a] -= K[r][c] * f;
+          }
+          if (j > 0 && ((fmp >> c) & 1)) {
+            const double f = in.val(j - 1, c, a);
+#pragma unroll
+            for (int r = 0; r < H; r++) b[r][a] -= sep[c][r] * f;
+          }
+          if (j < W - 1 && ((fmn >> c) & 1)) {
+            const double f = in.val(j + 1, c, a);
+#pragma unroll
+            for (int r = 0; r < H; r++) b[r][a] -= se[r][c] * f;
+          }
+        }
+      // fixed rows and columns become unit ones
+#pragma unroll
+      for (int r = 0; r < H; r++)
+        if ((fm >> r) & 1) {
+#pragma unroll
+          for (int c = 0; c < H; c++) K[r][c] = K[c][r] = 0.0;
+          K[r][r] = 1.0;
+#pragma unroll
+          for (int a = 0; a < NC; a++) b[r][a] = in.val(j, r, a);
+        }
+      if (j > 0) {
+        // Schur complement of the previous block: K -= Kjm C^-1 Kjm^T, b -= Kjm C^-1 y, Kjm = K_{j,j-1} masked
+        double Z[H][H];  // Z[:, r] = C^-1 Kjm[r, :]^T
+#pragma unroll
+        for (int r = 0; r < H; r++) {
+          double z[H];
+#pragma unroll
+          for (int c = 0; c < H; c++) z[c] = ((fm >> r) & 1) || ((fmp >> c) & 1) ? 0.0 : sep[c][r];
+          chol_solve<H>(Lp, z);
+#pragma unroll
+          for (int c = 0; c < H; c++) Z[c][r] = z[c];
+        }
+#pragma unroll
+        for (int r = 0; r < H; r++) {
+          if ((fm >> r) & 1) continue;
+#pragma unroll
+          for (int s = 0; s < H; s++) {
+            double acc = 0.0;
+#pragma unroll
+            for (int c = 0; c < H; c++) acc += (((fmp >> c) & 1) ? 0.0 : sep[c][r]) * Z[c][s];
+            K[r][s] -= acc;
+          }
+#pragma unroll
+          for (int a = 0; a < NC; a++) {
+            double acc = 0.0;
+#pragma unroll
+            for (int c = 0; c < H; c++) acc += Z[c][r] * yp[c][a];
+            b[r][a] -= acc;
+          }
+        }
+      }
+      double L[6] = {0, 0, 0, 0, 0, 0};
+      chol<H>(K, L);
+#pragma unroll
+      for (int q = 0; q < 6; q++) fac[(size_t)j * 6 + q] = Lp[q] = L[q];
+#pragma unroll
+      for (int r = 0; r < H; r++)
+#pragma unroll
+        for (int a = 0; a < NC; a++) D[(size_t)j * HN + r * NC + a] = yp[r][a] = b[r][a];
+#pragma unroll
+      for (int r = 0; r < H; r++)
+#pragma unroll
+        for (int c = 0; c < H; c++) { sep[r][c] = se[r][c]; eep[r][c] = ee[r][c]; }
+      fmp = fm;
+    }
+    // back substitution: x_j = C_j^-1 (y_j - K_{j,j+1} x_{j+1}), K_{j,j+1} masked
+    double xn[H][NC];
+    int fmn = 0;
+    for (int j = W - 1; j >= 0; j--) {
+      const int fm = in.flags(j, H);
+      double Lj[6];
+#pragma unroll
+      for (int q = 0; q < 6; q++) Lj[q] = fac[(size_t)j * 6 + q];
+      double rhs[H][NC];
+#pragma unroll
+      for (int r = 0; r < H; r++)
+#pragma unroll
+        for (int a = 0; a < NC; a++) rhs[r][a] = D[(size_t)j * HN + r * NC + a];
+      if (j < W - 1) {
+        double ss[H][H], se[H][H], ee[H][H];
+        seg_blocks<H>(seg_t[j], ss, se, ee);
+#pragma unroll
+        for (int r = 0; r < H; r++) {
+          if ((fm >> r) & 1) continue;
+#pragma unroll
+          for (int c = 0; c < H; c++) {
+            if ((fmn >> c) & 1) continue;
+#pragma unroll
+            for (int a = 0; a < NC; a++) rhs[r][a] -= se[r][c] * xn[c][a];
+          }
+        }
+      }
+#pragma unroll
+      for (int a = 0; a < NC; a++) {
+        double x[H];
+#pragma unroll
+        for (int r = 0; r < H; r++) x[r] = rhs[r][a];
+        chol_solve<H>(Lj, x);
+#pragma unroll
+        for (int r = 0; r < H; r++) xn[r][a] = x[r];
+      }
+#pragma unroll
+      for (int r = 0; r < H; r++)
+#pragma unroll
+        for (int a = 0; a < NC; a++) D[(size_t)j * HN + r * NC + a] = xn[r][a];
+      fmn = fm;
+    }
+  }
+  // fixed derivatives are the given values exactly; with two waypoints the free ones are 0
+  for (int j = 0; j < W; j++) {
+    const int fm = in.flags(j, H);
+#pragma unroll
+    for (int r = 0; r < H; r++)
+#pragma unroll
+      for (int a = 0; a < NC; a++)
+        if ((fm >> r) & 1) D[(size_t)j * HN + r * NC + a] = in.val(j, r, a);
+        else if (W == 2) D[(size_t)j * HN + r * NC + a] = 0.0;
+  }
+}
+
+struct TrajArgs {
+  int n_paths;
+  const long long *offset;
+  const mplx_waypoint *wps;
+  const uint8_t *ctl;
+  const double *dts;
+  double v;
+  int control, yaw_control, n_samples;
+  int32_t *status;
+  uint8_t *mono;  // per path: the running sum of segment times never decreases
+  double *seg_t, *taus, *coeff, *samples;
+  double *fac, *dpos, *dyaw;  // scratch: [n_wp*6], [n_wp*H*DIM], [n_wp*HY]
+};
+
+template <int DIM, int H, int HY>
+__global__ void __launch_bounds__(128) traj_sweep_kernel(TrajArgs A) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int W = (int)(A.offset[p + 1] - b);
+  const mplx_waypoint *w = A.wps + b;
+  double *seg_t = A.seg_t + b, *taus = A.taus + b;
+  // segment times (given, or TrajSolver::allocate_time: |p_j+1 - p_j|_inf / v) and their running sum, as
+  // Trajectory's constructor adds them (trajectory.h:48-54)
+  bool mono = true;
+  if (W > 0) taus[0] = 0.0;
+  for (int j = 0; j + 1 < W; j++) {
+    double t;
+    if (A.dts) {
+      t = A.dts[b + j];
+    } else {
+      double d = 0.0;
+#pragma unroll
+      for (int a = 0; a < DIM; a++) {
+        const double x = fabs(w[j + 1].pos[a] - w[j].pos[a]);
+        if (x > d) d = x;
+      }
+      t = d / A.v;
+    }
+    seg_t[j] = t;
+    taus[j + 1] = t + taus[j];
+    mono = mono && taus[j + 1] >= taus[j];
+  }
+  if (W > 0) seg_t[W - 1] = 0.0;
+  A.status[p] = W >= 2 ? 1 : 0;
+  A.mono[p] = mono ? 1 : 0;
+  if (W < 2) return;
+  const uint8_t *ctl = A.ctl ? A.ctl + b : nullptr;
+  const PathIn pin{w, ctl, A.control, W, false};
+  sweep<H, DIM>(pin, seg_t, A.fac + b * 6, A.dpos + b * H * DIM);
+  const PathIn yin{w, ctl, A.yaw_control, W, true};
+  sweep<HY, 1>(yin, seg_t, A.fac + b * 6, A.dyaw + b * HY);
+}
+
+__device__ __forceinline__ int path_of(const long long *offset, int n_paths, long long slot) {
+  int lo = 0, hi = n_paths - 1;  // the last path p with offset[p] <= slot
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offset[mid] <= slot) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Coefficients of one axis of one segment from the derivatives d0 (start) and d1 (end), as Primitive1D holds them
+// (c[5-k] = k! p_k, p_k the coefficient of t^k).
+template <int H>
+__device__ __forceinline__ void seg_coeff(double tau, const double (&d0)[H], const double (&d1)[H], double *c) {
+#pragma unroll
+  for (int k = 0; k < 6; k++) c[k] = 0.0;
+  double tp[2 * H];
+  tp[0] = 1.0;
+#pragma unroll
+  for (int k = 1; k < 2 * H; k++) tp[k] = tp[k - 1] * tau;
+  double t[H];  // tau^k (d1_k - sum_{n=k}^{h-1} d0_n tau^(n-k) / (n-k)!)
+#pragma unroll
+  for (int k = 0; k < H; k++) {
+    double r = d1[k];
+    double f = 1.0;
+#pragma unroll
+    for (int n = k; n < H; n++) {
+      if (n > k) f *= (double)(n - k);
+      r -= d0[n] * tp[n - k] / f;
+    }
+    t[k] = tp[k] * r;
+  }
+  double fact = 1.0;
+#pragma unroll
+  for (int k = 0; k < 2 * H; k++) {
+    if (k > 0) fact *= (double)k;
+    if (k < H) {
+      c[5 - k] = d0[k];
+    } else {
+      double q = 0.0;
+#pragma unroll
+      for (int m = 0; m < H; m++) q += binv<H>(k - H, m) * t[m];
+      c[5 - k] = q / tp[k] * fact;
+    }
+  }
+}
+
+template <int DIM, int H, int HY>
+__global__ void __launch_bounds__(128) traj_coeff_kernel(TrajArgs A, long long n_wp) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n_wp; s += (long long)gridDim.x * blockDim.x) {
+    const int p = path_of(A.offset, A.n_paths, s);
+    const long long b = A.offset[p];
+    const int W = (int)(A.offset[p + 1] - b), j = (int)(s - b);
+    double *c = A.coeff + s * (DIM + 1) * 6;
+    if (j + 1 >= W) {  // the last slot of a path has no segment
+      for (int k = 0; k < (DIM + 1) * 6; k++) c[k] = 0.0;
+      continue;
+    }
+    const double tau = A.seg_t[s];
+    bool finite = true;
+#pragma unroll
+    for (int a = 0; a < DIM; a++) {
+      double d0[H], d1[H];
+#pragma unroll
+      for (int k = 0; k < H; k++) {
+        d0[k] = A.dpos[s * H * DIM + k * DIM + a];
+        d1[k] = A.dpos[(s + 1) * H * DIM + k * DIM + a];
+      }
+      seg_coeff<H>(tau, d0, d1, c + a * 6);
+    }
+    {
+      double d0[HY], d1[HY];
+#pragma unroll
+      for (int k = 0; k < HY; k++) {
+        d0[k] = A.dyaw[s * HY + k];
+        d1[k] = A.dyaw[(s + 1) * HY + k];
+      }
+      seg_coeff<HY>(tau, d0, d1, c + DIM * 6);
+    }
+    for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+    if (!finite) A.status[p] = 0;
+  }
+}
+
+// include/mpl_basis/math.h power / normalize_angle and Primitive1D's evaluators, in the host's operand order
+__device__ __forceinline__ double power(double t, int n) {
+  double tn = 1;
+  while (n > 0) { tn *= t; n--; }
+  return tn;
+}
+__device__ __forceinline__ double normalize_angle(double angle) {
+  while (angle > kPi) angle -= 2.0 * kPi;
+  while (angle < -kPi) angle += 2.0 * kPi;
+  return angle;
+}
+__device__ __forceinline__ double pr_p(const double *c, double t) {
+  return c[0] / 120 * power(t, 5) + c[1] / 24 * power(t, 4) + c[2] / 6 * power(t, 3) + c[3] / 2 * t * t + c[4] * t + c[5];
+}
+__device__ __forceinline__ double pr_v(const double *c, double t) {
+  return c[0] / 24 * power(t, 4) + c[1] / 6 * power(t, 3) + c[2] / 2 * t * t + c[3] * t + c[4];
+}
+__device__ __forceinline__ double pr_a(const double *c, double t) { return c[0] / 6 * power(t, 3) + c[1] / 2 * t * t + c[2] * t + c[3]; }
+__device__ __forceinline__ double pr_j(const double *c, double t) { return c[0] / 2 * t * t + c[1] * t + c[2]; }
+
+template <int DIM>
+__global__ void __launch_bounds__(128) traj_sample_kernel(TrajArgs A) {
+  const int per = A.n_samples + 1;
+  constexpr int RW = 4 * DIM + 3;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < (long long)A.n_paths * per;
+       g += (long long)gridDim.x * blockDim.x) {
+    const int p = (int)(g / per), i = (int)(g % per);
+    double *o = A.samples + g * RW;
+    double row[RW];
+#pragma unroll
+    for (int k = 0; k < RW; k++) row[k] = 0.0;
+    if (A.status[p]) {
+      const long long b = A.offset[p];
+      const int S = (int)(A.offset[p + 1] - b) - 1;
+      const double *taus = A.taus + b;
+      const double total = taus[S];
+      const double dt = total / A.n_samples;
+      const double time = i * dt;
+      double tau = time;
+      if (tau < 0) tau = 0;
+      if (tau > total) tau = total;
+      // Trajectory::evaluate(t, Command&): the first segment with taus[id] <= tau <= taus[id+1]; when the
+      // running sum never decreases, the first id with taus[id+1] >= tau
+      int id = -1;
+      if (A.mono[p]) {
+        int lo = 0, hi = S - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (taus[mid + 1] >= tau) hi = mid;
+          else lo = mid + 1;
+        }
+        if (tau >= taus[lo] && tau <= taus[lo + 1]) id = lo;
+      } else {
+        for (int k = 0; k < S; k++)
+          if (tau >= taus[k] && tau <= taus[k + 1]) { id = k; break; }
+      }
+      if (id >= 0) {
+        tau -= taus[id];
+        const double *c = A.coeff + (b + id) * (DIM + 1) * 6;
+        const double lambda = 1, lambda_dot = 0;
+        const double yaw = normalize_angle(pr_p(c + DIM * 6, tau));
+        const double yaw_dot = normalize_angle(pr_v(c + DIM * 6, tau));
+#pragma unroll
+        for (int a = 0; a < DIM; a++) {
+          const double *ca = c + a * 6;
+          const double vel = pr_v(ca, tau) / lambda;
+          const double acc = pr_a(ca, tau) / lambda / lambda - vel * lambda_dot / lambda / lambda / lambda;
+          row[a] = pr_p(ca, tau);
+          row[DIM + a] = vel;
+          row[2 * DIM + a] = acc;
+          row[3 * DIM + a] = pr_j(ca, tau) / lambda / lambda - 3 / power(lambda, 3) * acc * acc * lambda_dot +
+                             3 / power(lambda, 4) * vel * lambda_dot * lambda_dot;
+        }
+        row[4 * DIM] = yaw;
+        row[4 * DIM + 1] = yaw_dot;
+        row[4 * DIM + 2] = time;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < RW; k++) o[k] = row[k];
+  }
+}
+
+int order_of(int control) {  // h = N/2 of TrajSolver's PolySolver for this control, 0 when it has none
+  switch (control) {
+    case MPLX_VEL: case MPLX_VELxYAW: return 1;
+    case MPLX_ACC: case MPLX_ACCxYAW: return 2;
+    case MPLX_JRK: case MPLX_JRKxYAW: return 3;
+    default: return 0;
+  }
+}
+
+template <int DIM, int H, int HY>
+cudaError_t launch3(const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
+  traj_sweep_kernel<DIM, H, HY><<<(A.n_paths + 127) / 128, 128, 0, st>>>(A);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  if (n_wp > 0) {
+    const long long blocks = std::min<long long>((n_wp + 127) / 128, (long long)sm_count() * 16);
+    traj_coeff_kernel<DIM, H, HY><<<(int)blocks, 128, 0, st>>>(A, n_wp);
+    *launches += 1;
+    if (cudaError_t e = cudaGetLastError()) return e;
+  }
+  if (A.samples) {
+    const long long n = (long long)A.n_paths * (A.n_samples + 1);
+    const long long blocks = std::min<long long>((n + 127) / 128, (long long)sm_count() * 16);
+    traj_sample_kernel<DIM><<<(int)blocks, 128, 0, st>>>(A);
+    *launches += 1;
+    if (cudaError_t e = cudaGetLastError()) return e;
+  }
+  return cudaSuccess;
+}
+
+template <int DIM, int H>
+cudaError_t launch_yaw(int hy, const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
+  if (hy == 1) return launch3<DIM, H, 1>(A, n_wp, st, launches);
+  if (hy == 2) return launch3<DIM, H, 2>(A, n_wp, st, launches);
+  return launch3<DIM, H, 3>(A, n_wp, st, launches);
+}
+template <int DIM>
+cudaError_t launch_dim(int h, int hy, const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
+  if (h == 1) return launch_yaw<DIM, 1>(hy, A, n_wp, st, launches);
+  if (h == 2) return launch_yaw<DIM, 2>(hy, A, n_wp, st, launches);
+  return launch_yaw<DIM, 3>(hy, A, n_wp, st, launches);
+}
+
+}  // namespace
+}  // namespace mplx
+
+extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, const mplx_waypoint *wps,
+                               const uint8_t *wp_control, const double *dts, double v, int control, int yaw_control,
+                               int n_samples, mplx_traj_out *out) {
+  if (int r = mplx_bind(c)) return r;
+  const int h = mplx::order_of(control);
+  if (h == 0) return fail(MPLX_ERR_ARG, "control 0x%x: TrajSolver solves VEL, ACC and JRK (with or without YAW)", control);
+  const int hy = (yaw_control == MPLX_VEL || yaw_control == MPLX_ACC || yaw_control == MPLX_JRK) ? mplx::order_of(yaw_control) : 0;
+  if (hy == 0) return fail(MPLX_ERR_ARG, "yaw_control 0x%x: must be VEL, ACC or JRK", yaw_control);
+  if (!dts && !(v > 0)) return fail(MPLX_ERR_ARG, "no segment times: dts is NULL and v <= 0");
+  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
+  if (!offset || !out || !out->status || !out->seg_t || !out->coeff) return fail(MPLX_ERR_ARG, "missing array");
+  if (out->samples && n_samples <= 0) return fail(MPLX_ERR_ARG, "samples with n_samples <= 0");
+  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
+  for (int p = 0; p < n_paths; p++)
+    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
+  const long long n_wp = offset[n_paths];
+  if (n_wp > 0 && !wps) return fail(MPLX_ERR_ARG, "missing array");
+  if (out->samples && (long long)n_paths * (n_samples + 1) >= ((long long)1 << 40)) return fail(MPLX_ERR_ARG, "too many samples");
+  out->seconds = 0.0;
+  if (n_paths == 0) return MPLX_OK;
+  const int dim = c->dim;
+  TrajBufs &B = c->tb;
+  const size_t nw = (size_t)std::max<long long>(n_wp, 1);
+  CU(B.offset.reserve(n_paths + 1)); CU(B.status.reserve(n_paths)); CU(B.mono.reserve(n_paths));
+  CU(B.wps.reserve(nw)); CU(B.seg_t.reserve(nw)); CU(B.taus.reserve(nw));
+  CU(B.coeff.reserve(nw * (dim + 1) * 6)); CU(B.fac.reserve(nw * 6)); CU(B.dpos.reserve(nw * h * dim));
+  CU(B.dyaw.reserve(nw * hy));
+  if (wp_control) CU(B.ctl.reserve(nw));
+  if (dts) CU(B.dts.reserve(nw));
+  const size_t n_rows = out->samples ? (size_t)n_paths * (n_samples + 1) : 0;
+  if (out->samples) CU(B.samples.reserve(n_rows * (4 * dim + 3)));
+  cudaStream_t st = c->stream;
+  static_assert(sizeof(long long) == sizeof(int64_t), "offset width");
+  CU(cudaMemcpyAsync(B.offset.p, offset, sizeof(int64_t) * (n_paths + 1), cudaMemcpyHostToDevice, st));
+  if (n_wp > 0) {
+    CU(cudaMemcpyAsync(B.wps.p, wps, sizeof(mplx_waypoint) * n_wp, cudaMemcpyHostToDevice, st));
+    if (wp_control) CU(cudaMemcpyAsync(B.ctl.p, wp_control, (size_t)n_wp, cudaMemcpyHostToDevice, st));
+    if (dts) CU(cudaMemcpyAsync(B.dts.p, dts, sizeof(double) * n_wp, cudaMemcpyHostToDevice, st));
+  }
+  mplx::TrajArgs A{n_paths, B.offset.p, B.wps.p, wp_control ? B.ctl.p : nullptr, dts ? B.dts.p : nullptr, v, control,
+                   yaw_control, n_samples, B.status.p, B.mono.p, B.seg_t.p, B.taus.p, B.coeff.p,
+                   out->samples ? B.samples.p : nullptr, B.fac.p, B.dpos.p, B.dyaw.p};
+  cudaEvent_t e0, e1;
+  CU(cudaEventCreate(&e0));
+  CU(cudaEventCreate(&e1));
+  int launches = 0;
+  cudaError_t le = cudaEventRecord(e0, st);
+  if (le == cudaSuccess)
+    le = dim == 2 ? mplx::launch_dim<2>(h, hy, A, n_wp, st, &launches) : mplx::launch_dim<3>(h, hy, A, n_wp, st, &launches);
+  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
+  c->launches += launches;
+  if (le != cudaSuccess) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    CU(le);
+  }
+  CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
+  if (n_wp > 0) {
+    CU(cudaMemcpyAsync(out->seg_t, B.seg_t.p, sizeof(double) * n_wp, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->coeff, B.coeff.p, sizeof(double) * n_wp * (dim + 1) * 6, cudaMemcpyDeviceToHost, st));
+  }
+  if (out->samples) CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  out->seconds = ms * 1e-3;
+  return MPLX_OK;
+}

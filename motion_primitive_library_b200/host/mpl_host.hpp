@@ -178,6 +178,14 @@ class Primitive {
     }
     if (control_ & 16) { pr_yaw_.c[4] = u[Dim]; pr_yaw_.c[5] = p.yaw; }
   }
+  /// From coefficients (each highest order first) and a duration: primitive.h:309-313.  cs holds Dim
+  /// axes, then optionally the yaw axis.
+  Primitive(const vec_E<Vecf<6>> &cs, decimal_t t, int control) : t_(t), control_(control) {
+    for (int i = 0; i < Dim; i++)
+      for (int k = 0; k < 6; k++) prs_[i].c[k] = cs[i](k);
+    if ((int)cs.size() == Dim + 1)
+      for (int k = 0; k < 6; k++) pr_yaw_.c[k] = cs[Dim](k);
+  }
   /// primitive.h:321-331
   Waypoint<Dim> evaluate(decimal_t t) const {
     Waypoint<Dim> p(control_);
@@ -319,6 +327,287 @@ class Trajectory {
   std::vector<decimal_t> taus, Ts;
   decimal_t total_t_{0};
 };
+
+/// factorial: include/mpl_basis/math.h:187-194
+inline int factorial(int n) {
+  int nf = 1;
+  while (n > 0) { nf *= n; n--; }
+  return nf;
+}
+
+namespace MPL {
+/// The dense linear algebra of PolySolver: a column-major matrix, products that sum each element in
+/// increasing k from 0, and LU with row partial pivoting.  The reference calls Eigen here; the Eigen
+/// stand-in the tests compile the reference against implements the same operations in the same order,
+/// so the restatement is pinned to the reference bit for bit under that stand-in.
+namespace dense {
+struct Mat {
+  int r = 0, c = 0;
+  std::vector<decimal_t> d;
+  Mat() {}
+  Mat(int rows, int cols) : r(rows), c(cols), d((size_t)rows * cols, 0.0) {}
+  decimal_t &operator()(int i, int j) { return d[i + (size_t)j * r]; }
+  const decimal_t &operator()(int i, int j) const { return d[i + (size_t)j * r]; }
+  Mat block(int i0, int j0, int rows, int cols) const {
+    Mat b(rows, cols);
+    for (int j = 0; j < cols; j++)
+      for (int i = 0; i < rows; i++) b(i, j) = (*this)(i0 + i, j0 + j);
+    return b;
+  }
+  Mat transpose() const {
+    Mat t(c, r);
+    for (int j = 0; j < c; j++)
+      for (int i = 0; i < r; i++) t(j, i) = (*this)(i, j);
+    return t;
+  }
+};
+/// a * b, element (i, j) = ((0 + a(i,0) b(0,j)) + a(i,1) b(1,j)) + ...
+inline Mat mul(const Mat &a, const Mat &b) {
+  Mat p(a.r, b.c);
+  for (int j = 0; j < b.c; j++)
+    for (int k = 0; k < a.c; k++) {
+      const decimal_t bkj = b(k, j);
+      for (int i = 0; i < a.r; i++) p(i, j) += a(i, k) * bkj;
+    }
+  return p;
+}
+/// Doolittle LU with row partial pivoting: the pivot of column k is the first row >= k of largest |value|.
+/// A zero pivot is divided by, so a singular matrix gives non-finite solutions.
+struct LU {
+  Mat lu;
+  std::vector<int> swap;  // row k was exchanged with row swap[k]
+  explicit LU(Mat a) : lu(std::move(a)), swap(lu.r) {
+    const int n = lu.r;
+    for (int k = 0; k < n; k++) {
+      int p = k;
+      decimal_t amax = std::abs(lu(k, k));
+      for (int i = k + 1; i < n; i++)
+        if (std::abs(lu(i, k)) > amax) { amax = std::abs(lu(i, k)); p = i; }
+      swap[k] = p;
+      if (p != k)
+        for (int j = 0; j < n; j++) std::swap(lu(k, j), lu(p, j));
+      for (int i = k + 1; i < n; i++) lu(i, k) = lu(i, k) / lu(k, k);
+      for (int j = k + 1; j < n; j++)
+        for (int i = k + 1; i < n; i++) lu(i, j) = lu(i, j) - lu(i, k) * lu(k, j);
+    }
+  }
+  /// lu^-1 b: the row exchanges, then forward (unit lower) and back substitution, each sum in increasing index
+  Mat solve(const Mat &b) const {
+    Mat x(b);
+    const int n = lu.r;
+    for (int k = 0; k < n; k++)
+      if (swap[k] != k)
+        for (int j = 0; j < x.c; j++) std::swap(x(k, j), x(swap[k], j));
+    for (int j = 0; j < x.c; j++) {
+      for (int i = 0; i < n; i++)
+        for (int k = 0; k < i; k++) x(i, j) = x(i, j) - lu(i, k) * x(k, j);
+      for (int i = n - 1; i >= 0; i--) {
+        for (int k = i + 1; k < n; k++) x(i, j) = x(i, j) - lu(i, k) * x(k, j);
+        x(i, j) = x(i, j) / lu(i, i);
+      }
+    }
+    return x;
+  }
+};
+}  // namespace dense
+
+/// PolySolver<Dim>: src/mpl_traj_solver/poly_solver.cpp:4-219 and PolyTraj::toPrimitives
+/// (poly_traj.cpp:72-88).  Fits N = 2 (smooth_derivative_order + 1) coefficients per segment through the
+/// waypoints, minimising the integral of the squared minimize_derivative-th derivative, by the reference's
+/// dense formulation, operation by operation: the A, Q and M assembly, A^-1 M by LU, R = ((A^-1 M)^T Q) A^-1 M,
+/// Dp = -Rpp^-1 (Rpf Df), d = M D and one N x N LU solve per segment.  The cost is cubic in the number of
+/// segments; libmplx's mplx_traj_solve solves the same problem in linear time on the device.
+///
+/// Where the reference is undefined:
+///  * two waypoints with free derivatives (the reference skips the free solve, poly_solver.cpp:205, and leaves
+///    those rows of D uninitialised): they are 0;
+///  * a zero-length or non-finite segment time makes A singular: the coefficients are not all finite.
+template <int Dim>
+class PolySolver {
+ public:
+  PolySolver(unsigned smooth_derivative_order, unsigned minimize_derivative)
+      : N_(2 * (smooth_derivative_order + 1)), R_(minimize_derivative) {}
+
+  /// false (and no coefficients) for fewer than two waypoints; dts[i] is segment i's duration
+  bool solve(const vec_E<Waypoint<Dim>> &waypoints, const std::vector<decimal_t> &dts) {
+    coeffs_.clear();
+    waypoints_ = waypoints;
+    dts_ = dts;
+    const int W = (int)waypoints.size(), S = W - 1, N = (int)N_, h = N / 2, R = (int)R_;
+    if (W < 2) return false;
+    dense::Mat A(S * N, S * N), Q(S * N, S * N);
+    for (int i = 0; i < S; i++) {
+      const decimal_t seg_time = dts[i];
+      for (int n = 0; n < N; n++) {
+        if (n < h) {
+          int val = 1;
+          for (int m = 0; m < n; m++) val *= (n - m);
+          A(i * N + n, i * N + n) = val;
+        }
+        for (int r = 0; r < h; r++)
+          if (r <= n) {
+            int val = 1;
+            for (int m = 0; m < r; m++) val *= (n - m);
+            A(i * N + h + r, i * N + n) = val * power(seg_time, n - r);
+          }
+        for (int r = 0; r < N; r++)
+          if (r >= R && n >= R) {
+            int val = 1;
+            for (int m = 0; m < R; m++) val *= (r - m) * (n - m);
+            Q(i * N + r, i * N + n) = val * power(seg_time, r + n - 2 * R + 1) / (unsigned)(r + n - 2 * R + 1);
+          }
+      }
+    }
+    // derivative k < h of a waypoint is fixed when its control flag says so (use_pos, use_vel, use_acc)
+    auto fixed = [&](const Waypoint<Dim> &w, int k) { return ((w.control >> k) & 1) != 0; };
+    int nfix = 0;
+    for (const auto &w : waypoints)
+      for (int k = 0; k < h; k++) nfix += fixed(w, k) ? 1 : 0;
+    const int nfree = W * h - nfix;
+    // (row of the raw per-segment derivative vector, column of D): fixed derivatives first, then the free
+    // ones, each in waypoint order; an interior waypoint ends one segment and starts the next
+    std::vector<std::pair<int, int>> perm;
+    int raw = 0, fix_cnt = 0, free_cnt = 0;
+    for (int id = 0; id < W; id++) {
+      const bool interior = id > 0 && id < W - 1;
+      for (int k = 0; k < h; k++) {
+        const int col = fixed(waypoints[id], k) ? fix_cnt++ : nfix + free_cnt++;
+        perm.push_back({raw, col});
+        if (interior) perm.push_back({raw + h, col});
+        raw++;
+      }
+      if (interior) raw += h;
+    }
+    dense::Mat M(S * N, W * h);
+    for (const auto &pc : perm) M(pc.first, pc.second) = 1;
+    const dense::Mat AinvM = dense::LU(A).solve(M);
+    const dense::Mat Rm = dense::mul(dense::mul(AinvM.transpose(), Q), AinvM);
+    const dense::Mat Rpp = Rm.block(nfix, nfix, nfree, nfree), Rpf = Rm.block(nfix, 0, nfree, nfix);
+    dense::Mat Df(nfix, Dim);
+    for (const auto &pc : perm)
+      if (pc.second < nfix) {
+        const Waypoint<Dim> &w = waypoints[(pc.first + h) / N];
+        const int k = pc.first % h;
+        for (int a = 0; a < Dim; a++) Df(pc.second, a) = k == 0 ? w.pos(a) : k == 1 ? w.vel(a) : k == 2 ? w.acc(a) : w.jrk(a);
+      }
+    dense::Mat D(W * h, Dim);
+    for (int a = 0; a < Dim; a++)
+      for (int i = 0; i < nfix; i++) D(i, a) = Df(i, a);
+    if (W > 2 && nfree > 0) {
+      const dense::Mat Dp = dense::LU(Rpp).solve(dense::mul(Rpf, Df));
+      for (int a = 0; a < Dim; a++)
+        for (int i = 0; i < nfree; i++) D(nfix + i, a) = -Dp(i, a);
+    }
+    const dense::Mat d = dense::mul(M, D);
+    for (int i = 0; i < S; i++) coeffs_.push_back(dense::LU(A.block(i * N, i * N, N, N)).solve(d.block(i * N, 0, N, Dim)));
+    return true;
+  }
+
+  /// PolyTraj::toPrimitives: Primitive1D coefficient k! p_k at index 5 - k, control = the first waypoint's
+  vec_E<Primitive<Dim>> toPrimitives() const {
+    vec_E<Primitive<Dim>> prs;
+    for (std::size_t i = 0; i < coeffs_.size(); i++) {
+      const dense::Mat &p = coeffs_[i];
+      vec_E<Vecf<6>> cs;
+      for (int j = 0; j < p.c; j++) {
+        Vecf<6> c;
+        for (int k = 0; k < p.r; k++) c(5 - k) = p(k, j) * factorial(k);
+        cs.push_back(c);
+      }
+      prs.push_back(Primitive<Dim>(cs, dts_[i], waypoints_.front().control));
+    }
+    return prs;
+  }
+
+ private:
+  unsigned N_, R_;
+  vec_E<Waypoint<Dim>> waypoints_;
+  std::vector<decimal_t> dts_;
+  std::vector<dense::Mat> coeffs_;  // per segment: N x Dim, p(k, axis) multiplies t^k
+};
+
+/// TrajSolver<Dim>: include/mpl_traj_solver/traj_solver.h.  control VEL / ACC / JRK (with or without YAW)
+/// minimises velocity / acceleration / jerk; SNP, or a yaw_control other than VEL / ACC / JRK, leaves the
+/// solver unset and solve() returns an empty Trajectory, as in the reference.  The yaw axis comes from a
+/// PolySolver<1> pass over the waypoints' yaw (endpoints yaw_control, interior VEL).
+/// Where the reference is undefined (see also PolySolver): solve() without usable segment times (no
+/// setDts of n - 1 entries and v <= 0, for two or more waypoints) throws std::invalid_argument.
+template <int Dim>
+class TrajSolver {
+ public:
+  explicit TrajSolver(int control, int yaw_control = Control::VEL) : control_(control), yaw_control_(yaw_control) {
+    if (control == Control::VEL || control == Control::VELxYAW) poly_solver_.reset(new PolySolver<Dim>(0, 1));
+    else if (control == Control::ACC || control == Control::ACCxYAW) poly_solver_.reset(new PolySolver<Dim>(1, 2));
+    else if (control == Control::JRK || control == Control::JRKxYAW) poly_solver_.reset(new PolySolver<Dim>(2, 3));
+    if (yaw_control == Control::VEL) yaw_solver_.reset(new PolySolver<1>(0, 1));
+    else if (yaw_control == Control::ACC) yaw_solver_.reset(new PolySolver<1>(1, 2));
+    else if (yaw_control == Control::JRK) yaw_solver_.reset(new PolySolver<1>(2, 3));
+  }
+  /// waypoints with their own control flags (which derivatives are fixed) and yaw
+  void setWaypoints(const vec_E<Waypoint<Dim>> &ws) {
+    path_.resize(ws.size());
+    for (std::size_t i = 0; i < ws.size(); i++) path_[i] = ws[i].pos;
+    waypoints_ = ws;
+  }
+  /// velocity of the L-inf time allocation used when no segment times are set
+  void setV(decimal_t v) { v_ = v; }
+  void setDts(const std::vector<decimal_t> &dts) { dts_ = dts; }
+  /// positions only: the endpoints take the solver's control, the interior waypoints VEL (position fixed)
+  void setPath(const vec_E<Vecf<Dim>> &path) {
+    path_ = path;
+    waypoints_.assign(path.size(), Waypoint<Dim>(Control::VEL));
+    for (std::size_t i = 0; i < path.size(); i++) waypoints_[i].pos = path[i];
+    if (!waypoints_.empty()) waypoints_.front().control = waypoints_.back().control = control_;
+  }
+  Trajectory<Dim> solve() {
+    if (waypoints_.size() != dts_.size() + 1) dts_ = allocate_time(path_, v_);
+    if (!poly_solver_ || !yaw_solver_) return Trajectory<Dim>();
+    if (waypoints_.size() >= 2 && dts_.size() + 1 != waypoints_.size())
+      throw std::invalid_argument("TrajSolver: no segment times (setDts with n - 1 entries, or setV with v > 0)");
+    poly_solver_->solve(waypoints_, dts_);
+    vec_E<Waypoint<1>> yaws(waypoints_.size(), Waypoint<1>(Control::VEL));
+    for (std::size_t i = 0; i < waypoints_.size(); i++) yaws[i].pos(0) = waypoints_[i].yaw;
+    if (!yaws.empty()) yaws.front().control = yaws.back().control = yaw_control_;
+    yaw_solver_->solve(yaws, dts_);
+    vec_E<Primitive<Dim>> prs = poly_solver_->toPrimitives();
+    const vec_E<Primitive<1>> yaw_prs = yaw_solver_->toPrimitives();
+    for (std::size_t i = 0; i < prs.size(); i++) {
+      vec_E<Vecf<6>> cs(Dim + 1);
+      for (int a = 0; a < Dim; a++)
+        for (int k = 0; k < 6; k++) cs[a](k) = prs[i].pr(a).c[k];
+      for (int k = 0; k < 6; k++) cs[Dim](k) = yaw_prs[i].pr(0).c[k];
+      prs[i] = Primitive<Dim>(cs, prs[i].t(), prs[i].control());
+    }
+    return Trajectory<Dim>(prs);
+  }
+  vec_E<Vecf<Dim>> getPath() const { return path_; }
+  vec_E<Waypoint<Dim>> getWaypoints() const { return waypoints_; }
+  std::vector<decimal_t> getDts() const { return dts_; }
+
+ private:
+  /// traj_solver.h allocate_time: |p_i - p_{i-1}|_inf / v; empty for fewer than two points or v <= 0
+  static std::vector<decimal_t> allocate_time(const vec_E<Vecf<Dim>> &pts, decimal_t v) {
+    if (pts.size() < 2 || v <= 0) return std::vector<decimal_t>();
+    std::vector<decimal_t> dts(pts.size() - 1);
+    for (std::size_t i = 1; i < pts.size(); i++) {
+      decimal_t d = 0;
+      for (int a = 0; a < Dim; a++) {
+        const decimal_t x = std::abs(pts[i](a) - pts[i - 1](a));
+        if (x > d) d = x;
+      }
+      dts[i - 1] = d / v;
+    }
+    return dts;
+  }
+  vec_E<Vecf<Dim>> path_;
+  vec_E<Waypoint<Dim>> waypoints_;
+  std::vector<decimal_t> dts_;
+  decimal_t v_{1};
+  int control_, yaw_control_;
+  std::unique_ptr<PolySolver<Dim>> poly_solver_;
+  std::unique_ptr<PolySolver<1>> yaw_solver_;
+};
+}  // namespace MPL
 
 namespace MPL {
 using Tmap = std::vector<signed char>;

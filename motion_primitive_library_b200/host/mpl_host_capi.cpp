@@ -479,3 +479,113 @@ int mplh_plan_batch(const mplh_plan_args *a, const mplx_waypoint *starts, const 
   return rc;
 }
 }
+
+/* ---- TrajSolver (mpl_host.hpp): one path on the host -------------------------------------------------- */
+
+namespace {
+template <int Dim>
+void put_samples(const Trajectory<Dim> &traj, int n_samples, double *samples) {
+  const auto cmds = traj.sample(n_samples);
+  const int W = 4 * Dim + 3;
+  for (int i = 0; i <= n_samples; i++) {
+    double *o = samples + (size_t)i * W;
+    for (int d = 0; d < Dim; d++) { o[d] = cmds[i].pos(d); o[Dim + d] = cmds[i].vel(d); o[2 * Dim + d] = cmds[i].acc(d); o[3 * Dim + d] = cmds[i].jrk(d); }
+    o[4 * Dim] = cmds[i].yaw; o[4 * Dim + 1] = cmds[i].yaw_dot; o[4 * Dim + 2] = cmds[i].t;
+  }
+}
+template <int Dim>
+void put_waypoints(const Trajectory<Dim> &traj, double *waypoints) {
+  const int V = 4 * Dim + 2;
+  const auto ws = traj.getWaypoints();
+  for (std::size_t i = 0; i < ws.size(); i++) {
+    double *o = waypoints + i * V;
+    const Waypoint<Dim> &w = ws[i];
+    for (int d = 0; d < Dim; d++) { o[d] = w.pos(d); o[Dim + d] = w.vel(d); o[2 * Dim + d] = w.acc(d); o[3 * Dim + d] = w.jrk(d); }
+    o[4 * Dim] = w.yaw; o[4 * Dim + 1] = w.t;
+  }
+}
+template <typename F>
+int with_traj_dim(int dim, F &&f) {
+  try {
+    if (dim == 2) f(std::integral_constant<int, 2>());
+    else if (dim == 3) f(std::integral_constant<int, 3>());
+    else { g_err = "dim must be 2 or 3"; return 1; }
+    return 0;
+  } catch (const std::exception &e) {
+    g_err = e.what();
+    return 2;
+  }
+}
+}  // namespace
+
+extern "C" {
+/* MPL::TrajSolver<dim>(control, yaw_control) on one path of n_wp waypoints.  wp_control NULL: setPath(wps[].pos);
+ * else setWaypoints(wps, waypoint i with control wp_control[i]).  dts (n_wp - 1 entries) given: setDts(dts).
+ * setV(v), then solve().  Outputs (host arrays; any may be NULL except n_seg):
+ *   *n_seg     segments of the solved trajectory (0 when it is empty)
+ *   seg_t      [n_wp - 1] getDts(): the segment times used
+ *   coeff      [n_seg * (dim + 1) * 6] segment j's Primitive1D coefficients, highest order first, axes then yaw
+ *   samples    [(n_samples + 1) * (4 dim + 3)] Trajectory::sample(n_samples) rows {pos, vel, acc, jrk, yaw, yaw_dot, t}
+ *   waypoints  [(n_seg + 1) * (4 dim + 2)] Trajectory::getWaypoints() rows {pos, vel, acc, jrk, yaw, t}
+ * 1: bad argument (dim, n_wp < 0, samples with n_samples < 1, missing wps); 2: solve() threw (no segment times). */
+int mplh_traj_solve(int dim, int control, int yaw_control, const mplx_waypoint *wps, const uint8_t *wp_control, int n_wp,
+                    const double *dts, double v, int n_samples, int32_t *n_seg, double *seg_t, double *coeff,
+                    double *samples, double *waypoints) {
+  if (n_wp < 0 || (n_wp > 0 && !wps) || !n_seg || (samples && n_samples < 1)) { g_err = "bad argument"; return 1; }
+  *n_seg = 0;
+  return with_traj_dim(dim, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    MPL::TrajSolver<Dim> solver(control, yaw_control);
+    if (wp_control) {
+      vec_E<Waypoint<Dim>> ws(n_wp);
+      for (int i = 0; i < n_wp; i++) {
+        ws[i].control = wp_control[i];
+        for (int d = 0; d < Dim; d++) {
+          ws[i].pos(d) = wps[i].pos[d]; ws[i].vel(d) = wps[i].vel[d]; ws[i].acc(d) = wps[i].acc[d]; ws[i].jrk(d) = wps[i].jrk[d];
+        }
+        ws[i].yaw = wps[i].yaw;
+      }
+      solver.setWaypoints(ws);
+    } else {
+      vec_E<Vecf<Dim>> path(n_wp);
+      for (int i = 0; i < n_wp; i++)
+        for (int d = 0; d < Dim; d++) path[i](d) = wps[i].pos[d];
+      solver.setPath(path);
+    }
+    if (dts && n_wp > 0) solver.setDts(std::vector<decimal_t>(dts, dts + (n_wp - 1)));
+    solver.setV(v);
+    const Trajectory<Dim> traj = solver.solve();
+    *n_seg = (int32_t)traj.segs.size();
+    const std::vector<decimal_t> used = solver.getDts();
+    if (seg_t)
+      for (std::size_t i = 0; i < used.size() && (int)i + 1 < n_wp; i++) seg_t[i] = used[i];
+    if (coeff)
+      for (std::size_t j = 0; j < traj.segs.size(); j++)
+        for (int a = 0; a <= Dim; a++)
+          for (int k = 0; k < 6; k++) coeff[(j * (Dim + 1) + a) * 6 + k] = (a < Dim ? traj.segs[j].pr(a) : traj.segs[j].pr_yaw()).c[k];
+    if (samples) put_samples<Dim>(traj, n_samples, samples);
+    if (waypoints) put_waypoints<Dim>(traj, waypoints);
+  });
+}
+
+/* Trajectory<dim> of n_seg segments with durations seg_t and coefficients coeff (mplh_traj_solve's layout), each
+ * segment with the control flag `control`: sample(n_samples) into samples and getWaypoints() into waypoints
+ * (layouts as mplh_traj_solve's; either may be NULL). */
+int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coeff, int control, int n_samples,
+                     double *samples, double *waypoints) {
+  if (n_seg < 0 || (n_seg > 0 && (!seg_t || !coeff)) || (samples && n_samples < 1)) { g_err = "bad argument"; return 1; }
+  return with_traj_dim(dim, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    vec_E<Primitive<Dim>> prs;
+    for (int j = 0; j < n_seg; j++) {
+      vec_E<Vecf<6>> cs(Dim + 1);
+      for (int a = 0; a <= Dim; a++)
+        for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)j * (Dim + 1) + a) * 6 + k];
+      prs.push_back(Primitive<Dim>(cs, seg_t[j], control));
+    }
+    const Trajectory<Dim> traj(prs);
+    if (samples) put_samples<Dim>(traj, n_samples, samples);
+    if (waypoints) put_waypoints<Dim>(traj, waypoints);
+  });
+}
+}

@@ -451,3 +451,84 @@ class BatchPlanner:
             self.close()
         except Exception:
             pass
+
+
+def _traj_lib():
+    if not LIB.exists():
+        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
+    lib = C.CDLL(str(LIB))
+    lib.mplh_last_error.restype = C.c_char_p
+    return lib
+
+
+def load_traj_solve_fn(path, fn):
+    """fn(dim, control, yaw_control, wps, wp_control, n_wp, dts, v, n_samples, n_seg, seg_t, coeff, samples,
+    waypoints): mplh_traj_solve's signature (host/mpl_host_capi.cpp)."""
+    L = C.CDLL(str(path))
+    f = getattr(L, fn)
+    f.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_int,
+                  C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    f.restype = C.c_int
+    return L, f
+
+
+def run_traj_solve(fn, lib, dim, control, pos=None, waypoints=None, wp_control=None, dts=None, v=1.0, yaw_control=0x01,
+                   n_samples=50):
+    """TrajSolver<dim>(control, yaw_control) on one path: setPath(pos) (n x dim), or setWaypoints(waypoints
+    (WAYPOINT_DTYPE) with controls wp_control); setDts(dts) when given; setV(v); solve().  Returns a dict:
+    `segments`, `seg_t` (getDts), `coeff` (segments x (dim+1) x 6: Primitive1D coefficients, axes then yaw),
+    `samples` = sample(n_samples) rows {pos, vel, acc, jrk, yaw, yaw_dot, t} and `waypoints` = getWaypoints()
+    rows {pos, vel, acc, jrk, yaw, t}."""
+    if waypoints is None:
+        pos = np.asarray(pos, dtype=np.float64).reshape(-1, dim)
+        wps = np.zeros(len(pos), dtype=WAYPOINT_DTYPE)
+        wps["pos"][:, :dim] = pos
+        ctl = None
+    else:
+        wps = np.ascontiguousarray(waypoints, dtype=WAYPOINT_DTYPE)
+        ctl = np.ascontiguousarray(wp_control, dtype=np.uint8)
+        assert len(ctl) == len(wps)
+    n = len(wps)
+    d = None if dts is None else np.ascontiguousarray(dts, dtype=np.float64)
+    assert d is None or len(d) == max(n - 1, 0)
+    seg_t = np.zeros(max(n - 1, 1))
+    coeff = np.zeros((max(n - 1, 1), dim + 1, 6))
+    samples = np.zeros((n_samples + 1, 4 * dim + 3))
+    wout = np.zeros((max(n, 1), 4 * dim + 2))
+    n_seg = C.c_int32(0)
+    rc = fn(dim, control, yaw_control, wps.ctypes.data if n else None, None if ctl is None else ctl.ctypes.data, n,
+            None if d is None else d.ctypes.data, float(v), n_samples, C.byref(n_seg), seg_t.ctypes.data,
+            coeff.ctypes.data, samples.ctypes.data, wout.ctypes.data)
+    if rc != 0:
+        err = getattr(lib, "mplh_last_error", None)
+        raise RuntimeError(err().decode() if err else f"trajectory solve failed rc={rc}")
+    s = n_seg.value
+    return dict(segments=s, seg_t=seg_t[: max(n - 1, 0)].copy(), coeff=coeff[:s].copy(), samples=samples,
+                waypoints=wout[: s + 1 if s else 0].copy())
+
+
+def traj_solve(dim, control, **kw):
+    """MPL::TrajSolver on the host (mpl_host.hpp: the reference's dense formulation, one path).  Arguments as
+    run_traj_solve."""
+    lib = _traj_lib()
+    _, fn = load_traj_solve_fn(LIB, "mplh_traj_solve")
+    return run_traj_solve(fn, lib, dim, control, **kw)
+
+
+def traj_sample(dim, seg_t, coeff, control, n_samples):
+    """Trajectory<dim> built on the host from segment times and Primitive1D coefficients (segments x (dim+1) x 6,
+    axes then yaw), each segment with the control flag `control`: (sample(n_samples), getWaypoints()) as arrays
+    of rows {pos, vel, acc, jrk, yaw, yaw_dot, t} and {pos, vel, acc, jrk, yaw, t}."""
+    lib = _traj_lib()
+    lib.mplh_traj_sample.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_void_p]
+    lib.mplh_traj_sample.restype = C.c_int
+    seg_t = np.ascontiguousarray(seg_t, dtype=np.float64)
+    coeff = np.ascontiguousarray(coeff, dtype=np.float64).reshape(len(seg_t), dim + 1, 6)
+    samples = np.zeros((n_samples + 1, 4 * dim + 3))
+    wout = np.zeros((len(seg_t) + 1, 4 * dim + 2))
+    rc = lib.mplh_traj_sample(dim, len(seg_t), seg_t.ctypes.data, coeff.ctypes.data, control, n_samples,
+                              samples.ctypes.data, wout.ctypes.data)
+    if rc != 0:
+        raise RuntimeError(lib.mplh_last_error().decode())
+    return samples, wout[: len(seg_t) + 1 if len(seg_t) else 0]
