@@ -401,6 +401,49 @@ int mplx_traj_solve(mplx_ctx *ctx, int n_paths, const int64_t *offset, const mpl
                     const uint8_t *wp_control, const double *dts, double v, int control, int yaw_control,
                     int n_samples, mplx_traj_out *out);
 
+/* ---- time scaling of trajectories (Trajectory::scale / scale_down) ------------------------------ */
+
+#define MPLX_TRAJ_SCALE 1      /* Trajectory::scale(ri, rf)          */
+#define MPLX_TRAJ_SCALE_DOWN 2 /* Trajectory::scale_down(mv, ri, rf) */
+
+/* Results of mplx_traj_scale (HOST arrays), slots as mplx_traj_out's. */
+typedef struct {
+  int32_t *status;   /* [n_paths] 1: scaled; 2: SCALE_DOWN found no velocity above mv (max_l <= 1), unchanged;
+                        0: not scaled (fewer than 2 waypoints, a segment time <= 0 or not finite, a coefficient
+                        not finite, or ri, rf or (SCALE_DOWN) mv not finite and > 0)                         */
+  double *total_t;   /* [n_paths] the trajectory's total time after the call (0 for status 0)                  */
+  double *seg_T;     /* [n_wp] getSegmentTimes(): Ts[j+1] - Ts[j] of the scaled waypoint times; the path's last
+                        slot and every slot of a status-0 path hold 0                                          */
+  int32_t *n_lambda; /* NULL, or [n_paths] lambda segments of the path (0 unless status 1)                    */
+  double *lambda;    /* NULL, or [n_wp*5*dim*7] lambda segments {a3, a2, a1, a0, ti, tf, dT}: path p's start at
+                        slot offset[p]*5*dim, unused slots hold 0                                             */
+  double *samples;   /* NULL, or [n_paths*(n_samples+1)*(4*dim+3)] Trajectory::sample(n_samples) rows after the
+                        scaling, mplx_traj_out's row format; zeros for status-0 paths                          */
+  double seconds;    /* out: device time of the kernels (CUDA events)                                        */
+} mplx_traj_scale_out;
+
+/* Trajectory<Dim>::scale(ri, rf) (mode MPLX_TRAJ_SCALE) or scale_down(mv, ri, rf) (MPLX_TRAJ_SCALE_DOWN) on
+ * n_paths trajectories on the device, Dim = the ctx's dimension.  Path p's segment j has the duration
+ * seg_t[offset[p] + j] and the coefficients coeff[(offset[p] + j)*(dim+1)*6 ...], exactly mplx_traj_out's
+ * layout, so mplx_traj_solve's output feeds straight in.  mv, ri and rf are per-path arrays; mv may be NULL
+ * for SCALE.
+ *   scale: lambda(tau) is the cubic from 1/ri (slope 0) at tau = 0 to 1/rf (slope 0) at the end.
+ *   scale_down: each segment and axis whose max_vel exceeds mv adds a knot at its velocity extrema, at its
+ *     start (except segment 0) and at its end where |v| / mv > 1; between (0, ri) and (end, rf) the knots
+ *     take the largest ratio max_l.  Note ri, rf here against 1/ri, 1/rf for scale, as in the reference.
+ * Then t = integral of lambda maps real time to polynomial time; sampling inverts it per sample by the
+ * closed-form quartic root (Lambda::getTau).  Each path is what the host Trajectory gives (mpl_host.hpp),
+ * bit for bit where only arithmetic is involved (VEL and ACC paths, lambda constant), else within 1e-9
+ * relative: cbrt, acos and cos are CUDA's (DESIGN.md §8).  As in the reference, the last sample can land an
+ * ulp past the final lambda segment, and is then the trajectory's start state.  Each path's outputs do not
+ * depend on the other paths.  Scratch is kept in the ctx.
+ * Refusals, each with MPLX_ERR_ARG, the outputs untouched and no launch: an unknown mode, mv NULL for
+ * SCALE_DOWN, ri or rf NULL, n_paths < 0, offset NULL, offset[0] != 0 or decreasing, out / status / total_t /
+ * seg_T NULL, seg_t or coeff NULL with waypoints, and samples given with n_samples <= 0.  Synchronous. */
+int mplx_traj_scale(mplx_ctx *ctx, int n_paths, const int64_t *offset, const double *seg_t, const double *coeff,
+                    int mode, const double *mv, const double *ri, const double *rf, int n_samples,
+                    mplx_traj_scale_out *out);
+
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field
  * planning once a batch fills the GPU, else the register kernel),

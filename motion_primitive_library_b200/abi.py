@@ -18,6 +18,7 @@ LIB_PATH = PKG_DIR / "lib" / "libmplx.so"
 MPLX_OK, MPLX_ERR_ARG, MPLX_ERR_CUDA, MPLX_ERR_ALLOC = 0, 1, 2, 3
 VEL, ACC, JRK, SNP = 0x01, 0x03, 0x07, 0x0F
 VELxYAW, ACCxYAW, JRKxYAW, SNPxYAW = 0x11, 0x13, 0x17, 0x1F
+TRAJ_SCALE, TRAJ_SCALE_DOWN = 1, 2  # mplx_traj_scale modes
 LATTICE_MAX = 13
 
 # Waypoint<Dim> payload (include/mplx.h mplx_waypoint; reference include/mpl_basis/waypoint.h:33-38)
@@ -52,6 +53,7 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_grow",
     "mplx_plan_batch_grow_results",
     "mplx_traj_solve",
+    "mplx_traj_scale",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -148,6 +150,20 @@ class TrajOut(C.Structure):
     ]
 
 
+class TrajScaleOut(C.Structure):
+    """mplx_traj_scale_out"""
+
+    _fields_ = [
+        ("status", C.c_void_p),
+        ("total_t", C.c_void_p),
+        ("seg_T", C.c_void_p),
+        ("n_lambda", C.c_void_p),
+        ("lambda_", C.c_void_p),
+        ("samples", C.c_void_p),
+        ("seconds", C.c_double),
+    ]
+
+
 class MplxError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libmplx error {code}: {msg}")
@@ -221,6 +237,8 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch_grow_results.restype = i32
     lib.mplx_traj_solve.argtypes = [vp, i32, vp, vp, vp, vp, f64, i32, i32, i32, C.POINTER(TrajOut)]
     lib.mplx_traj_solve.restype = i32
+    lib.mplx_traj_scale.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(TrajScaleOut)]
+    lib.mplx_traj_scale.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

@@ -161,16 +161,21 @@ struct UpdateBufs {
   }
 };
 
-// inputs, outputs and per-waypoint scratch of mplx_traj_solve (mplx_traj.cu), sized by the largest batch so far
+// inputs, outputs and per-waypoint scratch of mplx_traj_solve and mplx_traj_scale (mplx_traj.cu), sized by the
+// largest batch so far; the second line of members is mplx_traj_scale's alone
 struct TrajBufs {
   DevBuf<long long> offset;
   DevBuf<mplx_waypoint> wps;
   DevBuf<uint8_t> ctl, mono;
   DevBuf<int32_t> status;
   DevBuf<double> dts, seg_t, taus, coeff, samples, fac, dpos, dyaw;
+  DevBuf<int32_t> n_cand, n_knot;
+  DevBuf<double> par, total, seg_T, cand, cand_p, knot_t, knot_p, lam, lam_T;
   void release() {
     offset.release(); wps.release(); ctl.release(); mono.release(); status.release(); dts.release(); seg_t.release();
     taus.release(); coeff.release(); samples.release(); fac.release(); dpos.release(); dyaw.release();
+    n_cand.release(); n_knot.release(); par.release(); total.release(); seg_T.release(); cand.release();
+    cand_p.release(); knot_t.release(); knot_p.release(); lam.release(); lam_T.release();
   }
 };
 

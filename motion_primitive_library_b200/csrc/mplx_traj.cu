@@ -430,6 +430,49 @@ __device__ __forceinline__ double pr_v(const double *c, double t) {
 __device__ __forceinline__ double pr_a(const double *c, double t) { return c[0] / 6 * power(t, 3) + c[1] / 2 * t * t + c[2] * t + c[3]; }
 __device__ __forceinline__ double pr_j(const double *c, double t) { return c[0] / 2 * t * t + c[1] * t + c[2]; }
 
+// One row of Trajectory::sample at polynomial time tau (already clamped) and real time `time`:
+// Trajectory::evaluate(t, Command&) (trajectory.h:100-137) after its getTau and lambda lookup, in the host's
+// operand order.  taus is the path's running sum of segment times (S + 1 entries), coeff its first segment's
+// coefficients; mono says the running sum never decreases.  Leaves row untouched when no segment holds tau.
+template <int DIM>
+__device__ __forceinline__ void eval_row(const double *taus, int S, bool mono, const double *coeff, double tau,
+                                         double time, double lambda, double lambda_dot, double *row) {
+  // the first segment with taus[id] <= tau <= taus[id+1]; when the running sum never decreases, the first id
+  // with taus[id+1] >= tau
+  int id = -1;
+  if (mono) {
+    int lo = 0, hi = S - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (taus[mid + 1] >= tau) hi = mid;
+      else lo = mid + 1;
+    }
+    if (tau >= taus[lo] && tau <= taus[lo + 1]) id = lo;
+  } else {
+    for (int k = 0; k < S; k++)
+      if (tau >= taus[k] && tau <= taus[k + 1]) { id = k; break; }
+  }
+  if (id < 0) return;
+  tau -= taus[id];
+  const double *c = coeff + (size_t)id * (DIM + 1) * 6;
+  const double yaw = normalize_angle(pr_p(c + DIM * 6, tau));
+  const double yaw_dot = normalize_angle(pr_v(c + DIM * 6, tau));
+#pragma unroll
+  for (int a = 0; a < DIM; a++) {
+    const double *ca = c + a * 6;
+    const double vel = pr_v(ca, tau) / lambda;
+    const double acc = pr_a(ca, tau) / lambda / lambda - vel * lambda_dot / lambda / lambda / lambda;
+    row[a] = pr_p(ca, tau);
+    row[DIM + a] = vel;
+    row[2 * DIM + a] = acc;
+    row[3 * DIM + a] = pr_j(ca, tau) / lambda / lambda - 3 / power(lambda, 3) * acc * acc * lambda_dot +
+                       3 / power(lambda, 4) * vel * lambda_dot * lambda_dot;
+  }
+  row[4 * DIM] = yaw;
+  row[4 * DIM + 1] = yaw_dot;
+  row[4 * DIM + 2] = time;
+}
+
 template <int DIM>
 __global__ void __launch_bounds__(128) traj_sample_kernel(TrajArgs A) {
   const int per = A.n_samples + 1;
@@ -451,42 +494,7 @@ __global__ void __launch_bounds__(128) traj_sample_kernel(TrajArgs A) {
       double tau = time;
       if (tau < 0) tau = 0;
       if (tau > total) tau = total;
-      // Trajectory::evaluate(t, Command&): the first segment with taus[id] <= tau <= taus[id+1]; when the
-      // running sum never decreases, the first id with taus[id+1] >= tau
-      int id = -1;
-      if (A.mono[p]) {
-        int lo = 0, hi = S - 1;
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (taus[mid + 1] >= tau) hi = mid;
-          else lo = mid + 1;
-        }
-        if (tau >= taus[lo] && tau <= taus[lo + 1]) id = lo;
-      } else {
-        for (int k = 0; k < S; k++)
-          if (tau >= taus[k] && tau <= taus[k + 1]) { id = k; break; }
-      }
-      if (id >= 0) {
-        tau -= taus[id];
-        const double *c = A.coeff + (b + id) * (DIM + 1) * 6;
-        const double lambda = 1, lambda_dot = 0;
-        const double yaw = normalize_angle(pr_p(c + DIM * 6, tau));
-        const double yaw_dot = normalize_angle(pr_v(c + DIM * 6, tau));
-#pragma unroll
-        for (int a = 0; a < DIM; a++) {
-          const double *ca = c + a * 6;
-          const double vel = pr_v(ca, tau) / lambda;
-          const double acc = pr_a(ca, tau) / lambda / lambda - vel * lambda_dot / lambda / lambda / lambda;
-          row[a] = pr_p(ca, tau);
-          row[DIM + a] = vel;
-          row[2 * DIM + a] = acc;
-          row[3 * DIM + a] = pr_j(ca, tau) / lambda / lambda - 3 / power(lambda, 3) * acc * acc * lambda_dot +
-                             3 / power(lambda, 4) * vel * lambda_dot * lambda_dot;
-        }
-        row[4 * DIM] = yaw;
-        row[4 * DIM + 1] = yaw_dot;
-        row[4 * DIM + 2] = time;
-      }
+      eval_row<DIM>(taus, S, A.mono[p] != 0, A.coeff + b * (DIM + 1) * 6, tau, time, 1.0, 0.0, row);
     }
 #pragma unroll
     for (int k = 0; k < RW; k++) o[k] = row[k];
@@ -602,6 +610,533 @@ extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, 
   }
   if (out->samples) CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  out->seconds = ms * 1e-3;
+  return MPLX_OK;
+}
+
+// ---- time scaling of trajectories (mplx_traj_scale, include/mplx.h) -------------------------------------------
+//   scale_prep_kernel    one thread per path: parameter and duration checks, the running sum of segment times
+//   scale_cand_kernel    one thread per segment: finite coefficients; for SCALE_DOWN the knots of the segment's
+//                        axes (max_vel, extrema_v), sorted by time
+//   scale_knot_kernel    one thread per path: max_l, the knot list with equal times merged
+//   scale_fit_kernel     one thread per lambda slot: the LambdaSeg fit of knots k and k + 1
+//   scale_times_kernel   one thread per path: the running sum of dT, the scaled waypoint times Ts
+//   scale_sample_kernel  one thread per sample: getTau, the lambda lookup and eval_row
+// Within a path the knots of segment j lie in [taus[j], taus[j+1]] (a root tv in (0, t) rounds to
+// tv + taus[j] <= t + taus[j]), so sorting each segment's knots and concatenating them in segment order sorts
+// the path's knots as std::sort does, up to the order of equal times, which the merge makes irrelevant
+// (DESIGN.md §8).
+namespace mplx {
+namespace {
+
+constexpr int kCand = 5;  // knots per segment and axis: <= 3 extrema_v roots, the start and the end
+
+// math.h:21-131 (quad, cubic, quartic, solve), operation by operation; r receives the roots in the host's order
+__device__ __forceinline__ int quad_roots(double b, double c, double d, double *r) {
+  const double p = c * c - 4 * b * d;
+  if (p < 0) return 0;
+  r[0] = (-c - sqrt(p)) / (2 * b);
+  r[1] = (-c + sqrt(p)) / (2 * b);
+  return 2;
+}
+__device__ __forceinline__ int cubic_roots(double a, double b, double c, double d, double *r) {
+  const double a2 = b / a, a1 = c / a, a0 = d / a;
+  const double Q = (3 * a1 - a2 * a2) / 9;
+  const double R = (9 * a1 * a2 - 27 * a0 - 2 * a2 * a2 * a2) / 54;
+  const double D = Q * Q * Q + R * R;
+  if (D > 0) {
+    const double S = cbrt(R + sqrt(D));
+    const double T = cbrt(R - sqrt(D));
+    r[0] = -a2 / 3 + (S + T);
+    return 1;
+  }
+  if (D == 0) {
+    const double S = cbrt(R);
+    r[0] = -a2 / 3 + S + S;
+    r[1] = -a2 / 3 - S;
+    return 2;
+  }
+  const double theta = acos(R / sqrt(-Q * Q * Q));
+  r[0] = 2 * sqrt(-Q) * cos(theta / 3) - a2 / 3;
+  r[1] = 2 * sqrt(-Q) * cos((theta + 2 * kPi) / 3) - a2 / 3;
+  r[2] = 2 * sqrt(-Q) * cos((theta + 4 * kPi) / 3) - a2 / 3;
+  return 3;
+}
+__device__ __forceinline__ int quartic_roots(double a, double b, double c, double d, double e, double *r) {
+  const double a3 = b / a, a2 = c / a, a1 = d / a, a0 = e / a;
+  double ys[3];
+  cubic_roots(1, -a2, a1 * a3 - 4 * a0, 4 * a2 * a0 - a1 * a1 - a3 * a3 * a0, ys);
+  const double y1 = ys[0];
+  const double rr = a3 * a3 / 4 - a2 + y1;
+  if (rr < 0) return 0;
+  const double R = sqrt(rr);
+  double D, E;
+  if (R != 0) {
+    D = sqrt(0.75 * a3 * a3 - R * R - 2 * a2 + 0.25 * (4 * a3 * a2 - 8 * a1 - a3 * a3 * a3) / R);
+    E = sqrt(0.75 * a3 * a3 - R * R - 2 * a2 - 0.25 * (4 * a3 * a2 - 8 * a1 - a3 * a3 * a3) / R);
+  } else {
+    D = sqrt(0.75 * a3 * a3 - 2 * a2 + 2 * sqrt(y1 * y1 - 4 * a0));
+    E = sqrt(0.75 * a3 * a3 - 2 * a2 - 2 * sqrt(y1 * y1 - 4 * a0));
+  }
+  int n = 0;
+  if (!isnan(D)) {
+    r[n++] = -a3 / 4 + R / 2 + D / 2;
+    r[n++] = -a3 / 4 + R / 2 - D / 2;
+  }
+  if (!isnan(E)) {
+    r[n++] = -a3 / 4 - R / 2 + E / 2;
+    r[n++] = -a3 / 4 - R / 2 - E / 2;
+  }
+  return n;
+}
+__device__ __forceinline__ int solve_roots(double a, double b, double c, double d, double e, double *r) {
+  if (a != 0) return quartic_roots(a, b, c, d, e, r);
+  if (b != 0) return cubic_roots(b, c, d, e, r);
+  if (c != 0) return quad_roots(c, d, e, r);
+  if (d != 0) { r[0] = -e / d; return 1; }
+  return 0;
+}
+
+// Primitive1D::extrema_v (primitive.h:152-162): roots of a(t) in (0, t), stopping at the first root >= t
+__device__ __forceinline__ int extrema_v(const double *c, double t, double *ts) {
+  double r[4];
+  const int n = solve_roots(0, c[0] / 6, c[1] / 2, c[2], c[3], r);
+  int m = 0;
+  for (int k = 0; k < n; k++) {
+    if (r[k] > 0 && r[k] < t) ts[m++] = r[k];
+    else if (r[k] >= t) break;
+  }
+  return m;
+}
+// Primitive::max_vel (primitive.h:353-363)
+__device__ __forceinline__ double max_vel(const double *c, double t) {
+  double ts[3];
+  const int n = extrema_v(c, t, ts);
+  const double v0 = fabs(pr_v(c, 0)), v1 = fabs(pr_v(c, t));
+  double m = v0 < v1 ? v1 : v0;  // std::max
+  for (int k = 0; k < n; k++)
+    if (ts[k] > 0 && ts[k] < t) {
+      const double v = fabs(pr_v(c, ts[k]));
+      m = v > m ? v : m;
+    }
+  return m;
+}
+
+// LambdaSeg (lambda.h:24-71): the Hermite fit by Gauss-Jordan inversion as on the host (mpl_host.hpp)
+struct LSeg {
+  double a[4], ti, tf, dT;
+};
+__device__ __forceinline__ double lseg_T(const double *a, double t) {
+  return a[0] / 4 * power(t, 4) + a[1] / 3 * power(t, 3) + a[2] / 2 * t * t + a[3] * t;
+}
+__device__ void lseg_fit(double t1, double p1, double t2, double p2, LSeg &s) {
+  double A[4][4] = {{power(t1, 3), t1 * t1, t1, 1}, {3 * t1 * t1, 2 * t1, 1, 0},
+                    {power(t2, 3), t2 * t2, t2, 1}, {3 * t2 * t2, 2 * t2, 1, 0}};
+  double inv[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
+#pragma unroll
+  for (int col = 0; col < 4; col++) {
+    int piv = col;
+#pragma unroll
+    for (int r = col + 1; r < 4; r++)
+      if (fabs(A[r][col]) > fabs(A[piv][col])) piv = r;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      // a row exchange without dynamic register indexing
+      double x = A[col][k], y = inv[col][k];
+#pragma unroll
+      for (int r = col + 1; r < 4; r++)
+        if (r == piv) {
+          A[col][k] = A[r][k]; A[r][k] = x;
+          inv[col][k] = inv[r][k]; inv[r][k] = y;
+        }
+    }
+    const double d = A[col][col];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      A[col][k] /= d;
+      inv[col][k] /= d;
+    }
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      if (r == col) continue;
+      const double f = A[r][col];
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        A[r][k] -= f * A[col][k];
+        inv[r][k] -= f * inv[col][k];
+      }
+    }
+  }
+  const double b[4] = {p1, 0.0, p2, 0.0};
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    double acc = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) acc += inv[i][k] * b[k];
+    s.a[i] = fabs(acc) < 1e-5 ? 0.0 : acc;
+  }
+  s.ti = t1;
+  s.tf = t2;
+  s.dT = lseg_T(s.a, t2) - lseg_T(s.a, t1);
+}
+
+struct ScaleArgs {
+  int n_paths, mode, n_samples;
+  const long long *offset;
+  const double *seg_t, *coeff, *par;  // par: [3 * n_paths] mv, ri, rf
+  int32_t *status, *n_cand, *n_knot;
+  double *taus, *cand, *cand_p, *knot_t, *knot_p, *lam, *lam_T, *total, *seg_T, *samples;
+  uint8_t *lam_mono;
+};
+
+__device__ __forceinline__ bool pos_finite(double x) { return isfinite(x) && x > 0; }
+
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_prep_kernel(ScaleArgs A) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int W = (int)(A.offset[p + 1] - b);
+  const double *par = A.par + 3 * p;
+  bool ok = W >= 2 && pos_finite(par[1]) && pos_finite(par[2]) && (A.mode == MPLX_TRAJ_SCALE || pos_finite(par[0]));
+  // Trajectory's constructor: taus[j+1] = t_j + taus[j]
+  if (W > 0) A.taus[b] = 0.0;
+  for (int j = 0; j + 1 < W; j++) {
+    const double t = A.seg_t[b + j];
+    ok = ok && pos_finite(t);
+    A.taus[b + j + 1] = t + A.taus[b + j];
+  }
+  A.status[p] = ok ? 1 : 0;
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_cand_kernel(ScaleArgs A, long long n_wp) {
+  constexpr int NC = kCand * DIM;
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n_wp; s += (long long)gridDim.x * blockDim.x) {
+    const int p = path_of(A.offset, A.n_paths, s);
+    const long long b = A.offset[p];
+    const int W = (int)(A.offset[p + 1] - b), j = (int)(s - b);
+    A.n_cand[s] = 0;
+    if (j + 1 >= W) continue;
+    const double *c = A.coeff + s * (DIM + 1) * 6;
+    bool finite = true;
+    for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+    if (!finite) A.status[p] = 0;  // every writer stores 0
+    if (A.mode != MPLX_TRAJ_SCALE_DOWN || !finite) continue;
+    const double t = A.seg_t[s], mv = A.par[3 * p], tau0 = A.taus[s];
+    double kt[NC], pmax = 0.0;
+    int n = 0;
+    for (int i = 0; i < DIM; i++) {
+      const double *ci = c + i * 6;
+      if (!(max_vel(ci, t) > mv)) continue;
+      double ts[kCand];
+      int m = extrema_v(ci, t, ts);
+      if (j != 0) ts[m++] = 0;
+      ts[m++] = t;
+      for (int k = 0; k < m; k++) {
+        const double lv = fabs(pr_v(ci, ts[k])) / mv;
+        if (lv <= 1) continue;
+        // insertion by time
+        const double tk = ts[k] + tau0;
+        int q = n++;
+        while (q > 0 && kt[q - 1] > tk) { kt[q] = kt[q - 1]; q--; }
+        kt[q] = tk;
+        pmax = lv > pmax ? lv : pmax;
+      }
+    }
+    for (int k = 0; k < n; k++) A.cand[s * NC + k] = kt[k];
+    A.n_cand[s] = n;
+    A.cand_p[s] = pmax;
+  }
+}
+
+// Trajectory::scale_down's knot list (trajectory.h:173-228 as the host defines it), or scale's two knots
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_knot_kernel(ScaleArgs A) {
+  constexpr int NC = kCand * DIM;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int S = (int)(A.offset[p + 1] - b) - 1;
+  double *kt = A.knot_t + b * NC, *kp = A.knot_p + b * NC;
+  A.n_knot[p] = 0;
+  if (!A.status[p]) return;
+  const double *par = A.par + 3 * p;
+  const double T = A.taus[b + S];
+  if (A.mode == MPLX_TRAJ_SCALE) {
+    kt[0] = 0; kp[0] = 1.0 / par[1];
+    kt[1] = T; kp[1] = 1.0 / par[2];
+    A.n_knot[p] = 2;
+    return;
+  }
+  const double ri = par[1], rf = par[2];
+  double max_l = 1;
+  if (ri > max_l) max_l = ri;
+  for (int j = 0; j < S; j++)
+    if (A.n_cand[b + j] && A.cand_p[b + j] > max_l) max_l = A.cand_p[b + j];
+  if (rf > max_l) max_l = rf;
+  if (max_l <= 1) {
+    A.status[p] = 2;
+    return;
+  }
+  // the sorted knots with equal times merged into their first: (0, ri), every interior time with max_l, and
+  // (T, rf) unless a knot of the last segment ends there too, which then comes first and keeps max_l
+  int n = 1;
+  kt[0] = 0; kp[0] = ri;
+  for (int j = 0; j < S; j++) {
+    const int m = A.n_cand[b + j];
+    const double *ct = A.cand + (b + j) * NC;
+    for (int k = 0; k < m; k++)
+      if (ct[k] > kt[n - 1]) { kt[n] = ct[k]; kp[n] = max_l; n++; }
+  }
+  if (T > kt[n - 1]) { kt[n] = T; kp[n] = rf; n++; }
+  A.n_knot[p] = n;
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_fit_kernel(ScaleArgs A, long long n_slot) {
+  constexpr int NC = kCand * DIM;
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n_slot; s += (long long)gridDim.x * blockDim.x) {
+    const int p = path_of(A.offset, A.n_paths, s / NC);
+    const long long b = A.offset[p] * NC;
+    const int k = (int)(s - b);
+    double *o = A.lam + s * 7;
+    LSeg g = {{0, 0, 0, 0}, 0, 0, 0};
+    if (k + 1 < A.n_knot[p]) lseg_fit(A.knot_t[s], A.knot_p[s], A.knot_t[s + 1], A.knot_p[s + 1], g);
+    o[0] = g.a[0]; o[1] = g.a[1]; o[2] = g.a[2]; o[3] = g.a[3]; o[4] = g.ti; o[5] = g.tf; o[6] = g.dT;
+  }
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_times_kernel(ScaleArgs A) {
+  constexpr int NC = kCand * DIM;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int W = (int)(A.offset[p + 1] - b), S = W - 1;
+  double *segT = A.seg_T + b;
+  const double *taus = A.taus + b;
+  const int st = A.status[p];
+  if (st == 0) {
+    for (int j = 0; j < W; j++) segT[j] = 0.0;
+    A.total[p] = 0.0;
+    return;
+  }
+  if (st == 2) {  // no lambda: Ts = taus
+    for (int j = 0; j < S; j++) segT[j] = taus[j + 1] - taus[j];
+    segT[S] = 0.0;
+    A.total[p] = taus[S];
+    A.lam_mono[p] = 1;
+    return;
+  }
+  const int nl = A.n_knot[p] - 1;
+  const double *lam = A.lam + b * NC * 7;
+  double *lT = A.lam_T + b * NC;
+  // getTau's running T += dT, left to right
+  double T = 0;
+  bool mono = true;
+  lT[0] = 0;
+  for (int k = 0; k < nl; k++) {
+    const double Tn = T + lam[k * 7 + 6];
+    mono = mono && Tn >= T;
+    lT[k + 1] = T = Tn;
+  }
+  A.lam_mono[p] = mono ? 1 : 0;
+  // Lambda::getT(taus[j]): the first segment with ti <= tau <= tf; the knots increase strictly from 0 and the
+  // taus never decrease, so that segment's index never decreases along the path
+  int k = 0;
+  double prev = 0;
+  for (int j = 0; j <= S; j++) {
+    const double tau = taus[j];
+    while (k < nl && !(tau >= lam[k * 7 + 4] && tau <= lam[k * 7 + 5])) k++;
+    const double *a = lam + k * 7;
+    const double Ts = k < nl ? lT[k] + (lseg_T(a, tau) - lseg_T(a, a[4])) : lT[nl];
+    if (j > 0) segT[j - 1] = Ts - prev;
+    prev = Ts;
+  }
+  segT[S] = 0.0;
+  A.total[p] = prev;
+}
+
+// Lambda::getTau (lambda.h:157-179): -1 when no segment gives a root
+__device__ __forceinline__ double get_tau(const double *lam, const double *lT, int nl, bool mono, double t) {
+  int k = 0;
+  if (mono) {  // skip the segments whose [T, T + dT] ends below t; the rest are scanned as on the host
+    int lo = 0, hi = nl;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (lT[mid + 1] >= t) hi = mid;
+      else lo = mid + 1;
+    }
+    k = lo;
+  }
+  for (; k < nl; k++) {
+    if (t >= lT[k] && t <= lT[k + 1]) {
+      const double *a = lam + k * 7;
+      const double e = lT[k] - t - lseg_T(a, a[4]);
+      double r[4];
+      const int n = solve_roots(a[0] / 4, a[1] / 3, a[2] / 2, a[3], e, r);
+      for (int q = 0; q < n; q++)
+        if (r[q] >= a[4] && r[q] <= a[5]) return r[q];
+    } else if (mono && t < lT[k]) {
+      break;
+    }
+  }
+  return -1;
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(128) scale_sample_kernel(ScaleArgs A) {
+  constexpr int NC = kCand * DIM;
+  const int per = A.n_samples + 1;
+  constexpr int RW = 4 * DIM + 3;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < (long long)A.n_paths * per;
+       g += (long long)gridDim.x * blockDim.x) {
+    const int p = (int)(g / per), i = (int)(g % per);
+    double row[RW];
+#pragma unroll
+    for (int k = 0; k < RW; k++) row[k] = 0.0;
+    const int st = A.status[p];
+    if (st) {
+      const long long b = A.offset[p];
+      const int S = (int)(A.offset[p + 1] - b) - 1;
+      const double *taus = A.taus + b;
+      const double total = A.total[p];
+      const double dt = total / A.n_samples;
+      const double time = i * dt;
+      double tau = time, lambda = 1, lambda_dot = 0;
+      const int nl = st == 1 ? A.n_knot[p] - 1 : 0;
+      const double *lam = A.lam + b * NC * 7;
+      if (nl > 0) tau = get_tau(lam, A.lam_T + b * NC, nl, A.lam_mono[p] != 0, time);
+      if (tau < 0) tau = 0;
+      if (tau > total) tau = total;
+      if (nl > 0) {
+        // Lambda::evaluate: the first segment with ti <= tau < tf, else (tau at the last tf) the last one
+        int lo = 0, hi = nl - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (lam[mid * 7 + 5] > tau) hi = mid;
+          else lo = mid + 1;
+        }
+        const double *a = lam + lo * 7;
+        lambda = a[0] * power(tau, 3) + a[1] * tau * tau + a[2] * tau + a[3];
+        lambda_dot = 3 * a[0] * tau * tau + 2 * a[1] * tau + a[2];
+      }
+      // the running sum of positive segment times never decreases
+      eval_row<DIM>(taus, S, true, A.coeff + b * (DIM + 1) * 6, tau, time, lambda, lambda_dot, row);
+    }
+    double *o = A.samples + g * RW;
+#pragma unroll
+    for (int k = 0; k < RW; k++) o[k] = row[k];
+  }
+}
+
+template <int DIM>
+cudaError_t launch_scale(const ScaleArgs &A, long long n_wp, cudaStream_t st, int *launches) {
+  const int pb = (A.n_paths + 127) / 128;
+  auto grid = [](long long n) { return (int)std::min<long long>((n + 127) / 128, (long long)sm_count() * 16); };
+  scale_prep_kernel<DIM><<<pb, 128, 0, st>>>(A);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  scale_cand_kernel<DIM><<<grid(n_wp), 128, 0, st>>>(A, n_wp);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  scale_knot_kernel<DIM><<<pb, 128, 0, st>>>(A);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  scale_fit_kernel<DIM><<<grid(n_wp * kCand * DIM), 128, 0, st>>>(A, n_wp * kCand * DIM);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  scale_times_kernel<DIM><<<pb, 128, 0, st>>>(A);
+  *launches += 1;
+  if (cudaError_t e = cudaGetLastError()) return e;
+  if (A.samples) {
+    scale_sample_kernel<DIM><<<grid((long long)A.n_paths * (A.n_samples + 1)), 128, 0, st>>>(A);
+    *launches += 1;
+    if (cudaError_t e = cudaGetLastError()) return e;
+  }
+  return cudaSuccess;
+}
+
+}  // namespace
+}  // namespace mplx
+
+extern "C" int mplx_traj_scale(mplx_ctx *c, int n_paths, const int64_t *offset, const double *seg_t,
+                               const double *coeff, int mode, const double *mv, const double *ri, const double *rf,
+                               int n_samples, mplx_traj_scale_out *out) {
+  if (int r = mplx_bind(c)) return r;
+  if (mode != MPLX_TRAJ_SCALE && mode != MPLX_TRAJ_SCALE_DOWN) return fail(MPLX_ERR_ARG, "mode %d: must be MPLX_TRAJ_SCALE or MPLX_TRAJ_SCALE_DOWN", mode);
+  if (mode == MPLX_TRAJ_SCALE_DOWN && !mv) return fail(MPLX_ERR_ARG, "SCALE_DOWN without mv");
+  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
+  if (!offset || !ri || !rf || !out || !out->status || !out->total_t || !out->seg_T) return fail(MPLX_ERR_ARG, "missing array");
+  if (out->samples && n_samples <= 0) return fail(MPLX_ERR_ARG, "samples with n_samples <= 0");
+  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
+  for (int p = 0; p < n_paths; p++)
+    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
+  const long long n_wp = offset[n_paths];
+  if (n_wp > 0 && (!seg_t || !coeff)) return fail(MPLX_ERR_ARG, "missing array");
+  if (out->samples && (long long)n_paths * (n_samples + 1) >= ((long long)1 << 40)) return fail(MPLX_ERR_ARG, "too many samples");
+  out->seconds = 0.0;
+  if (n_paths == 0) return MPLX_OK;
+  const int dim = c->dim;
+  const size_t NC = (size_t)mplx::kCand * dim;
+  TrajBufs &B = c->tb;
+  const size_t nw = (size_t)std::max<long long>(n_wp, 1);
+  CU(B.offset.reserve(n_paths + 1)); CU(B.status.reserve(n_paths)); CU(B.mono.reserve(n_paths));
+  CU(B.par.reserve(3 * (size_t)n_paths)); CU(B.n_knot.reserve(n_paths)); CU(B.total.reserve(n_paths));
+  CU(B.seg_t.reserve(nw)); CU(B.taus.reserve(nw)); CU(B.seg_T.reserve(nw)); CU(B.n_cand.reserve(nw));
+  CU(B.cand_p.reserve(nw)); CU(B.coeff.reserve(nw * (dim + 1) * 6));
+  CU(B.cand.reserve(nw * NC)); CU(B.knot_t.reserve(nw * NC)); CU(B.knot_p.reserve(nw * NC));
+  CU(B.lam.reserve(nw * NC * 7)); CU(B.lam_T.reserve(nw * NC));
+  const size_t n_rows = out->samples ? (size_t)n_paths * (n_samples + 1) : 0;
+  if (out->samples) CU(B.samples.reserve(n_rows * (4 * dim + 3)));
+  std::vector<double> par(3 * (size_t)n_paths);
+  for (int p = 0; p < n_paths; p++) {
+    par[3 * p] = mv ? mv[p] : 0.0;
+    par[3 * p + 1] = ri[p];
+    par[3 * p + 2] = rf[p];
+  }
+  cudaStream_t st = c->stream;
+  CU(cudaMemcpyAsync(B.offset.p, offset, sizeof(int64_t) * (n_paths + 1), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(B.par.p, par.data(), sizeof(double) * par.size(), cudaMemcpyHostToDevice, st));
+  if (n_wp > 0) {
+    CU(cudaMemcpyAsync(B.seg_t.p, seg_t, sizeof(double) * n_wp, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.coeff.p, coeff, sizeof(double) * n_wp * (dim + 1) * 6, cudaMemcpyHostToDevice, st));
+  }
+  mplx::ScaleArgs A{n_paths, mode, n_samples, B.offset.p, B.seg_t.p, B.coeff.p, B.par.p, B.status.p, B.n_cand.p,
+                    B.n_knot.p, B.taus.p, B.cand.p, B.cand_p.p, B.knot_t.p, B.knot_p.p, B.lam.p, B.lam_T.p,
+                    B.total.p, B.seg_T.p, out->samples ? B.samples.p : nullptr, B.mono.p};
+  cudaEvent_t e0, e1;
+  CU(cudaEventCreate(&e0));
+  CU(cudaEventCreate(&e1));
+  int launches = 0;
+  cudaError_t le = cudaEventRecord(e0, st);
+  if (le == cudaSuccess)
+    le = dim == 2 ? mplx::launch_scale<2>(A, n_wp, st, &launches) : mplx::launch_scale<3>(A, n_wp, st, &launches);
+  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
+  c->launches += launches;
+  if (le != cudaSuccess) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    CU(le);
+  }
+  CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out->total_t, B.total.p, sizeof(double) * n_paths, cudaMemcpyDeviceToHost, st));
+  if (n_wp > 0) CU(cudaMemcpyAsync(out->seg_T, B.seg_T.p, sizeof(double) * n_wp, cudaMemcpyDeviceToHost, st));
+  std::vector<int32_t> nk;
+  if (out->n_lambda) {
+    nk.resize(n_paths);
+    CU(cudaMemcpyAsync(nk.data(), B.n_knot.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
+  }
+  if (out->lambda && n_wp > 0) CU(cudaMemcpyAsync(out->lambda, B.lam.p, sizeof(double) * n_wp * NC * 7, cudaMemcpyDeviceToHost, st));
+  if (out->samples) CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (out->n_lambda)
+    for (int p = 0; p < n_paths; p++) out->n_lambda[p] = out->status[p] == 1 ? nk[p] - 1 : 0;
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   cudaEventDestroy(e0);

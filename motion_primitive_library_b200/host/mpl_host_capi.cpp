@@ -589,3 +589,82 @@ int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coef
   });
 }
 }
+
+/* ---- Trajectory time scaling (mpl_host.hpp): one path on the host ------------------------------------------ */
+
+namespace {
+/// whether mplx_traj_scale would scale this path (status 1 or 2) rather than refuse it (status 0)
+template <int Dim>
+bool scalable(int n_seg, const double *seg_t, const double *coeff, int mode, double mv, double ri, double rf) {
+  auto pos = [](double x) { return std::isfinite(x) && x > 0; };
+  if (n_seg < 1 || !pos(ri) || !pos(rf) || (mode == MPLX_TRAJ_SCALE_DOWN && !pos(mv))) return false;
+  for (int j = 0; j < n_seg; j++)
+    if (!pos(seg_t[j])) return false;
+  for (size_t k = 0; k < (size_t)n_seg * (Dim + 1) * 6; k++)
+    if (!std::isfinite(coeff[k])) return false;
+  return true;
+}
+}  // namespace
+
+extern "C" {
+/* Trajectory<dim> of n_seg segments (mplh_traj_sample's inputs), then scale(ri, rf) (mode MPLX_TRAJ_SCALE) or
+ * scale_down(mv, ri, rf) (MPLX_TRAJ_SCALE_DOWN), as mplx_traj_scale does it for one path.  Outputs (host arrays):
+ *   *status    1 scaled, 2 scale_down returned false (unchanged), 0 not scaled: mplx_traj_scale's classes
+ *   *total_t   getTotalTime() (0 for status 0)
+ *   seg_T      [n_seg + 1] getSegmentTimes(), then 0 (all 0 for status 0)
+ *   *n_lambda  lambda segments (NULL allowed)
+ *   lambda     NULL or [(n_seg + 1) * 5 * dim * 7] {a3, a2, a1, a0, ti, tf, dT} per lambda segment, then zeros
+ *   samples    NULL or [(n_samples + 1) * (4 dim + 3)] sample(n_samples) rows (zeros for status 0)
+ * 1: bad argument (dim, mode, n_seg < 0, missing arrays, samples with n_samples < 1). */
+int mplh_traj_scale(int dim, int n_seg, const double *seg_t, const double *coeff, int control, int mode, double mv,
+                    double ri, double rf, int n_samples, int32_t *status, double *total_t, double *seg_T,
+                    int32_t *n_lambda, double *lambda, double *samples) {
+  if (n_seg < 0 || (n_seg > 0 && (!seg_t || !coeff)) || !status || !total_t || !seg_T || (samples && n_samples < 1) ||
+      (mode != MPLX_TRAJ_SCALE && mode != MPLX_TRAJ_SCALE_DOWN)) {
+    g_err = "bad argument";
+    return 1;
+  }
+  return with_traj_dim(dim, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    const size_t n_slot = (size_t)(n_seg + 1) * 5 * Dim;
+    *status = 0;
+    *total_t = 0;
+    for (int j = 0; j <= n_seg; j++) seg_T[j] = 0;
+    if (n_lambda) *n_lambda = 0;
+    if (lambda) std::fill(lambda, lambda + n_slot * 7, 0.0);
+    if (samples) std::fill(samples, samples + (size_t)(n_samples + 1) * (4 * Dim + 3), 0.0);
+    if (!scalable<Dim>(n_seg, seg_t, coeff, mode, mv, ri, rf)) return;
+    vec_E<Primitive<Dim>> prs;
+    for (int j = 0; j < n_seg; j++) {
+      vec_E<Vecf<6>> cs(Dim + 1);
+      for (int a = 0; a <= Dim; a++)
+        for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)j * (Dim + 1) + a) * 6 + k];
+      prs.push_back(Primitive<Dim>(cs, seg_t[j], control));
+    }
+    Trajectory<Dim> traj(prs);
+    const bool scaled = mode == MPLX_TRAJ_SCALE ? traj.scale(ri, rf) : traj.scale_down(mv, ri, rf);
+    *status = scaled ? 1 : 2;
+    *total_t = traj.getTotalTime();
+    const std::vector<decimal_t> dts = traj.getSegmentTimes();
+    for (int j = 0; j < n_seg; j++) seg_T[j] = dts[j];
+    const auto &ls = traj.lambda().segs;
+    if (ls.size() > n_slot) throw std::logic_error("lambda segments exceed their slots");
+    if (n_lambda) *n_lambda = (int32_t)ls.size();
+    if (lambda)
+      for (size_t k = 0; k < ls.size(); k++) {
+        double *o = lambda + k * 7;
+        for (int i = 0; i < 4; i++) o[i] = ls[k].a[i];
+        o[4] = ls[k].ti; o[5] = ls[k].tf; o[6] = ls[k].dT;
+      }
+    if (samples) put_samples<Dim>(traj, n_samples, samples);
+  });
+}
+
+/* The closed-form root solver solve(a, b, c, d, e) (mpl_host.hpp): *n roots (at most 4) into roots. */
+int mplh_solve(double a, double b, double c, double d, double e, int32_t *n, double *roots) {
+  const std::vector<decimal_t> r = solve(a, b, c, d, e);
+  *n = (int32_t)r.size();
+  for (size_t k = 0; k < r.size() && k < 4; k++) roots[k] = r[k];
+  return 0;
+}
+}

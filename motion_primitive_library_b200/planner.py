@@ -532,3 +532,76 @@ def traj_sample(dim, seg_t, coeff, control, n_samples):
     if rc != 0:
         raise RuntimeError(lib.mplh_last_error().decode())
     return samples, wout[: len(seg_t) + 1 if len(seg_t) else 0]
+
+
+def load_traj_scale_fn(path, fn, flags=False):
+    """fn(dim, n_seg, seg_t, coeff, control, mode, mv, ri, rf, n_samples, status, total_t, seg_T, n_lambda, lambda,
+    samples[, flags]): mplh_traj_scale's signature (host/mpl_host_capi.cpp), with the reference driver's trailing
+    per-row flags when `flags`."""
+    L = C.CDLL(str(path))
+    f = getattr(L, fn)
+    f.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
+                  C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
+                  C.c_void_p] + ([C.c_void_p] if flags else [])
+    f.restype = C.c_int
+    return L, f
+
+
+def run_traj_scale(fn, lib, dim, seg_t, coeff, mode, mv=1.0, ri=1.0, rf=1.0, control=0x07, n_samples=50, flags=False):
+    """Trajectory<dim> from segment times and Primitive1D coefficients (segments x (dim+1) x 6, axes then yaw),
+    then scale(ri, rf) (mode 1) or scale_down(mv, ri, rf) (mode 2).  Returns a dict: `status` (1 scaled,
+    2 unchanged, 0 not scaled), `total_t`, `seg_T` (getSegmentTimes, segments entries), `lambda` (n x 7 rows
+    {a3, a2, a1, a0, ti, tf, dT}), `samples` = sample(n_samples) rows {pos, vel, acc, jrk, yaw, yaw_dot, t} and,
+    with flags, `flags` (1 on the rows whose lambda the reference leaves indeterminate)."""
+    seg_t = np.ascontiguousarray(seg_t, dtype=np.float64)
+    n = len(seg_t)
+    coeff = np.ascontiguousarray(coeff, dtype=np.float64).reshape(n, dim + 1, 6)
+    st, nl, tot = C.c_int32(0), C.c_int32(0), C.c_double(0)
+    seg_T = np.zeros(n + 1)
+    lam = np.zeros(((n + 1) * 5 * dim, 7))
+    samples = np.zeros((n_samples + 1, 4 * dim + 3))
+    fl = np.zeros(n_samples + 1, dtype=np.uint8)
+    args = [dim, n, seg_t.ctypes.data, coeff.ctypes.data, control, mode, float(mv), float(ri), float(rf), n_samples,
+            C.byref(st), C.byref(tot), seg_T.ctypes.data, C.byref(nl), lam.ctypes.data, samples.ctypes.data]
+    rc = fn(*(args + ([fl.ctypes.data] if flags else [])))
+    if rc != 0:
+        err = getattr(lib, "mplh_last_error", None)
+        raise RuntimeError(err().decode() if err else f"trajectory scale failed rc={rc}")
+    r = dict(status=st.value, total_t=tot.value, seg_T=seg_T[:n].copy(), **{"lambda": lam[: nl.value].copy()},
+             samples=samples)
+    if flags:
+        r["flags"] = fl
+    return r
+
+
+def traj_scale(dim, seg_t, coeff, mode, **kw):
+    """Trajectory::scale / scale_down on the host (mpl_host.hpp, one path).  Arguments as run_traj_scale.
+
+    As in the reference, sample(N)'s last time N * (total / N) can land an ulp past the last lambda segment;
+    getTau then finds no root and that row is the trajectory's start state."""
+    lib = _traj_lib()
+    _, fn = load_traj_scale_fn(LIB, "mplh_traj_scale")
+    return run_traj_scale(fn, lib, dim, seg_t, coeff, mode, **kw)
+
+
+def load_solve_fn(path, fn):
+    L = C.CDLL(str(path))
+    f = getattr(L, fn)
+    f.argtypes = [C.c_double] * 5 + [C.POINTER(C.c_int32), C.c_void_p]
+    f.restype = C.c_int
+    return L, f
+
+
+def run_solve(fn, a, b, c, d, e):
+    """solve(a, b, c, d, e) of math.h: the real roots of a t^4 + b t^3 + c t^2 + d t + e, in solver order."""
+    n = C.c_int32(0)
+    r = np.zeros(4)
+    fn(float(a), float(b), float(c), float(d), float(e), C.byref(n), r.ctypes.data)
+    return r[: n.value].copy()
+
+
+def solve_roots(a, b, c, d, e):
+    """The host's closed-form root solver (mpl_host.hpp), as run_solve."""
+    _traj_lib()
+    _, fn = load_solve_fn(LIB, "mplh_solve")
+    return run_solve(fn, a, b, c, d, e)

@@ -8,6 +8,7 @@ import numpy as np
 from . import abi
 
 VEL, ACC, JRK = abi.VEL, abi.ACC, abi.JRK
+SCALE, SCALE_DOWN = abi.TRAJ_SCALE, abi.TRAJ_SCALE_DOWN
 
 
 class TrajSolverBatch:
@@ -68,6 +69,62 @@ class TrajSolverBatch:
             s = max(int(n[p]) - 1, 0)
             r = dict(status=int(status[p]), seg_t=seg_t[offset[p]:offset[p] + s].copy(),
                      coeff=coeff[offset[p]:offset[p] + s].copy())
+            if samples is not None:
+                r["samples"] = samples[p].copy()
+            res.append(r)
+        return res, out.seconds
+
+    def scale(self, results, mode, mv=None, ri=1.0, rf=1.0, n_samples=0, with_lambda=False):
+        """Trajectory::scale(ri, rf) (mode SCALE) or scale_down(mv, ri, rf) (SCALE_DOWN) on the device for the
+        trajectories `results` (dicts with `seg_t` and `coeff`, as solve returns them).  mv, ri and rf are scalars
+        or one value per path.  Returns (results, seconds): one dict per path with `status` (1: scaled; 2:
+        scale_down found no velocity above mv, unchanged; 0: not scaled — fewer than 2 waypoints, a segment time
+        <= 0 or not finite, a coefficient not finite, or a parameter not finite and > 0), `total_t`, `seg_T`
+        (getSegmentTimes of the scaled trajectory), with with_lambda `lambda` (rows {a3, a2, a1, a0, ti, tf, dT})
+        and, with n_samples > 0, `samples` = sample(n_samples) rows as solve's.
+
+        As in the reference, sample(N)'s last time N * (total / N) can land an ulp past the last lambda segment;
+        no root is then found and that row is the trajectory's start state."""
+        dim = self.dim
+        n_paths = len(results)
+        if mode == SCALE_DOWN and mv is None:
+            raise ValueError("scale_down needs mv")
+        n = np.array([len(r["seg_t"]) + 1 if len(r["seg_t"]) else 0 for r in results], dtype=np.int64)
+        offset = np.zeros(n_paths + 1, dtype=np.int64)
+        np.cumsum(n, out=offset[1:])
+        total = int(offset[-1])
+        seg_t = np.zeros(max(total, 1))
+        coeff = np.zeros((max(total, 1), dim + 1, 6))
+        for p, r in enumerate(results):
+            s = int(n[p]) - 1
+            if s > 0:
+                seg_t[offset[p]:offset[p] + s] = r["seg_t"]
+                coeff[offset[p]:offset[p] + s] = np.asarray(r["coeff"]).reshape(s, dim + 1, 6)
+
+        def per_path(x):
+            return np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (n_paths,)))
+
+        mva = None if mv is None else per_path(mv)
+        ria, rfa = per_path(ri), per_path(rf)
+        NC = 5 * dim
+        status = np.zeros(max(n_paths, 1), dtype=np.int32)
+        total_t = np.zeros(max(n_paths, 1))
+        seg_T = np.zeros(max(total, 1))
+        n_lambda = np.zeros(max(n_paths, 1), dtype=np.int32)
+        lam = np.zeros((max(total, 1) * NC, 7)) if with_lambda else None
+        samples = np.zeros((max(n_paths, 1), n_samples + 1, 4 * dim + 3)) if n_samples > 0 else None
+        out = abi.TrajScaleOut(status.ctypes.data, total_t.ctypes.data, seg_T.ctypes.data, n_lambda.ctypes.data,
+                               None if lam is None else lam.ctypes.data,
+                               None if samples is None else samples.ctypes.data, 0.0)
+        abi.check(self._lib.mplx_traj_scale(self._h, n_paths, offset.ctypes.data, seg_t.ctypes.data, coeff.ctypes.data,
+                                            mode, None if mva is None else mva.ctypes.data, ria.ctypes.data,
+                                            rfa.ctypes.data, n_samples, C.byref(out)))
+        res = []
+        for p in range(n_paths):
+            s = max(int(n[p]) - 1, 0)
+            r = dict(status=int(status[p]), total_t=float(total_t[p]), seg_T=seg_T[offset[p]:offset[p] + s].copy())
+            if lam is not None:
+                r["lambda"] = lam[offset[p] * NC:offset[p] * NC + n_lambda[p]].copy()
             if samples is not None:
                 r["samples"] = samples[p].copy()
             res.append(r)
