@@ -144,15 +144,18 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
   CU(mplx::launch_pack_bits(c->map.p, nvox, c->occ.p, true, c->stream));
   const int nz = c->dim == 3 ? dim[2] : 1;
   const size_t npairs = mplx::occ2_pair_count(c->dim, dim[0], dim[1], nz);
-  CU(c->occ2.reserve(npairs));
+  CU(c->occ2.reserve(2 * npairs));
   CU(mplx::launch_pack_occ2(c->occ.p, nvox, c->dim, dim[0], dim[1], nz, c->occ2.p, c->stream));
   c->launches += 2;
   {
-    // L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_expand_fxn
-    const size_t bytes = npairs * sizeof(uint2);
+    // L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_expand_fxn.  Both
+    // halves when they fit it; otherwise the occupancy half, which every sample reads, and not the summary
+    // half, which only uncertain samples read (a window larger than the carve-out thrashes it).
     int maxp = 0, maxw = 0;
     cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
     cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
+    const size_t half = npairs * sizeof(uint32_t);
+    const size_t bytes = 2 * half <= (size_t)maxp ? 2 * half : half;
     c->occ2_window = 0;
     if (maxp > 0 && maxw > 0) {
       const size_t want = bytes < (size_t)maxp ? bytes : (size_t)maxp;
@@ -171,6 +174,7 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
   }
   c->P.occ2_nb[0] = mplx::occ2_bricks_x(c->dim, dim[0]);
   c->P.occ2_nb[1] = mplx::occ2_bricks_y(c->dim, dim[1]);
+  c->P.occ2_sum = (unsigned)npairs;
   c->P.res = res;
   c->P.rinv = 1.0 / res;
   c->has_map = true;

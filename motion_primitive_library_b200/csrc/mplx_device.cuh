@@ -35,10 +35,11 @@ struct EnvParams {
   const int *tcount;           // [kNMax+1]
   const double *tdt;           // [kNMax+1]  T/n (env_map.h:98)
   int maxn;                    // largest n the flat sample phase accepts (<= kNMax)
-  // {occupancy word, candidate-summary word} pairs of the fixed-point kernels (mplx_fx.cu), in bricks
-  // (layout: mplx_pack.cuh)
-  const uint2 *occ2;
-  size_t occ2_bytes;  // size of occ2 when an L2 persisting carve-out was granted for it, else 0
+  // {occupancy word, candidate-summary word} pairs of the fixed-point kernels (mplx_fx.cu), in bricks,
+  // occupancy half first (layout: mplx_pack.cuh)
+  const uint32_t *occ2;
+  unsigned occ2_sum;  // words of each half: the summary word of pair p is occ2[occ2_sum + p]
+  size_t occ2_bytes;  // bytes of occ2 (from its start) an L2 persisting carve-out was granted for, else 0
   int occ2_nb[2];     // bricks of occ2 along x and y (occ2_bricks_x, occ2_bricks_y)
   // Per-axis value tables of U for the node-cooperative kernel (mplx_fx.cu): the distinct values of
   // U[.][a] (bitwise) of all axes listed one after the other as "rows"; U[i][a] == row_u[prow[3*i+a]].

@@ -15,7 +15,8 @@
 //   fraction word >= 128  (y_fx + eps at least 2 eps = 2^-25 above a cell boundary)
 //       => floor(y_ref) = floor(y_fx + eps): the sample is CERTAIN and its verdict is the voxel bit;
 //   fraction word <  128  => the sample is UNCERTAIN: y_ref lies within 2^-25 of the boundary below
-//       cell c' = floor(y_fx + eps), its true cell is c' or c'-1 on that axis.  A second bitmap holds,
+//       cell c' = floor(y_fx + eps), its true cell is c' or c'-1 on that axis.  A second bitmap (the
+//       summary half of occ2, apart from the occupancy half the certain samples read) holds,
 //       per voxel, the OR of the occupancy of the <= 2^Dim cells {c', c'-1}^Dim (out of map = 1): if
 //       that bit is clear every candidate is free and the sample is free whichever the reference
 //       picks; otherwise the sample is AMBIGUOUS and is re-evaluated with the exact FP64 chain.
@@ -239,7 +240,7 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
         double C[DIM][ORD + 1];
 #pragma unroll
         for (int a = 0; a < DIM; a++) fx_axis<ORD>(pr.ax[a], P.origin[a], P.rinv, C[a]);
-        const unsigned *__restrict__ occ_words = reinterpret_cast<const unsigned *>(P.occ2);
+        const unsigned *__restrict__ occ_words = P.occ2;
         unsigned long long amask = 0;
         bool full = false;
         double t = 0;
@@ -318,18 +319,20 @@ cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, i
   });
 }
 
-// The {occupancy word, candidate-summary word} pairs in bricks (layout and bits: occ2_brick_pair).
+// The {occupancy word, candidate-summary word} pairs in bricks (layout and bits: occ2_brick_pair), each
+// half of the buffer holding one word of every pair.
 __global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, int dim, int nx, int ny, int nz,
-                                 uint2 *__restrict__ out) {
+                                 uint32_t *__restrict__ out) {
   const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
   for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < npairs; p += (size_t)gridDim.x * blockDim.x) {
     uint32_t o, s;
     occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
-    out[p] = make_uint2(o, s);
+    out[p] = o;
+    out[npairs + p] = s;
   }
 }
 
-cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint2 *d_out,
+cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint32_t *d_out,
                              cudaStream_t st) {
   const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
   int grid = (int)((npairs + 255) / 256);

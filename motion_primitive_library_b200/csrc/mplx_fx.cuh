@@ -32,7 +32,7 @@ __device__ __forceinline__ void fx_axis(const Axis<ORD> &ax, double origin, doub
 // One group of UNR samples.  `left` as in sample_group.  Returns 2 when a CERTAIN sample blocks,
 // else 1 when the group held the loop's end, else 0; bit j of `amb` = sample j is ambiguous.
 // Per sample one 32-bit word is loaded: the occupancy word of the cell when the sample is certain,
-// the candidate-summary word when it is uncertain (the two are interleaved in bricks, mplx_pack.cuh);
+// the candidate-summary word when it is uncertain (the two halves of occ2, mplx_pack.cuh);
 // a sample outside the map reads as all-ones (blocked / never "all candidates free").  The word is
 // rotated so that the cell's bit lands on bit j, and the group is decided on the OR of those bits.
 __device__ __forceinline__ unsigned rotr_wrap(unsigned x, unsigned s) {
@@ -81,7 +81,7 @@ __device__ __forceinline__ int fx_group(const EnvParams &P, const unsigned *__re
       // occ2 in bricks (mplx_pack.cuh): the pair of the cell, its occupancy (certain) or summary word
       const int z = DIM == 3 ? cell[DIM - 1] : 0;
       rot[j] = occ2_bit<DIM>(cell[0], cell[1]) - j;
-      if (inside) w[j] = __ldg(base + (2 * occ2_pair<DIM>(cell[0], cell[1], z, P.occ2_nb[0], P.occ2_nb[1]) | ub));
+      if (inside) w[j] = __ldg(base + (occ2_pair<DIM>(cell[0], cell[1], z, P.occ2_nb[0], P.occ2_nb[1]) + (ub ? P.occ2_sum : 0u)));
     }
     t += dt;  // the reference's running sum (env_map.h:99)
   }
@@ -137,7 +137,7 @@ __device__ __forceinline__ void fx_issue(const EnvParams &P, const unsigned *__r
     } else {
       const int z = DIM == 3 ? cell[DIM - 1] : 0;
       G.rot[j] = occ2_bit<DIM>(cell[0], cell[1]) - j;
-      if (inside) G.w[j] = __ldg(base + (2 * occ2_pair<DIM>(cell[0], cell[1], z, P.occ2_nb[0], P.occ2_nb[1]) | ub));
+      if (inside) G.w[j] = __ldg(base + (occ2_pair<DIM>(cell[0], cell[1], z, P.occ2_nb[0], P.occ2_nb[1]) + (ub ? P.occ2_sum : 0u)));
     }
     t += dt;  // the reference's running sum (env_map.h:99)
   }
@@ -159,7 +159,7 @@ __device__ __forceinline__ int fx_decide(const FxWords<UNR> &G, int left, unsign
 template <int DIM, int ORD, int UNR, bool REGION>
 __device__ __forceinline__ int fx_traverse(const EnvParams &P, const double (&C)[DIM][ORD + 1], double dt, int count,
                                            unsigned long long &amask, bool &full) {
-  const unsigned *__restrict__ base = reinterpret_cast<const unsigned *>(P.occ2);
+  const unsigned *__restrict__ base = P.occ2;
   amask = 0;
   full = false;
   double t = 0;

@@ -633,13 +633,14 @@ cudaError_t launch_expand_fxn(const EnvParams &P, const mplx_waypoint *d_nodes, 
   static const int span_env = [] { const char *v = getenv("MPLX_FXN_SPAN"); return v ? atoi(v) : -1; }();
   cudaError_t e = cudaMemsetAsync(amb_n, 0, sizeof(unsigned) * kFxSegments, st);
   if (e != cudaSuccess) return e;
-  // Keep the voxel bitmaps in the L2's persisting carve-out: every CTA of every launch re-reads them while
-  // ~0.9 GB of successor records stream through the same cache (mplx_set_map sized the carve-out).
+  // Keep the voxel bitmap in the L2's persisting carve-out: every CTA of every launch re-reads it while ~0.9 GB
+  // of successor records stream through the same cache (mplx_set_map sized the carve-out and the window: the
+  // whole buffer where it fits, else its occupancy half, 16 MiB at 512^3).
   static const bool no_window = getenv("MPLX_NO_L2_WINDOW") != nullptr;  // tuning / A-B
   if (!no_window && P.occ2_bytes > 0) {
     cudaStreamAttrValue av;
     memset(&av, 0, sizeof av);
-    av.accessPolicyWindow.base_ptr = const_cast<uint2 *>(P.occ2);
+    av.accessPolicyWindow.base_ptr = const_cast<uint32_t *>(P.occ2);
     av.accessPolicyWindow.num_bytes = P.occ2_bytes;
     av.accessPolicyWindow.hitRatio = 1.0f;
     av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;

@@ -217,11 +217,11 @@ struct mplx_ctx {
   // static data in HBM
   DevBuf<int8_t> map, pot;
   DevBuf<uint32_t> region, occ;
-  DevBuf<uint2> occ2;
+  DevBuf<uint32_t> occ2;
   DevBuf<unsigned char> prow, row_axis;  // per-axis value tables of U (EnvParams::prow ...)
   DevBuf<double> row_u;
   int n_rows = 0;
-  size_t occ2_window = 0;  // bytes of occ2 covered by the L2 access-policy window (0 = none)  // {occupancy, candidate summary} words of the fixed-point kernel
+  size_t occ2_window = 0;  // bytes of occ2 (from its start) covered by the L2 access-policy window (0 = none)
   DevBuf<double> U, ttab, tdt;
   DevBuf<int> tcount;
   int kernel = 0;  // mplx_set_kernel

@@ -41,7 +41,7 @@ size_t fx_amb_record_bytes();
 // SMs of the current device: the grid-size rules of the launchers scale with it
 int sm_count();
 // occupancy bits -> the {occupancy word, candidate-summary word} pairs in bricks (mplx_pack.cuh; mplx_fx.cu)
-cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint2 *d_out,
+cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint32_t *d_out,
                              cudaStream_t st);
 // bytes -> 1 bit/voxel: occ ? (byte == 100) : (byte != 0)
 cudaError_t launch_pack_bits(const int8_t *d_bytes, size_t nvox, uint32_t *d_bits, bool occ, cudaStream_t st);

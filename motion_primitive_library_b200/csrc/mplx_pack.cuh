@@ -59,19 +59,22 @@ __host__ __device__ inline uint32_t occ2_summary_word(const uint32_t *occ, size_
 
 // ---- occ2: the {occupancy, candidate-summary} pairs of the fixed-point sample loop, in bricks ----
 // The words above are in voxel order; occ2 stores the same bits in bricks so that a primitive's
-// consecutive samples, and the 27 primitives of a node, fall on few cache lines.
+// consecutive samples, and the 27 primitives of a node, fall on few cache lines.  The buffer holds the
+// two halves of the pairs apart: word p (p < occ2_pair_count) is the occupancy word of pair p and word
+// occ2_pair_count + p its summary word.  Only uncertain samples (~3 %) read the summary half, so the
+// occupancy half alone is what the sample loop keeps hot: 16 MiB at 512^3, which the H100's persisting
+// L2 carve-out (31.2 MiB) holds whole, where the interleaved 32 MiB did not fit.
 //   3-D: bricks of 8x8x8 voxels, counted ceil(nx/8) x ceil(ny/8) x ceil(nz/8), x fastest.  Inside a
 //        brick local = x&7 | (y&7)<<3 | (z&7)<<6; the cell's pair is local>>5 and its bit local&31.
 //   2-D: bricks of 32x16 voxels, counted ceil(nx/32) x ceil(ny/16); pair y&15, bit x&31.
-// A brick is 16 pairs (uint2 {occupancy word, summary word}) = one 128-byte line, so the certain and
-// the uncertain read of a cell hit the same line.  Padding bits (cells past the map's edge) are 1 in
-// both words: such a cell can never look free.
+// A brick is 16 words = 64 bytes in each half.  Padding bits (cells past the map's edge) are 1 in both
+// words: such a cell can never look free.
 constexpr int kOcc2BrickPairs = 16;
 
 __host__ __device__ inline int occ2_bricks_x(int dim, int nx) { return dim == 3 ? (nx + 7) >> 3 : (nx + 31) >> 5; }
 __host__ __device__ inline int occ2_bricks_y(int dim, int ny) { return dim == 3 ? (ny + 7) >> 3 : (ny + 15) >> 4; }
 
-// pairs of the whole buffer (nz = 1 in 2-D)
+// pairs of the whole buffer (nz = 1 in 2-D): the words of each half
 __host__ __device__ inline size_t occ2_pair_count(int dim, int nx, int ny, int nz) {
   const size_t bz = dim == 3 ? (size_t)((nz + 7) >> 3) : 1;
   return (size_t)occ2_bricks_x(dim, nx) * occ2_bricks_y(dim, ny) * bz * kOcc2BrickPairs;

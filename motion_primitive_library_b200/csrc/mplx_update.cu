@@ -45,7 +45,8 @@ __global__ void repack_occ_kernel(const uint32_t *__restrict__ idx, int n, const
 // predecessor in the sorted list is the voxel before it in x within the same brick row (not at either end
 // of the row) reaches no pair the predecessor does not, and is skipped; duplicates are skipped too.
 __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, const uint32_t *__restrict__ occ, size_t nvox,
-                                   int dim, int nx, int ny, int nz, uint2 *__restrict__ occ2) {
+                                   int dim, int nx, int ny, int nz, uint32_t *__restrict__ occ2) {
+  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
   const size_t sxy = (size_t)nx * ny;
   const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
   const int xmask = dim == 3 ? 7 : 31;  // x extent of a brick row - 1
@@ -67,7 +68,8 @@ __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, cons
           done[nd++] = p;
           uint32_t o, s;
           occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
-          occ2[p] = make_uint2(o, s);
+          occ2[p] = o;
+          occ2[npairs + p] = s;
         }
   }
 }
@@ -75,8 +77,8 @@ __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, cons
 // The pairs in voxel order, as mplx_read_map returns them: pair w holds the occupancy word w and the summary
 // bits of voxels 32w..32w+31, gathered from the bricks; bits at i >= nvox read as they did in voxel order
 // (occupancy 0, summary 1).
-__global__ void unbrick_occ2_kernel(const uint2 *__restrict__ occ2, size_t nvox, int dim, int nx, int ny,
-                                    uint2 *__restrict__ out) {
+__global__ void unbrick_occ2_kernel(const uint32_t *__restrict__ occ2, size_t npairs, size_t nvox, int dim, int nx,
+                                    int ny, uint2 *__restrict__ out) {
   const size_t nwords = (nvox + 31) >> 5, sxy = (size_t)nx * ny;
   const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
   for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < nwords; w += (size_t)gridDim.x * blockDim.x) {
@@ -90,9 +92,8 @@ __global__ void unbrick_occ2_kernel(const uint2 *__restrict__ occ2, size_t nvox,
       const int x = (int)(i % nx), y = (int)(i / nx % ny), z = (int)(i / sxy);
       const unsigned p = dim == 3 ? occ2_pair<3>(x, y, z, nbx, nby) : occ2_pair<2>(x, y, 0, nbx, nby);
       const unsigned bit = dim == 3 ? occ2_bit<3>(x, y) : occ2_bit<2>(x, y);
-      const uint2 q = occ2[p];
-      o |= ((q.x >> bit) & 1u) << b;
-      s |= ((q.y >> bit) & 1u) << b;
+      o |= ((occ2[p] >> bit) & 1u) << b;
+      s |= ((occ2[npairs + p] >> bit) & 1u) << b;
     }
     out[w] = make_uint2(o, s);
   }
@@ -168,7 +169,8 @@ extern "C" int mplx_read_map(mplx_ctx *c, int8_t *grid, uint32_t *occ, uint32_t 
     ScopedDevBuf<uint2> tmp;
     CU(tmp.reserve(nwords));
     const int grid = grid_for_entries(nwords < (1u << 30) ? (int)nwords : 1 << 30);
-    unbrick_occ2_kernel<<<grid, 256, 0, st>>>(c->occ2.p, c->nvox, c->dim, c->P.mdim[0], c->P.mdim[1], tmp.p);
+    unbrick_occ2_kernel<<<grid, 256, 0, st>>>(c->occ2.p, c->P.occ2_sum, c->nvox, c->dim, c->P.mdim[0], c->P.mdim[1],
+                                              tmp.p);
     CU(cudaGetLastError());
     c->launches += 1;
     CU(cudaMemcpyAsync(occ2, tmp.p, nwords * sizeof(uint2), cudaMemcpyDeviceToHost, st));
