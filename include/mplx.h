@@ -444,6 +444,65 @@ int mplx_traj_scale(mplx_ctx *ctx, int n_paths, const int64_t *offset, const dou
                     int mode, const double *mv, const double *ri, const double *rf, int n_samples,
                     mplx_traj_scale_out *out);
 
+/* ---- checking trajectories against the map and the limits ------------------------------------ */
+
+/* Largest sample count n that a trajectory or segment check evaluates (traverse_trajectory's N, is_free's n).
+ * Beyond it the reference would allocate n + 1 samples; the checks report the path not evaluated or the
+ * segment not free instead. */
+#define MPLX_SAMPLE_N_MAX (1 << 20)
+
+/* Results of mplx_traj_check (HOST arrays), slots as mplx_traj_out's. */
+typedef struct {
+  int32_t *status;    /* [n_paths] 1: cost evaluated; 0: not (fewer than 2 waypoints, a segment time <= 0 or not
+                         finite, a coefficient not finite, or N = ceil(v_max * total / res) outside
+                         [1, MPLX_SAMPLE_N_MAX])                                                             */
+  double *cost;       /* [n_paths] env_map::traverse_trajectory: +inf when a counted sample leaves the map or
+                         hits an obstacle, else the potential terms' sum (0 without a potential map); 0 for
+                         status 0                                                                            */
+  uint8_t *seg_free;  /* NULL, or [n_wp] env_map::is_free(segment j) at slot offset[p] + j; the path's last slot
+                         and every slot of a path with a bad segment time or coefficient hold 0              */
+  uint8_t *seg_valid; /* NULL, or [n_wp] validate_primitive(segment j, v_max, a_max, j_max, yaw_max), slots as
+                         seg_free's                                                                          */
+  double seconds;     /* out: device time of the kernels (CUDA events)                                       */
+} mplx_traj_check_out;
+
+/* Checks n_paths trajectories against the ctx's map and parameters on the device, as the reference's env_map
+ * and validate_primitive do after the same mplx_set_map / mplx_set_potential (or mplx_update_potential_map) /
+ * mplx_set_search_region / mplx_set_params calls.  The trajectories are mplx_traj_out's layout (offset, seg_t,
+ * coeff), so mplx_traj_solve's output feeds straight in; total_t, n_lambda and lambda (mplx_traj_scale_out's,
+ * all three or none) add mplx_traj_scale's time scaling, path p scaled when n_lambda[p] > 0.  control[p] is the
+ * control flag of path p's segments (a TrajSolver segment carries its first waypoint's control); it may be
+ * NULL when seg_valid is.
+ *   cost: traverse_trajectory (env_map.h:228-255).  N = ceil(v_max * total / res) with the path's (scaled)
+ *     total time; the N + 1 rows of Trajectory::sample(N).  A sample counts when its getIndex(floatToInt(pos)),
+ *     wrapped to 32 bits, differs from the previous sample's (-1 before the first).  A counted sample outside
+ *     the map, or with a potential map installed at a potential >= 100, or without one in an occupied cell,
+ *     makes the cost +inf; otherwise, with a potential map, a counted sample with 0 < potential < 100 adds
+ *     potential_weight * potential + gradient_weight * |vel|, summed in sample order.  No search-region test.
+ *   seg_free: is_free(segment) (env_map.h:60-76): the n + 1 samples of Primitive::sample(n), n =
+ *     ceil(max_v * T / res), max_v the largest Primitive::max_vel over the axes; a sample that is occupied,
+ *     outside the map or outside the search region makes it not free.  A stationary segment (n = 0) samples at
+ *     t = NaN, outside the map: not free.  n above MPLX_SAMPLE_N_MAX: not free.  No time scaling enters.
+ *   seg_valid: validate_primitive (primitive.h:449-525) by control[p]: validate_xxx per axis (max_vel,
+ *     max_acc, max_jrk; a limit <= 0 passes) and validate_yaw at the segment's two ends.
+ * Each path is what the host env_map_host / validate_primitive give (mpl_host.hpp): cost and status bit for bit
+ * without scaling; seg_free and seg_valid bit for bit for VEL and ACC segments, and for JRK ones except where
+ * CUDA's cbrt / acos / cos put max_vel on the other side of an integer or a limit; with a yaw control
+ * validate_yaw uses CUDA's sin / cos, so seg_valid may also differ where d is within 1e-12 of cos(yaw_max).  A
+ * scaled path's samples pass through the closed-form quartic of Lambda::getTau, whose roots are not bitwise the
+ * host's, so its cost may differ in three ways (DESIGN.md §8): a sample within 1e-9 (1 + |x|) of a cell boundary
+ * can change cell; with a gradient weight, the |vel| = v / lambda of the terms carries the root's rounding, so the
+ * sum may differ by about 1e-9 relative where every cell agrees; and the final sample, whose time can land an ulp
+ * past the last lambda segment, can be the start state on one side and a root near the end on the other.  Each
+ * path's outputs do not depend on the other paths.  Scratch is kept in the ctx.
+ * Refusals, each with MPLX_ERR_ARG, the outputs untouched and no launch: no map or no parameters, n_paths < 0,
+ * offset NULL, offset[0] != 0 or decreasing, out / status / cost NULL, seg_t or coeff NULL with waypoints,
+ * control NULL with seg_valid, only some of total_t / n_lambda / lambda given, and n_lambda[p] outside
+ * [0, n_wp(p) * 5 * dim].  Synchronous. */
+int mplx_traj_check(mplx_ctx *ctx, int n_paths, const int64_t *offset, const double *seg_t, const double *coeff,
+                    const uint8_t *control, const double *total_t, const int32_t *n_lambda, const double *lambda,
+                    mplx_traj_check_out *out);
+
 /* Kernel selection (diagnostics): 0 = auto (occupancy planning without a yaw control: the fixed-point
  * kernels, 5; otherwise the dealing kernel for JRK/SNP controls, yaw controls and potential-field
  * planning once a batch fills the GPU, else the register kernel),

@@ -54,6 +54,7 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_grow_results",
     "mplx_traj_solve",
     "mplx_traj_scale",
+    "mplx_traj_check",
     "mplx_set_kernel",
     "mplx_sync",
     "mplx_launch_count",
@@ -164,6 +165,18 @@ class TrajScaleOut(C.Structure):
     ]
 
 
+class TrajCheckOut(C.Structure):
+    """mplx_traj_check_out"""
+
+    _fields_ = [
+        ("status", C.c_void_p),
+        ("cost", C.c_void_p),
+        ("seg_free", C.c_void_p),
+        ("seg_valid", C.c_void_p),
+        ("seconds", C.c_double),
+    ]
+
+
 class MplxError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libmplx error {code}: {msg}")
@@ -239,6 +252,8 @@ def load() -> C.CDLL:
     lib.mplx_traj_solve.restype = i32
     lib.mplx_traj_scale.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(TrajScaleOut)]
     lib.mplx_traj_scale.restype = i32
+    lib.mplx_traj_check.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, C.POINTER(TrajCheckOut)]
+    lib.mplx_traj_check.restype = i32
     lib.mplx_set_kernel.argtypes = [vp, i32]
     lib.mplx_set_kernel.restype = i32
     lib.mplx_sync.argtypes = [vp]

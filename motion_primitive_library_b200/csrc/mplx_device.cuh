@@ -6,6 +6,7 @@
 // round-half-away (round()), and the reference's operand association.  Citations are
 // path:line relative to the reference checkout.
 #pragma once
+#include <limits.h>
 #include <stdint.h>
 
 namespace mplx {
@@ -114,6 +115,17 @@ __device__ __forceinline__ double round_haz(double x, int &k) {
     if (f < 0.0 && x < 0.0) { kd -= 1.0; k -= 1; }  // rounded up to even: away from zero is down
   }
   return kd;
+}
+
+// floatToInt (map_util.h:103-108): (int)std::round((p - origin)/res - 0.5), true division.
+// NaN / out-of-int-range inputs convert to INT_MIN, the x86-64 cvttsd2si result the reference
+// build produces for them (a sample there is outside every map).
+__device__ __forceinline__ int float_to_int(double p, double origin, double res) {
+  const double x = (p - origin) / res - 0.5;
+  if (!(fabs(x) < 2147483648.0)) return INT_MIN;
+  int k;
+  round_haz(x, k);
+  return k;
 }
 
 // `int id = std::round(x / res)` (waypoint.h:97,101,105,109,115); rinv = RN(1/res)

@@ -161,8 +161,9 @@ struct UpdateBufs {
   }
 };
 
-// inputs, outputs and per-waypoint scratch of mplx_traj_solve and mplx_traj_scale (mplx_traj.cu), sized by the
-// largest batch so far; the second line of members is mplx_traj_scale's alone
+// inputs, outputs and per-waypoint scratch of mplx_traj_solve, mplx_traj_scale and mplx_traj_check (mplx_traj.cu),
+// sized by the largest batch so far; the second line of members is mplx_traj_scale's and mplx_traj_check's, the
+// third mplx_traj_check's alone
 struct TrajBufs {
   DevBuf<long long> offset;
   DevBuf<mplx_waypoint> wps;
@@ -171,11 +172,15 @@ struct TrajBufs {
   DevBuf<double> dts, seg_t, taus, coeff, samples, fac, dpos, dyaw;
   DevBuf<int32_t> n_cand, n_knot;
   DevBuf<double> par, total, seg_T, cand, cand_p, knot_t, knot_p, lam, lam_T;
+  DevBuf<int32_t> n_pts;
+  DevBuf<uint8_t> form, seg_free, seg_valid;
+  DevBuf<double> cost;
   void release() {
     offset.release(); wps.release(); ctl.release(); mono.release(); status.release(); dts.release(); seg_t.release();
     taus.release(); coeff.release(); samples.release(); fac.release(); dpos.release(); dyaw.release();
     n_cand.release(); n_knot.release(); par.release(); total.release(); seg_T.release(); cand.release();
     cand_p.release(); knot_t.release(); knot_p.release(); lam.release(); lam_T.release();
+    n_pts.release(); form.release(); seg_free.release(); seg_valid.release(); cost.release();
   }
 };
 

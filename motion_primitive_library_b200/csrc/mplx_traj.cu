@@ -1,4 +1,5 @@
-// mplx_traj.cu — TrajSolver for batches of paths (mplx_traj_solve, include/mplx.h).
+// mplx_traj.cu — TrajSolver for batches of paths (mplx_traj_solve, include/mplx.h), their time scaling
+// (mplx_traj_scale) and their checks against the map and the dynamic limits (mplx_traj_check).
 //
 // The reference (src/mpl_traj_solver/poly_solver.cpp) assembles dense (S*N) x (S*N) matrices for a path of S
 // segments and LU-factors them.  Here each path is solved in O(S): the cost of segment i in the derivatives at
@@ -12,6 +13,7 @@
 //                       operand order (include/mpl_basis/trajectory.h:100-137, primitive.h:128-145)
 #include <algorithm>
 
+#include "mplx_dispatch.h"
 #include "mplx_internal.h"
 
 namespace mplx {
@@ -726,6 +728,36 @@ __device__ __forceinline__ double max_vel(const double *c, double t) {
   return m;
 }
 
+// Primitive1D::extrema_a (primitive.h:169-179) with Primitive::max_acc (:369-379)
+__device__ __forceinline__ double max_acc(const double *c, double t) {
+  double r[4];
+  const int n = solve_roots(0, 0, c[0] / 2, c[1], c[2], r);
+  const double a0 = fabs(pr_a(c, 0)), a1 = fabs(pr_a(c, t));
+  double m = a0 < a1 ? a1 : a0;  // std::max
+  for (int k = 0; k < n; k++) {
+    if (r[k] > 0 && r[k] < t) {
+      const double a = fabs(pr_a(c, r[k]));
+      m = a > m ? a : m;
+    } else if (r[k] >= t) {
+      break;
+    }
+  }
+  return m;
+}
+// Primitive1D::extrema_j (primitive.h:186-193) with Primitive::max_jrk (:384-394)
+__device__ __forceinline__ double max_jrk(const double *c, double t) {
+  const double j0 = fabs(pr_j(c, 0)), j1 = fabs(pr_j(c, t));
+  double m = j0 < j1 ? j1 : j0;
+  if (c[0] != 0) {
+    const double ts = -c[1] * 2 / c[0];
+    if (ts > 0 && ts < t) {
+      const double j = fabs(pr_j(c, ts));
+      m = j > m ? j : m;
+    }
+  }
+  return m;
+}
+
 // LambdaSeg (lambda.h:24-71): the Hermite fit by Gauss-Jordan inversion as on the host (mpl_host.hpp)
 struct LSeg {
   double a[4], ti, tf, dT;
@@ -989,6 +1021,32 @@ __device__ __forceinline__ double get_tau(const double *lam, const double *lT, i
   return -1;
 }
 
+// Trajectory::evaluate(time, Command&) (trajectory.h:100-137) of a path whose segment times are all positive:
+// getTau, the clamp of tau to [0, total], the lambda lookup and eval_row.  nl = 0: no lambda (tau = time).
+template <int DIM>
+__device__ __forceinline__ void traj_row(const double *taus, int S, const double *coeff, const double *lam,
+                                         const double *lT, int nl, bool lam_mono, double total, double time,
+                                         double *row) {
+  double tau = time, lambda = 1, lambda_dot = 0;
+  if (nl > 0) tau = get_tau(lam, lT, nl, lam_mono, time);
+  if (tau < 0) tau = 0;
+  if (tau > total) tau = total;
+  if (nl > 0) {
+    // Lambda::evaluate: the first segment with ti <= tau < tf, else (tau at the last tf) the last one
+    int lo = 0, hi = nl - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (lam[mid * 7 + 5] > tau) hi = mid;
+      else lo = mid + 1;
+    }
+    const double *a = lam + lo * 7;
+    lambda = a[0] * power(tau, 3) + a[1] * tau * tau + a[2] * tau + a[3];
+    lambda_dot = 3 * a[0] * tau * tau + 2 * a[1] * tau + a[2];
+  }
+  // the running sum of positive segment times never decreases
+  eval_row<DIM>(taus, S, true, coeff, tau, time, lambda, lambda_dot, row);
+}
+
 template <int DIM>
 __global__ void __launch_bounds__(128) scale_sample_kernel(ScaleArgs A) {
   constexpr int NC = kCand * DIM;
@@ -1004,30 +1062,11 @@ __global__ void __launch_bounds__(128) scale_sample_kernel(ScaleArgs A) {
     if (st) {
       const long long b = A.offset[p];
       const int S = (int)(A.offset[p + 1] - b) - 1;
-      const double *taus = A.taus + b;
       const double total = A.total[p];
       const double dt = total / A.n_samples;
-      const double time = i * dt;
-      double tau = time, lambda = 1, lambda_dot = 0;
       const int nl = st == 1 ? A.n_knot[p] - 1 : 0;
-      const double *lam = A.lam + b * NC * 7;
-      if (nl > 0) tau = get_tau(lam, A.lam_T + b * NC, nl, A.lam_mono[p] != 0, time);
-      if (tau < 0) tau = 0;
-      if (tau > total) tau = total;
-      if (nl > 0) {
-        // Lambda::evaluate: the first segment with ti <= tau < tf, else (tau at the last tf) the last one
-        int lo = 0, hi = nl - 1;
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (lam[mid * 7 + 5] > tau) hi = mid;
-          else lo = mid + 1;
-        }
-        const double *a = lam + lo * 7;
-        lambda = a[0] * power(tau, 3) + a[1] * tau * tau + a[2] * tau + a[3];
-        lambda_dot = 3 * a[0] * tau * tau + 2 * a[1] * tau + a[2];
-      }
-      // the running sum of positive segment times never decreases
-      eval_row<DIM>(taus, S, true, A.coeff + b * (DIM + 1) * 6, tau, time, lambda, lambda_dot, row);
+      traj_row<DIM>(A.taus + b, S, A.coeff + b * (DIM + 1) * 6, A.lam + b * NC * 7, A.lam_T + b * NC, nl,
+                    A.lam_mono[p] != 0, total, i * dt, row);
     }
     double *o = A.samples + g * RW;
 #pragma unroll
@@ -1137,6 +1176,366 @@ extern "C" int mplx_traj_scale(mplx_ctx *c, int n_paths, const int64_t *offset, 
   CU(cudaStreamSynchronize(st));
   if (out->n_lambda)
     for (int p = 0; p < n_paths; p++) out->n_lambda[p] = out->status[p] == 1 ? nk[p] - 1 : 0;
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  out->seconds = ms * 1e-3;
+  return MPLX_OK;
+}
+
+// ---- checking trajectories against the map and the limits (mplx_traj_check, include/mplx.h) -------------------
+//   check_path_kernel    one thread per path: segment-time checks, the running sums of segment times and of the
+//                        lambda segments' dT, the total time and N = ceil(v_max * total / res)
+//   check_seg_kernel     one thread per segment: finite coefficients; is_free(segment) over its n + 1 samples
+//                        and validate_primitive
+//   check_sample_kernel  one warp per path: traverse_trajectory over the N + 1 samples, 32 at a time.  Lane l
+//                        takes sample base + l; the previous sample's cell index comes from lane l - 1, and from
+//                        the chunk before for lane 0.  The first counted sample that returns +inf ends the path
+//                        (a ballot); with a potential map the chunk's terms are added to the running cost one
+//                        lane after another in sample order, so the sum is the host's left-to-right sum.
+namespace mplx {
+namespace {
+
+struct CheckArgs {
+  int n_paths;
+  const long long *offset;
+  const double *seg_t, *coeff;
+  const double *total_in, *lam;  // NULL: no path is scaled
+  const int32_t *n_lam;
+  const uint8_t *ctl;
+  int32_t *status, *n_pts;  // n_pts: N of traverse_trajectory, 0 when outside [1, MPLX_SAMPLE_N_MAX]
+  uint8_t *form;            // per path: at least 2 waypoints, every segment time and coefficient usable
+  uint8_t *lam_mono;
+  double *taus, *lam_T, *total, *cost;
+  uint8_t *seg_free, *seg_valid;  // NULL: not asked for
+};
+
+template <int DIM>
+__global__ void __launch_bounds__(128) check_path_kernel(const __grid_constant__ EnvParams P, CheckArgs A) {
+  constexpr int NC = kCand * DIM;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int W = (int)(A.offset[p + 1] - b);
+  bool ok = W >= 2;
+  // Trajectory's constructor: taus[j+1] = t_j + taus[j]
+  if (W > 0) A.taus[b] = 0.0;
+  for (int j = 0; j + 1 < W; j++) {
+    const double t = A.seg_t[b + j];
+    ok = ok && pos_finite(t);
+    A.taus[b + j + 1] = t + A.taus[b + j];
+  }
+  // Lambda::getTau's running T += dT, as mplx_traj_scale keeps it
+  const int nl = A.lam ? A.n_lam[p] : 0;
+  bool mono = true;
+  if (nl > 0) {
+    const double *lam = A.lam + b * NC * 7;
+    double *lT = A.lam_T + b * NC;
+    double T = 0;
+    lT[0] = 0;
+    for (int k = 0; k < nl; k++) {
+      const double Tn = T + lam[k * 7 + 6];
+      mono = mono && Tn >= T;
+      lT[k + 1] = T = Tn;
+    }
+  }
+  A.lam_mono[p] = mono ? 1 : 0;
+  const double total = nl > 0 ? A.total_in[p] : (W > 0 ? A.taus[b + W - 1] : 0.0);
+  A.total[p] = total;
+  const double nd = ceil(P.v_max * total / P.res);
+  A.n_pts[p] = nd >= 1 && nd <= MPLX_SAMPLE_N_MAX ? (int)nd : 0;
+  A.form[p] = ok ? 1 : 0;
+}
+
+// env_map::is_free(pr) (env_map.h:60-76) of one segment
+template <int DIM>
+__device__ bool seg_is_free(const EnvParams &P, const double *c, double t) {
+  double max_v = 0;
+#pragma unroll
+  for (int a = 0; a < DIM; a++) {
+    const double mv = max_vel(c + a * 6, t);
+    if (mv > max_v) max_v = mv;
+  }
+  const double nd = ceil(max_v * t / P.res);
+  if (!(nd <= MPLX_SAMPLE_N_MAX)) return false;
+  const int n = (int)nd;
+  const double dt = t / n;  // n = 0: every sample time is 0 * inf = NaN, outside the map
+  for (int i = 0; i <= n; i++) {
+    int pn[DIM];
+    bool inside = true;
+#pragma unroll
+    for (int a = 0; a < DIM; a++) {
+      pn[a] = float_to_int(pr_p(c + a * 6, i * dt), P.origin[a], P.res);
+      inside = inside && (unsigned)pn[a] < (unsigned)P.mdim[a];
+    }
+    if (!inside) return false;
+    int idx = pn[0] + P.mdim[0] * pn[1];
+    if (DIM == 3) idx += P.mdim[0] * P.mdim[1] * pn[DIM - 1];
+    if ((__ldg(P.occ_bits + (idx >> 5)) >> (idx & 31)) & 1u) return false;
+    if (P.region_bits != nullptr && !((__ldg(P.region_bits + (idx >> 5)) >> (idx & 31)) & 1u)) return false;
+  }
+  return true;
+}
+
+// validate_xxx (primitive.h:476-493): ORD 1 max_vel, 2 max_acc, 3 max_jrk of every axis within mx
+template <int DIM, int ORD>
+__device__ bool validate_axes(const double *c, double t, double mx) {
+  if (mx <= 0) return true;
+  for (int a = 0; a < DIM; a++) {
+    const double m = ORD == 1 ? max_vel(c + a * 6, t) : ORD == 2 ? max_acc(c + a * 6, t) : max_jrk(c + a * 6, t);
+    if (m > mx) return false;
+  }
+  return true;
+}
+
+// validate_yaw (primitive.h:503-525): the velocity's direction against the yaw at both ends
+template <int DIM>
+__device__ bool validate_yaw_ends(const EnvParams &P, const double *c, double t) {
+  if (P.yaw_max <= 0) return true;
+  for (int e = 0; e < 2; e++) {
+    const double te = e == 0 ? 0.0 : t;
+    const double v0 = pr_v(c, te), v1 = pr_v(c + 6, te);
+    if (v0 != 0 || v1 != 0) {
+      const double yaw = normalize_angle(pr_p(c + DIM * 6, te));
+      double sn, cs;
+      sincos(yaw, &sn, &cs);
+      if (dot2_normalized(v0, v1, cs, sn) < P.cos_yaw_max) return false;
+    }
+  }
+  return true;
+}
+
+// validate_primitive (primitive.h:449-470), branch by branch
+template <int DIM>
+__device__ bool seg_valid(const EnvParams &P, const double *c, double t, int control) {
+  switch (control) {
+    case MPLX_ACC: return validate_axes<DIM, 1>(c, t, P.v_max);
+    case MPLX_JRK: return validate_axes<DIM, 1>(c, t, P.v_max) && validate_axes<DIM, 2>(c, t, P.a_max);
+    case MPLX_SNP:
+      return validate_axes<DIM, 1>(c, t, P.v_max) && validate_axes<DIM, 2>(c, t, P.a_max) &&
+             validate_axes<DIM, 3>(c, t, P.j_max);
+    case MPLX_VELxYAW: return validate_yaw_ends<DIM>(P, c, t);
+    case MPLX_ACCxYAW: return validate_yaw_ends<DIM>(P, c, t) && validate_axes<DIM, 1>(c, t, P.v_max);
+    case MPLX_JRKxYAW:
+      return validate_yaw_ends<DIM>(P, c, t) && validate_axes<DIM, 1>(c, t, P.v_max) &&
+             validate_axes<DIM, 2>(c, t, P.a_max);
+    case MPLX_SNPxYAW:
+      return validate_yaw_ends<DIM>(P, c, t) && validate_axes<DIM, 1>(c, t, P.v_max) &&
+             validate_axes<DIM, 2>(c, t, P.a_max) && validate_axes<DIM, 3>(c, t, P.j_max);
+    default: return true;
+  }
+}
+
+template <int DIM>
+__global__ void __launch_bounds__(128) check_seg_kernel(const __grid_constant__ EnvParams P, CheckArgs A, long long n_wp) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < n_wp; s += (long long)gridDim.x * blockDim.x) {
+    const int p = path_of(A.offset, A.n_paths, s);
+    const long long b = A.offset[p];
+    const int W = (int)(A.offset[p + 1] - b), j = (int)(s - b);
+    bool fr = false, va = false;
+    if (j + 1 < W) {
+      const double *c = A.coeff + s * (DIM + 1) * 6;
+      bool finite = true;
+      for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+      if (!finite) A.form[p] = 0;  // every writer stores 0
+      const double t = A.seg_t[s];
+      if (finite && pos_finite(t)) {
+        if (A.seg_free) fr = seg_is_free<DIM>(P, c, t);
+        if (A.seg_valid) va = seg_valid<DIM>(P, c, t, A.ctl[p]);
+      }
+    }
+    if (A.seg_free) A.seg_free[s] = fr ? 1 : 0;
+    if (A.seg_valid) A.seg_valid[s] = va ? 1 : 0;
+  }
+}
+
+template <int DIM, bool POT>
+__global__ void __launch_bounds__(128) check_sample_kernel(const __grid_constant__ EnvParams P, CheckArgs A) {
+  constexpr int NC = kCand * DIM;
+  constexpr int RW = 4 * DIM + 3;
+  constexpr unsigned kAll = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int n_warps = gridDim.x * (blockDim.x >> 5);
+  for (int p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < A.n_paths; p += n_warps) {
+    const long long b = A.offset[p];
+    const int W = (int)(A.offset[p + 1] - b);
+    const int N = A.form[p] ? A.n_pts[p] : 0;
+    if (!A.form[p]) {  // a path with a bad segment time or coefficient has no segment results either
+      for (int j = lane; j < W; j += 32) {
+        if (A.seg_free) A.seg_free[b + j] = 0;
+        if (A.seg_valid) A.seg_valid[b + j] = 0;
+      }
+    }
+    if (N == 0) {
+      if (lane == 0) {
+        A.status[p] = 0;
+        A.cost[p] = 0.0;
+      }
+      continue;
+    }
+    const double *taus = A.taus + b, *coeff = A.coeff + b * (DIM + 1) * 6;
+    const int nl = A.lam ? A.n_lam[p] : 0;
+    const double *lam = nl > 0 ? A.lam + b * NC * 7 : nullptr, *lT = A.lam_T + b * NC;
+    const bool lam_mono = A.lam_mono[p] != 0;
+    const double total = A.total[p], dt = total / N;  // Trajectory::sample(N)
+    unsigned carry = 0xffffffffu;  // prev_idx = -1
+    double cost = 0.0;
+    bool hit = false;
+    for (int base = 0; base <= N; base += 32) {
+      const int i = base + lane;
+      unsigned idx = 0;
+      bool inside = false;
+      double speed = 0.0;
+      if (i <= N) {
+        double row[RW];
+#pragma unroll
+        for (int k = 0; k < RW; k++) row[k] = 0.0;
+        traj_row<DIM>(taus, W - 1, coeff, lam, lT, nl, lam_mono, total, i * dt, row);
+        int pn[DIM];
+        inside = true;
+#pragma unroll
+        for (int a = 0; a < DIM; a++) {
+          pn[a] = float_to_int(row[a], P.origin[a], P.res);
+          inside = inside && (unsigned)pn[a] < (unsigned)P.mdim[a];
+        }
+        // getIndex before any bounds test, int arithmetic wrapping as on the reference's targets
+        idx = (unsigned)pn[0] + (unsigned)P.mdim[0] * (unsigned)pn[1];
+        if (DIM == 3) idx += (unsigned)P.mdim[0] * (unsigned)P.mdim[1] * (unsigned)pn[DIM - 1];
+        if (POT) {  // Vecf::norm: Eigen's a0 + a1, a0 + (a1 + a2)
+          const double *v = row + DIM;
+          speed = DIM == 2 ? sqrt(v[0] * v[0] + v[1] * v[1]) : sqrt(v[0] * v[0] + (v[1] * v[1] + v[DIM - 1] * v[DIM - 1]));
+        }
+      }
+      unsigned prev = __shfl_up_sync(kAll, idx, 1);
+      if (lane == 0) prev = carry;
+      carry = __shfl_sync(kAll, idx, 31);
+      const bool counted = i <= N && idx != prev;
+      bool bad = false, has_term = false;
+      double term = 0.0;
+      if (counted) {
+        if (!inside) {
+          bad = true;
+        } else if (POT) {
+          const int pv = __ldg(P.pot + idx);
+          if (pv >= 100) bad = true;
+          else if (pv > 0) {
+            term = P.pot_w * pv + P.grad_w * speed;
+            has_term = true;
+          }
+        } else {
+          bad = (__ldg(P.occ_bits + (idx >> 5)) >> (idx & 31)) & 1u;
+        }
+      }
+      if (__ballot_sync(kAll, bad)) {
+        hit = true;
+        break;
+      }
+      if (POT) {
+        for (unsigned m = __ballot_sync(kAll, has_term); m; m &= m - 1) cost = cost + __shfl_sync(kAll, term, __ffs(m) - 1);
+      }
+    }
+    if (lane == 0) {
+      A.status[p] = 1;
+      A.cost[p] = hit ? (double)INFINITY : cost;
+    }
+  }
+}
+
+cudaError_t launch_check(int dim, bool pot, const EnvParams &P, const CheckArgs &A, long long n_wp, cudaStream_t st,
+                         int *launches) {
+  auto grid = [](long long n) { return (int)std::max<long long>(1, std::min<long long>((n + 127) / 128, (long long)sm_count() * 16)); };
+  return with_dim(dim, [&](auto DIM) {
+    check_path_kernel<DIM><<<(A.n_paths + 127) / 128, 128, 0, st>>>(P, A);
+    *launches += 1;
+    if (cudaError_t e = cudaGetLastError()) return e;
+    check_seg_kernel<DIM><<<grid(n_wp), 128, 0, st>>>(P, A, n_wp);
+    *launches += 1;
+    if (cudaError_t e = cudaGetLastError()) return e;
+    return with_bool(pot, [&](auto POT) {
+      check_sample_kernel<DIM, POT><<<grid(32LL * A.n_paths), 128, 0, st>>>(P, A);
+      *launches += 1;
+      return cudaGetLastError();
+    });
+  });
+}
+
+}  // namespace
+}  // namespace mplx
+
+extern "C" int mplx_traj_check(mplx_ctx *c, int n_paths, const int64_t *offset, const double *seg_t,
+                               const double *coeff, const uint8_t *control, const double *total_t,
+                               const int32_t *n_lambda, const double *lambda, mplx_traj_check_out *out) {
+  if (int r = mplx_bind(c)) return r;
+  if (!c->has_map) return fail(MPLX_ERR_ARG, "no map: call mplx_set_map first");
+  if (!c->has_params) return fail(MPLX_ERR_ARG, "no params: call mplx_set_params first");
+  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
+  if (!offset || !out || !out->status || !out->cost) return fail(MPLX_ERR_ARG, "missing array");
+  if (out->seg_valid && !control) return fail(MPLX_ERR_ARG, "seg_valid without control");
+  const bool scaled = lambda != nullptr;
+  if ((total_t != nullptr) != scaled || (n_lambda != nullptr) != scaled)
+    return fail(MPLX_ERR_ARG, "total_t, n_lambda and lambda go together");
+  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
+  for (int p = 0; p < n_paths; p++)
+    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
+  const long long n_wp = offset[n_paths];
+  if (n_wp > 0 && (!seg_t || !coeff)) return fail(MPLX_ERR_ARG, "missing array");
+  const int dim = c->dim;
+  const long long NC = (long long)mplx::kCand * dim;
+  if (scaled)
+    for (int p = 0; p < n_paths; p++)
+      if (n_lambda[p] < 0 || n_lambda[p] > (offset[p + 1] - offset[p]) * NC)
+        return fail(MPLX_ERR_ARG, "n_lambda[%d] = %d outside [0, %lld]", p, n_lambda[p], (offset[p + 1] - offset[p]) * NC);
+  out->seconds = 0.0;
+  if (n_paths == 0) return MPLX_OK;
+  TrajBufs &B = c->tb;
+  const size_t nw = (size_t)std::max<long long>(n_wp, 1);
+  CU(B.offset.reserve(n_paths + 1)); CU(B.status.reserve(n_paths)); CU(B.mono.reserve(n_paths));
+  CU(B.n_pts.reserve(n_paths)); CU(B.form.reserve(n_paths)); CU(B.total.reserve(n_paths)); CU(B.cost.reserve(n_paths));
+  CU(B.seg_t.reserve(nw)); CU(B.taus.reserve(nw)); CU(B.coeff.reserve(nw * (dim + 1) * 6));
+  if (out->seg_free) CU(B.seg_free.reserve(nw));
+  if (out->seg_valid) {
+    CU(B.seg_valid.reserve(nw));
+    CU(B.ctl.reserve(n_paths));
+  }
+  if (scaled) {
+    CU(B.par.reserve(n_paths)); CU(B.n_knot.reserve(n_paths));
+    CU(B.lam.reserve(nw * NC * 7)); CU(B.lam_T.reserve(nw * NC + 1));
+  }
+  cudaStream_t st = c->stream;
+  CU(cudaMemcpyAsync(B.offset.p, offset, sizeof(int64_t) * (n_paths + 1), cudaMemcpyHostToDevice, st));
+  if (n_wp > 0) {
+    CU(cudaMemcpyAsync(B.seg_t.p, seg_t, sizeof(double) * n_wp, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.coeff.p, coeff, sizeof(double) * n_wp * (dim + 1) * 6, cudaMemcpyHostToDevice, st));
+  }
+  if (out->seg_valid) CU(cudaMemcpyAsync(B.ctl.p, control, (size_t)n_paths, cudaMemcpyHostToDevice, st));
+  if (scaled) {
+    CU(cudaMemcpyAsync(B.par.p, total_t, sizeof(double) * n_paths, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.n_knot.p, n_lambda, sizeof(int32_t) * n_paths, cudaMemcpyHostToDevice, st));
+    if (n_wp > 0) CU(cudaMemcpyAsync(B.lam.p, lambda, sizeof(double) * n_wp * NC * 7, cudaMemcpyHostToDevice, st));
+  }
+  mplx::CheckArgs A{n_paths, B.offset.p, B.seg_t.p, B.coeff.p, scaled ? B.par.p : nullptr, scaled ? B.lam.p : nullptr,
+                    scaled ? B.n_knot.p : nullptr, out->seg_valid ? B.ctl.p : nullptr, B.status.p, B.n_pts.p, B.form.p,
+                    B.mono.p, B.taus.p, B.lam_T.p, B.total.p, B.cost.p, out->seg_free ? B.seg_free.p : nullptr,
+                    out->seg_valid ? B.seg_valid.p : nullptr};
+  cudaEvent_t e0, e1;
+  CU(cudaEventCreate(&e0));
+  CU(cudaEventCreate(&e1));
+  int launches = 0;
+  cudaError_t le = cudaEventRecord(e0, st);
+  if (le == cudaSuccess) le = mplx::launch_check(dim, c->P.pot != nullptr, c->P, A, n_wp, st, &launches);
+  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
+  c->launches += launches;
+  if (le != cudaSuccess) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    CU(le);
+  }
+  CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out->cost, B.cost.p, sizeof(double) * n_paths, cudaMemcpyDeviceToHost, st));
+  if (n_wp > 0 && out->seg_free) CU(cudaMemcpyAsync(out->seg_free, B.seg_free.p, (size_t)n_wp, cudaMemcpyDeviceToHost, st));
+  if (n_wp > 0 && out->seg_valid) CU(cudaMemcpyAsync(out->seg_valid, B.seg_valid.p, (size_t)n_wp, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   cudaEventDestroy(e0);

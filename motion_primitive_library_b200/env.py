@@ -15,6 +15,7 @@ import numpy as np
 
 from . import abi
 from .abi import LATTICE_MAX, WAYPOINT_DTYPE, PackedOut, SuccOut
+from .traj import pack_lambda, pack_paths
 
 
 class MapUtil:
@@ -263,6 +264,19 @@ class env_map:
         )
         self._dirty = False
 
+    def _sync_limits(self):
+        """The device parameters for calls that read only the limits (mplx_traj_check): the env's own once set_u and
+        set_control were called; before that, the limits with a stand-in control set of one zero VEL input.  The
+        stand-in leaves the env marked unsynced, so the next expand sends the real U and control (or refuses without
+        them, as before)."""
+        if self.U_ is not None and self.control is not None:
+            self._sync_params()
+            return
+        u = np.zeros((1, self.Dim))
+        abi.check(self._lib.mplx_set_params(self._h, abi.VEL, self.dt_, self.w_, self.wyaw_, self.v_max_, self.a_max_,
+                                            self.j_max_, self.yaw_max_, u.ctypes.data, 1, self.Dim))
+        self._dirty = True
+
     # -- the hot path -----------------------------------------------------------------------
     def expand(self, nodes: np.ndarray, want=("succ", "cost", "action", "key"), pinned: bool = False) -> Expansion:
         """Batched env_map::get_succ through mplx_expand (HOST buffers)."""
@@ -337,6 +351,45 @@ class env_map:
         abi.check(self._lib.mplx_edges_is_free(self._h, parents.ctypes.data, actions.ctypes.data, parents.size,
                                                free.ctypes.data, cost.ctypes.data))
         return free, cost
+
+    def traverse_trajectories(self, results, control, scaled=None, segments=True):
+        """Checks trajectories against this env on the device (mplx_traj_check): per path the cost of
+        env_map::traverse_trajectory (+inf when the trajectory leaves the map or hits an obstacle) and, with
+        `segments`, env_map::is_free and validate_primitive(v_max, a_max, j_max, yaw_max) of every segment.
+        results: dicts with `seg_t` and `coeff`, as TrajSolverBatch.solve returns them; control: the segments'
+        control flag (a TrajSolver segment carries its first waypoint's), one for all paths or one per path;
+        scaled: None, or TrajSolverBatch.scale's results for the same paths (with_lambda=True), whose time
+        scaling then applies.  The checks read the map, the potential field, the search region and the limits;
+        set_u and set_control are not needed (see _sync_limits).  Returns (results,
+        seconds): one dict per path with `status` (1: cost evaluated; 0: not — fewer than 2 waypoints, a bad
+        segment time or coefficient, or N = ceil(v_max * total / res) outside [1, 2^20]), `cost` and, with
+        segments, `seg_free` and `seg_valid` (uint8 per segment); seconds is the device time of the kernels."""
+        self._sync_limits()
+        n_paths = len(results)
+        if scaled is not None and len(scaled) != n_paths:
+            raise ValueError("one scaled result per path")
+        n, offset, seg_t, coeff = pack_paths(results, self.Dim)
+        ctl = np.ascontiguousarray(np.broadcast_to(np.asarray(control, dtype=np.uint8), (n_paths,)))
+        total_t = n_lambda = lam = None
+        if scaled is not None:
+            total_t, n_lambda, lam = pack_lambda(scaled, offset, self.Dim)
+        status = np.zeros(max(n_paths, 1), dtype=np.int32)
+        cost = np.zeros(max(n_paths, 1))
+        free = np.zeros(seg_t.size, dtype=np.uint8) if segments else None
+        valid = np.zeros(seg_t.size, dtype=np.uint8) if segments else None
+        out = abi.TrajCheckOut(status.ctypes.data, cost.ctypes.data, abi.ptr(free), abi.ptr(valid), 0.0)
+        abi.check(self._lib.mplx_traj_check(self._h, n_paths, offset.ctypes.data, seg_t.ctypes.data,
+                                            coeff.ctypes.data, ctl.ctypes.data if n_paths else None, abi.ptr(total_t),
+                                            abi.ptr(n_lambda), abi.ptr(lam), C.byref(out)))
+        res = []
+        for p in range(n_paths):
+            r = dict(status=int(status[p]), cost=float(cost[p]))
+            if segments:
+                s = max(int(n[p]) - 1, 0)
+                r["seg_free"] = free[offset[p]:offset[p] + s].copy()
+                r["seg_valid"] = valid[offset[p]:offset[p] + s].copy()
+            res.append(r)
+        return res, out.seconds
 
     def edge_cells(self, parents: np.ndarray, actions: np.ndarray, table: bool = False):
         """The voxel walk of MapPlanner::getLinkedNodes (map_planner.cpp:135-151) for stored edges:

@@ -218,6 +218,25 @@ struct Primitive1D {
     }
     return ts;
   }
+  /// primitive.h:169-179: the roots of j(t) in (0, t), in solver order, stopping at the first root >= t
+  std::vector<decimal_t> extrema_a(decimal_t t) const {
+    const std::vector<decimal_t> roots = solve(0, 0, c[0] / 2, c[1], c[2]);
+    std::vector<decimal_t> ts;
+    for (const decimal_t it : roots) {
+      if (it > 0 && it < t) ts.push_back(it);
+      else if (it >= t) break;
+    }
+    return ts;
+  }
+  /// primitive.h:186-193: the root of the snap's linear jerk derivative in (0, t)
+  std::vector<decimal_t> extrema_j(decimal_t t) const {
+    std::vector<decimal_t> ts;
+    if (c[0] != 0) {
+      const decimal_t t_sol = -c[1] * 2 / c[0];
+      if (t_sol > 0 && t_sol < t) ts.push_back(t_sol);
+    }
+    return ts;
+  }
   /// primitive.h:92-122
   decimal_t J(decimal_t t, int control) const {
     const int o = control & 15;
@@ -299,6 +318,30 @@ class Primitive {
     }
     return max_v;
   }
+  /// primitive.h:369-379: max |a| along axis k over [0, t] from the ends and extrema_a
+  decimal_t max_acc(int k) const {
+    const std::vector<decimal_t> ts = prs_[k].extrema_a(t_);
+    decimal_t max_a = std::max(std::abs(prs_[k].a(0)), std::abs(prs_[k].a(t_)));
+    for (const decimal_t it : ts) {
+      if (it > 0 && it < t_) {
+        const decimal_t a = std::abs(prs_[k].a(it));
+        max_a = a > max_a ? a : max_a;
+      }
+    }
+    return max_a;
+  }
+  /// primitive.h:384-394: max |j| along axis k over [0, t] from the ends and extrema_j
+  decimal_t max_jrk(int k) const {
+    const std::vector<decimal_t> ts = prs_[k].extrema_j(t_);
+    decimal_t max_j = std::max(std::abs(prs_[k].j(0)), std::abs(prs_[k].j(t_)));
+    for (const decimal_t it : ts) {
+      if (it > 0 && it < t_) {
+        const decimal_t j = std::abs(prs_[k].j(it));
+        max_j = j > max_j ? j : max_j;
+      }
+    }
+    return max_j;
+  }
 
  private:
   decimal_t t_{0};
@@ -306,6 +349,61 @@ class Primitive {
   Primitive1D prs_[Dim];
   Primitive1D pr_yaw_;
 };
+
+/// validate_xxx: primitive.h:476-493 — every axis's max_vel (xxx VEL), max_acc (ACC) or max_jrk (JRK) within
+/// max; a max <= 0 passes
+template <int Dim>
+bool validate_xxx(const Primitive<Dim> &pr, decimal_t max, int xxx) {
+  if (max <= 0) return true;
+  for (int i = 0; i < Dim; i++) {
+    if (xxx == Control::VEL && pr.max_vel(i) > max) return false;
+    else if (xxx == Control::ACC && pr.max_acc(i) > max) return false;
+    else if (xxx == Control::JRK && pr.max_jrk(i) > max) return false;
+  }
+  return true;
+}
+
+/// validate_yaw: primitive.h:503-525 — at both ends, a nonzero planar velocity's direction against the yaw:
+/// v.normalized().dot((cos yaw, sin yaw)) >= cos(my); a my <= 0 passes
+template <int Dim>
+bool validate_yaw(const Primitive<Dim> &pr, decimal_t my) {
+  if (my <= 0) return true;
+  const Waypoint<Dim> ws[2] = {pr.evaluate(0), pr.evaluate(pr.t())};
+  for (const auto &w : ws) {
+    decimal_t v0 = w.vel(0), v1 = w.vel(1);
+    if (v0 != 0 || v1 != 0) {
+      const decimal_t z = v0 * v0 + v1 * v1;  // Eigen's normalized(): divide by sqrt(squaredNorm) when > 0
+      if (z > 0) {
+        const decimal_t n = std::sqrt(z);
+        v0 = v0 / n;
+        v1 = v1 / n;
+      }
+      const decimal_t d = v0 * std::cos(w.yaw) + v1 * std::sin(w.yaw);
+      if (d < std::cos(my)) return false;
+    }
+  }
+  return true;
+}
+
+/// validate_primitive: primitive.h:449-470 — the checks the primitive's control names
+template <int Dim>
+bool validate_primitive(const Primitive<Dim> &pr, decimal_t mv = 0, decimal_t ma = 0, decimal_t mj = 0,
+                        decimal_t myaw = 0) {
+  switch (pr.control()) {
+    case Control::ACC: return validate_xxx(pr, mv, Control::VEL);
+    case Control::JRK: return validate_xxx(pr, mv, Control::VEL) && validate_xxx(pr, ma, Control::ACC);
+    case Control::SNP:
+      return validate_xxx(pr, mv, Control::VEL) && validate_xxx(pr, ma, Control::ACC) && validate_xxx(pr, mj, Control::JRK);
+    case Control::VELxYAW: return validate_yaw(pr, myaw);
+    case Control::ACCxYAW: return validate_yaw(pr, myaw) && validate_xxx(pr, mv, Control::VEL);
+    case Control::JRKxYAW:
+      return validate_yaw(pr, myaw) && validate_xxx(pr, mv, Control::VEL) && validate_xxx(pr, ma, Control::ACC);
+    case Control::SNPxYAW:
+      return validate_yaw(pr, myaw) && validate_xxx(pr, mv, Control::VEL) && validate_xxx(pr, ma, Control::ACC) &&
+             validate_xxx(pr, mj, Control::JRK);
+    default: return true;
+  }
+}
 
 /// Command<Dim>: include/mpl_basis/trajectory.h:19-28
 template <int Dim>
@@ -564,6 +662,13 @@ class Trajectory {
     return true;
   }
   const Lambda &lambda() const { return lambda_; }
+  /// A lambda fitted elsewhere (mplx_traj_scale's segments) and the total time it gives, in place of
+  /// scale / scale_down
+  void set_lambda(const Lambda &lambda, decimal_t total_t) {
+    lambda_ = lambda;
+    set_scaled_times();
+    total_t_ = total_t;
+  }
   /// trajectory.h:230-237
   vec_E<Command<Dim>> sample(int N) const {
     vec_E<Command<Dim>> ps(N + 1);
@@ -1164,9 +1269,74 @@ class env_map_host : public env_base<Dim> {
   }
   /// env_map.h:48-51
   bool is_free(const Vecf<Dim> &pt) const override { return map_util_->isFree(map_util_->floatToInt(pt)); }
+  void set_potential_map(const std::vector<int8_t> &map) override { potential_map_ = map; this->touch(); }
+  void set_potential_weight(decimal_t w) override { potential_weight_ = w; this->touch(); }
+  void set_gradient_weight(decimal_t w) override { gradient_weight_ = w; this->touch(); }
+
+  /// env_map.h:60-76: the n + 1 samples of pr.sample(n), n = ceil(max_v * t / res), each one in a free cell of
+  /// the map and, with a search region, inside it.  A stationary primitive (n = 0) samples at t = 0 * inf = NaN,
+  /// which floatToInt makes INT_MIN (x86-64): outside, not free.  n above MPLX_SAMPLE_N_MAX, where the reference
+  /// would allocate the samples: not free.
+  bool is_free(const Primitive<Dim> &pr) const {
+    decimal_t max_v = 0;
+    for (int i = 0; i < Dim; i++)
+      if (pr.max_vel(i) > max_v) max_v = pr.max_vel(i);
+    const decimal_t nd = std::ceil(max_v * pr.t() / map_util_->getRes());
+    if (!(nd <= MPLX_SAMPLE_N_MAX)) return false;
+    const int n = (int)nd;
+    const decimal_t dt = pr.t() / n;
+    for (int i = 0; i <= n; i++) {
+      const Veci<Dim> pn = map_util_->floatToInt(pr.evaluate(i * dt).pos);
+      if (map_util_->isOccupied(pn) || map_util_->isOutside(pn)) return false;
+      if (!this->search_region_.empty() && !this->search_region_[map_util_->getIndex(pn)]) return false;
+    }
+    return true;
+  }
+
+  /// traverse_trajectory's sample count N = ceil(v_max * total / res) (env_map.h:230-231), or 0 where it is not
+  /// in [1, MPLX_SAMPLE_N_MAX]: with the default v_max < 0 the reference asks for a vector of negative size, at
+  /// N = 0 it samples t = 0 * inf = NaN, and above the bound it would allocate the samples.
+  int traverse_samples(const Trajectory<Dim> &traj) const {
+    const decimal_t nd = std::ceil(this->v_max_ * traj.getTotalTime() / map_util_->getRes());
+    return nd >= 1 && nd <= MPLX_SAMPLE_N_MAX ? (int)nd : 0;
+  }
+
+  /// env_map.h:228-255: the cost of traj.sample(N).  A sample counts when its cell index differs from the
+  /// previous sample's (-1 before the first; getIndex before any bounds test, in 32-bit arithmetic that wraps
+  /// as on the reference's targets).  A counted sample outside the map, or with a potential map at a potential
+  /// >= 100, or without one in an occupied cell, returns +inf; with a potential map a counted sample with
+  /// 0 < potential < 100 adds potential_weight * potential + gradient_weight * |vel|, in sample order.  Throws
+  /// std::domain_error where traverse_samples is 0.
+  decimal_t traverse_trajectory(const Trajectory<Dim> &traj) const {
+    const int n = traverse_samples(traj);
+    if (n < 1) throw std::domain_error("traverse_trajectory: N = ceil(v_max * total / res) outside [1, MPLX_SAMPLE_N_MAX]");
+    const Veci<Dim> dim = map_util_->getDim();
+    decimal_t c = 0;
+    const auto pts = traj.sample(n);
+    uint32_t prev_idx = ~0u;
+    for (const auto &pt : pts) {
+      const Veci<Dim> pn = map_util_->floatToInt(pt.pos);
+      uint32_t idx = (uint32_t)pn(0) + (uint32_t)dim(0) * (uint32_t)pn(1);
+      if (Dim == 3) idx += (uint32_t)dim(0) * (uint32_t)dim(1) * (uint32_t)pn(Dim - 1);
+      if (prev_idx == idx) continue;
+      prev_idx = idx;
+      if (map_util_->isOutside(pn)) return std::numeric_limits<decimal_t>::infinity();
+      if (!potential_map_.empty()) {
+        if (potential_map_[idx] < 100 && potential_map_[idx] > 0)
+          c += potential_weight_ * potential_map_[idx] + gradient_weight_ * pt.vel.norm();
+        else if (potential_map_[idx] >= 100)
+          return std::numeric_limits<decimal_t>::infinity();
+      } else if (map_util_->isOccupied(pn)) {
+        return std::numeric_limits<decimal_t>::infinity();
+      }
+    }
+    return c;
+  }
 
  protected:
   std::shared_ptr<MapUtil<Dim>> map_util_;
+  std::vector<int8_t> potential_map_;
+  decimal_t potential_weight_{0.1}, gradient_weight_{0.0};
 };
 
 /// env_map_gpu<Dim>: env_map<Dim> (include/mpl_planner/env/env_map.h) with get_succ served by
@@ -1174,6 +1344,9 @@ class env_map_host : public env_base<Dim> {
 template <int Dim>
 class env_map_gpu : public env_map_host<Dim> {
   using env_map_host<Dim>::map_util_;
+  using env_map_host<Dim>::potential_map_;
+  using env_map_host<Dim>::potential_weight_;
+  using env_map_host<Dim>::gradient_weight_;
 
  public:
   explicit env_map_gpu(std::shared_ptr<MapUtil<Dim>> map_util, int device = 0) : env_map_host<Dim>(map_util) {
@@ -1479,8 +1652,6 @@ class env_map_gpu : public env_map_host<Dim> {
   std::vector<mplx_waypoint> *trace_ = nullptr;
   int control_ = Control::NONE, speculate_ = 1;
   mutable bool potential_on_device_ = false, region_on_device_ = false;
-  std::vector<int8_t> potential_map_;
-  decimal_t potential_weight_{0.1}, gradient_weight_{0.0};
   mutable unsigned long map_version_ = ~0ul, sent_version_ = 0;
   mutable std::unordered_map<std::size_t, Entry> cache_;
   mutable vec_E<Waypoint<Dim>> pending_, batch_;

@@ -668,3 +668,124 @@ int mplh_solve(double a, double b, double c, double d, double e, int32_t *n, dou
   return 0;
 }
 }
+
+/* ---- Trajectory checks (mpl_host.hpp): env_map_host::traverse_trajectory, is_free, validate_primitive ------- */
+
+namespace {
+template <int Dim>
+struct CheckEnv : MPL::env_map_host<Dim> {  // the map queries only: get_succ is never called
+  using MPL::env_map_host<Dim>::env_map_host;
+  void get_succ(const Waypoint<Dim> &, vec_E<Waypoint<Dim>> &, std::vector<decimal_t> &, std::vector<int> &) const override {}
+};
+
+/// whether mplx_traj_check evaluates this path at all: at least one segment, every segment time finite and
+/// > 0, every coefficient finite
+template <int Dim>
+bool checkable(int n_seg, const double *seg_t, const double *coeff) {
+  if (n_seg < 1) return false;
+  for (int j = 0; j < n_seg; j++)
+    if (!(std::isfinite(seg_t[j]) && seg_t[j] > 0)) return false;
+  for (size_t k = 0; k < (size_t)n_seg * (Dim + 1) * 6; k++)
+    if (!std::isfinite(coeff[k])) return false;
+  return true;
+}
+}  // namespace
+
+extern "C" {
+/* mplx_traj_check on the host, the map and parameters given directly: the grid map[prod(mdim)] at origin with
+ * resolution res, potential NULL or [prod(mdim)] with its two weights, region NULL or [prod(mdim)] search-region
+ * bytes, and the limits.  The paths, control, total_t / n_lambda / lambda and the outputs are mplx_traj_check's
+ * (slots as mplx_traj_out's; total_t, n_lambda and lambda all NULL or all given).  Paths are spread over
+ * nthreads threads (< 1: one).  1: bad argument (dim, map, offset, missing arrays, n_lambda out of range). */
+int mplh_traj_check(int dim, const int8_t *map, const int32_t *mdim, const double *origin, double res,
+                    const int8_t *potential, double potential_weight, double gradient_weight, const uint8_t *region,
+                    double v_max, double a_max, double j_max, double yaw_max, int n_paths, const int64_t *offset,
+                    const double *seg_t, const double *coeff, const uint8_t *control, const double *total_t,
+                    const int32_t *n_lambda, const double *lambda, int nthreads, int32_t *status, double *cost,
+                    uint8_t *seg_free, uint8_t *seg_valid) {
+  const bool scaled = lambda != nullptr;
+  if (!map || !mdim || !origin || n_paths < 0 || !offset || offset[0] != 0 || !status || !cost ||
+      (seg_valid && !control) || (total_t != nullptr) != scaled || (n_lambda != nullptr) != scaled) {
+    g_err = "bad argument";
+    return 1;
+  }
+  for (int p = 0; p < n_paths; p++)
+    if (offset[p + 1] < offset[p] ||
+        (scaled && (n_lambda[p] < 0 || n_lambda[p] > (offset[p + 1] - offset[p]) * 5 * dim))) {
+      g_err = "bad argument";
+      return 1;
+    }
+  if (offset[n_paths] > 0 && (!seg_t || !coeff)) { g_err = "bad argument"; return 1; }
+  return with_traj_dim(dim, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    auto mu = std::make_shared<MPL::MapUtil<Dim>>();
+    Vecf<Dim> ori;
+    Veci<Dim> md;
+    size_t nvox = 1;
+    for (int k = 0; k < Dim; k++) {
+      ori(k) = origin[k];
+      md(k) = mdim[k];
+      nvox *= (size_t)mdim[k];
+    }
+    mu->setMap(ori, md, MPL::Tmap(map, map + nvox), res);
+    CheckEnv<Dim> env(mu);
+    env.set_v_max(v_max);
+    env.set_a_max(a_max);
+    env.set_j_max(j_max);
+    env.set_yaw_max(yaw_max);
+    if (potential) {
+      env.set_potential_map(std::vector<int8_t>(potential, potential + nvox));
+      env.set_potential_weight(potential_weight);
+      env.set_gradient_weight(gradient_weight);
+    }
+    if (region) env.set_search_region(std::vector<bool>(region, region + nvox));
+    const size_t NC = (size_t)5 * Dim;
+    auto one = [&](int p) {
+      const int64_t b = offset[p];
+      const int W = (int)(offset[p + 1] - b), S = W - 1;
+      status[p] = 0;
+      cost[p] = 0;
+      for (int j = 0; j < W; j++) {
+        if (seg_free) seg_free[b + j] = 0;
+        if (seg_valid) seg_valid[b + j] = 0;
+      }
+      if (!checkable<Dim>(S, seg_t + b, coeff + b * (Dim + 1) * 6)) return;
+      const int ctl = control ? control[p] : Control::NONE;
+      vec_E<Primitive<Dim>> prs;
+      for (int j = 0; j < S; j++) {
+        vec_E<Vecf<6>> cs(Dim + 1);
+        for (int a = 0; a <= Dim; a++)
+          for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)(b + j) * (Dim + 1) + a) * 6 + k];
+        prs.push_back(Primitive<Dim>(cs, seg_t[b + j], ctl));
+      }
+      Trajectory<Dim> traj(prs);
+      if (scaled && n_lambda[p] > 0) {
+        Lambda lam;
+        for (int k = 0; k < n_lambda[p]; k++) {
+          const double *r = lambda + ((size_t)b * NC + k) * 7;
+          LambdaSeg g;
+          for (int i = 0; i < 4; i++) g.a[i] = r[i];
+          g.ti = r[4]; g.tf = r[5]; g.dT = r[6];
+          lam.segs.push_back(g);
+        }
+        traj.set_lambda(lam, total_t[p]);
+      }
+      if (env.traverse_samples(traj) > 0) {
+        status[p] = 1;
+        cost[p] = env.traverse_trajectory(traj);
+      }
+      for (int j = 0; j < S; j++) {
+        if (seg_free) seg_free[b + j] = env.is_free(traj.segs[j]) ? 1 : 0;
+        if (seg_valid) seg_valid[b + j] = validate_primitive(traj.segs[j], v_max, a_max, j_max, yaw_max) ? 1 : 0;
+      }
+    };
+    const int nt = std::max(1, std::min(nthreads, n_paths));
+    std::atomic<int> next{0};
+    std::vector<std::thread> pool;
+    for (int t = 1; t < nt; t++)
+      pool.emplace_back([&] { for (int p; (p = next++) < n_paths;) one(p); });
+    for (int p; (p = next++) < n_paths;) one(p);
+    for (auto &th : pool) th.join();
+  });
+}
+}

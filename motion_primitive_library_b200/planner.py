@@ -605,3 +605,63 @@ def solve_roots(a, b, c, d, e):
     _traj_lib()
     _, fn = load_solve_fn(LIB, "mplh_solve")
     return run_solve(fn, a, b, c, d, e)
+
+
+def load_traj_check_fn(path, fn):
+    """fn(dim, map, mdim, origin, res, potential, potential_weight, gradient_weight, region, v_max, a_max, j_max,
+    yaw_max, n_paths, offset, seg_t, coeff, control, total_t, n_lambda, lambda, nthreads, status, cost, seg_free,
+    seg_valid): mplh_traj_check's signature (host/mpl_host_capi.cpp)."""
+    L = C.CDLL(str(path))
+    f = getattr(L, fn)
+    vp, d = C.c_void_p, C.c_double
+    f.argtypes = [C.c_int, vp, vp, vp, d, vp, d, d, vp, d, d, d, d, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp,
+                  vp, vp, vp]
+    f.restype = C.c_int
+    return L, f
+
+
+def run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, potential=None, potential_weight=0.1,
+                   gradient_weight=0.0, region=None, v_max=-1.0, a_max=-1.0, j_max=-1.0, yaw_max=-1.0, scaled=None,
+                   nthreads=1):
+    """The map and parameters given directly, the trajectories as TrajSolverBatch results (dicts with `seg_t` and
+    `coeff`; `scaled` as TrajSolverBatch.scale's, with `total_t` and `lambda`), control one flag or one per path.
+    Returns a dict of arrays: `status`, `cost` (one per path), `seg_free` and `seg_valid` (one per waypoint slot,
+    mplx_traj_out's layout) and `offset`."""
+    from .traj import pack_lambda, pack_paths
+
+    _, offset, seg_t, coeff = pack_paths(paths, dim)
+    n_paths = len(paths)
+    ctl = np.ascontiguousarray(np.broadcast_to(np.asarray(control, dtype=np.uint8), (max(n_paths, 1),)))
+    total_t = n_lambda = lam = None
+    if scaled is not None:
+        total_t, n_lambda, lam = pack_lambda(scaled, offset, dim)
+    grid = np.ascontiguousarray(grid, dtype=np.int8).reshape(-1)
+    mdim = np.ascontiguousarray(mdim, dtype=np.int32)
+    origin = np.ascontiguousarray(origin, dtype=np.float64)
+    pot = None if potential is None else np.ascontiguousarray(potential, dtype=np.int8).reshape(-1)
+    reg = None if region is None else np.ascontiguousarray(region, dtype=np.uint8).reshape(-1)
+    status = np.zeros(max(n_paths, 1), dtype=np.int32)
+    cost = np.zeros(max(n_paths, 1))
+    free = np.zeros(seg_t.size, dtype=np.uint8)
+    valid = np.zeros(seg_t.size, dtype=np.uint8)
+
+    def p(a):
+        return None if a is None else a.ctypes.data
+
+    rc = fn(dim, grid.ctypes.data, mdim.ctypes.data, origin.ctypes.data, float(res), p(pot), float(potential_weight),
+            float(gradient_weight), p(reg), float(v_max), float(a_max), float(j_max), float(yaw_max), n_paths,
+            offset.ctypes.data, seg_t.ctypes.data, coeff.ctypes.data, ctl.ctypes.data, p(total_t), p(n_lambda), p(lam),
+            int(nthreads), status.ctypes.data, cost.ctypes.data, free.ctypes.data, valid.ctypes.data)
+    if rc != 0:
+        err = getattr(lib, "mplh_last_error", None)
+        raise RuntimeError(err().decode() if err else f"trajectory check failed rc={rc}")
+    return dict(status=status[:n_paths], cost=cost[:n_paths], seg_free=free[:int(offset[-1])],
+                seg_valid=valid[:int(offset[-1])], offset=offset)
+
+
+def traj_check(dim, grid, mdim, origin, res, paths, control, **kw):
+    """env_map_host::traverse_trajectory, is_free and validate_primitive on the host (mpl_host.hpp) for a batch of
+    trajectories, as mplx_traj_check computes them on the device.  Arguments as run_traj_check."""
+    lib = _traj_lib()
+    _, fn = load_traj_check_fn(LIB, "mplh_traj_check")
+    return run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, **kw)

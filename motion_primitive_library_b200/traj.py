@@ -11,6 +11,39 @@ VEL, ACC, JRK = abi.VEL, abi.ACC, abi.JRK
 SCALE, SCALE_DOWN = abi.TRAJ_SCALE, abi.TRAJ_SCALE_DOWN
 
 
+def pack_paths(results, dim):
+    """The waypoint slots of trajectories given as dicts with `seg_t` and `coeff` (as TrajSolverBatch.solve returns
+    them): (waypoints per path, offset, seg_t, coeff) in mplx_traj_out's layout."""
+    n = np.array([len(r["seg_t"]) + 1 if len(r["seg_t"]) else 0 for r in results], dtype=np.int64)
+    offset = np.zeros(len(results) + 1, dtype=np.int64)
+    np.cumsum(n, out=offset[1:])
+    total = int(offset[-1])
+    seg_t = np.zeros(max(total, 1))
+    coeff = np.zeros((max(total, 1), dim + 1, 6))
+    for p, r in enumerate(results):
+        s = int(n[p]) - 1
+        if s > 0:
+            seg_t[offset[p]:offset[p] + s] = r["seg_t"]
+            coeff[offset[p]:offset[p] + s] = np.asarray(r["coeff"]).reshape(s, dim + 1, 6)
+    return n, offset, seg_t, coeff
+
+
+def pack_lambda(scaled, offset, dim):
+    """total_t, n_lambda and the lambda slots (mplx_traj_scale_out's layout) of TrajSolverBatch.scale's results
+    (with_lambda=True) for the paths at `offset`."""
+    NC = 5 * dim
+    n_paths = len(scaled)
+    total_t = np.zeros(max(n_paths, 1))
+    n_lambda = np.zeros(max(n_paths, 1), dtype=np.int32)
+    lam = np.zeros((max(int(offset[-1]), 1) * NC, 7))
+    for p, r in enumerate(scaled):
+        rows = np.asarray(r["lambda"], dtype=np.float64).reshape(-1, 7)
+        total_t[p] = r["total_t"]
+        n_lambda[p] = len(rows)
+        lam[offset[p] * NC:offset[p] * NC + len(rows)] = rows
+    return total_t, n_lambda, lam
+
+
 class TrajSolverBatch:
     """Smooth many paths at once: for each path, the piecewise polynomial through its waypoints that minimises the
     integral of the squared velocity (control VEL), acceleration (ACC) or jerk (JRK), as TrajSolver<dim> gives it,
@@ -89,17 +122,8 @@ class TrajSolverBatch:
         n_paths = len(results)
         if mode == SCALE_DOWN and mv is None:
             raise ValueError("scale_down needs mv")
-        n = np.array([len(r["seg_t"]) + 1 if len(r["seg_t"]) else 0 for r in results], dtype=np.int64)
-        offset = np.zeros(n_paths + 1, dtype=np.int64)
-        np.cumsum(n, out=offset[1:])
+        n, offset, seg_t, coeff = pack_paths(results, dim)
         total = int(offset[-1])
-        seg_t = np.zeros(max(total, 1))
-        coeff = np.zeros((max(total, 1), dim + 1, 6))
-        for p, r in enumerate(results):
-            s = int(n[p]) - 1
-            if s > 0:
-                seg_t[offset[p]:offset[p] + s] = r["seg_t"]
-                coeff[offset[p]:offset[p] + s] = np.asarray(r["coeff"]).reshape(s, dim + 1, 6)
 
         def per_path(x):
             return np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (n_paths,)))
