@@ -54,6 +54,39 @@ struct ScopedDevBuf : DevBuf<T> {
   ~ScopedDevBuf() { this->release(); }
 };
 
+// The device time of one batch of launches on a stream: an event pair that destroys itself on every exit path
+struct TimedRun {
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  TimedRun() = default;
+  TimedRun(const TimedRun &) = delete;
+  TimedRun &operator=(const TimedRun &) = delete;
+  ~TimedRun() {
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+  }
+  // Records e0, calls launch(int *n) -> cudaError_t, which launches on st and counts its launches in *n, then
+  // records e1; adds *n to launches whether or not a step failed.  Returns the first error.
+  template <class F>
+  cudaError_t run(cudaStream_t st, int64_t &launches, F &&launch) {
+    cudaError_t e = cudaEventCreate(&e0);
+    if (e == cudaSuccess) e = cudaEventCreate(&e1);
+    if (e != cudaSuccess) return e;
+    int n = 0;
+    e = cudaEventRecord(e0, st);
+    if (e == cudaSuccess) e = launch(&n);
+    if (e == cudaSuccess) e = cudaEventRecord(e1, st);
+    launches += n;
+    return e;
+  }
+  // the time between the records, once the caller has synchronised the stream
+  cudaError_t seconds(double *s) const {
+    float ms = 0.f;
+    const cudaError_t e = cudaEventElapsedTime(&ms, e0, e1);
+    *s = ms * 1e-3;
+    return e;
+  }
+};
+
 template <typename T>
 struct PinBuf {
   T *p = nullptr;

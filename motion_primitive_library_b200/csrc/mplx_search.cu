@@ -364,7 +364,7 @@ struct Round {
   std::vector<double> cost;
   std::vector<unsigned long long> offs;  // kDone: the query's place in pool; kPoolFull: the units it needed
   std::vector<uint64_t> pool;            // the result pool, drained
-  float ms = 0;
+  double seconds = 0;  // device time of the round's launch
   int32_t at(RoundField f, int q) const { return ires[(size_t)f * cost.size() + q]; }
 };
 
@@ -426,39 +426,31 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   EnvParams P = c->P;
   P.stats = nullptr;
   const int block = ((nU + 31) / 32) * 32;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  cudaEventRecord(e0, c->stream);
   // worst-case arenas cannot overflow: the capacity check would change nothing
   const bool check = b.max_expand <= 0 || L.cap < 1 + (int64_t)b.max_expand * nU;
-  cudaError_t le = with_search_kernel(P, b.cost_terms, check, [&](auto kernel) {
-    kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
-    return cudaGetLastError();
+  TimedRun timed;
+  const cudaError_t le = timed.run(c->stream, c->launches, [&](int *launches) {
+    return with_search_kernel(P, b.cost_terms, check, [&](auto kernel) {
+      kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
+      const cudaError_t e = cudaGetLastError();
+      if (e == cudaSuccess) *launches += 1;
+      return e;
+    });
   });
-  cudaEventRecord(e1, c->stream);
   if (le != cudaSuccess) {
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     cudaGetLastError();
     return fail(MPLX_ERR_CUDA, "search kernel launch failed: %s", cudaGetErrorString(le));
   }
-  c->launches++;
   R.ires.resize(5 * (size_t)n_q);
   R.cost.resize(n_q);
   R.offs.resize(n_q);
   unsigned long long used = 0;
-  cudaError_t ce = cudaMemcpyAsync(R.ires.data(), B.ires.p, sizeof(int32_t) * R.ires.size(), cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess) ce = cudaMemcpyAsync(R.cost.data(), B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess)
-    ce = cudaMemcpyAsync(R.offs.data(), B.offs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess) ce = cudaMemcpyAsync(&used, B.offs.p + n_q, sizeof used, cudaMemcpyDeviceToHost, c->stream);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-  R.ms = 0;
-  if (ce == cudaSuccess) ce = cudaEventElapsedTime(&R.ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  CU(ce);
+  CU(cudaMemcpyAsync(R.ires.data(), B.ires.p, sizeof(int32_t) * R.ires.size(), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(R.cost.data(), B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(R.offs.data(), B.offs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(&used, B.offs.p + n_q, sizeof used, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(timed.seconds(&R.seconds));
   // the pool is drained before the next round reuses it
   R.pool.resize((size_t)std::min<unsigned long long>(used, (unsigned long long)pool_units));
   if (!R.pool.empty())
@@ -546,7 +538,7 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
   }
   out->slots = (int32_t)slots;
   out->arena_bytes = L.bytes;
-  out->seconds = R.ms * 1e-3;
+  out->seconds = R.seconds;
   return MPLX_OK;
 }
 
@@ -657,7 +649,7 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
     // round completes at least one query
     rc = run_round(c, b, cur, L, slots, std::max(pool_units, again_units), R);
     if (rc) return rc;
-    seconds += R.ms * 1e-3;
+    seconds += R.seconds;
     if (rounds == 0) {
       out->slots = (int32_t)slots;
       out->arena_bytes = L.bytes;

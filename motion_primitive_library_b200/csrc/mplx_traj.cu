@@ -19,7 +19,34 @@
 namespace mplx {
 namespace {
 
-constexpr double kPi = 3.14159265358979323846;
+// The refusals the three batch calls share, in the order they make them.  arrays: offset and the call's other
+// required arrays are given; wp_in: its per-waypoint inputs are given, which may be NULL when no path has a
+// waypoint slot; samples: it is asked for n_samples + 1 sample rows per path.  Sets n_wp = offset[n_paths].
+int check_batch(int n_paths, const int64_t *offset, bool arrays, bool wp_in, bool samples, int n_samples,
+                long long &n_wp) {
+  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
+  if (!offset || !arrays) return fail(MPLX_ERR_ARG, "missing array");
+  if (samples && n_samples <= 0) return fail(MPLX_ERR_ARG, "samples with n_samples <= 0");
+  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
+  for (int p = 0; p < n_paths; p++)
+    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
+  n_wp = offset[n_paths];
+  if (n_wp > 0 && !wp_in) return fail(MPLX_ERR_ARG, "missing array");
+  if (samples && (long long)n_paths * (n_samples + 1) >= ((long long)1 << 40)) return fail(MPLX_ERR_ARG, "too many samples");
+  return MPLX_OK;
+}
+
+// Launches k over n items in blocks of 128 threads, at least one: one thread per item, or, for a grid-stride
+// kernel (stride), at most 16 blocks per SM.  Counts the launch once it is made.
+template <class... P, class... A>
+cudaError_t launch(void (*k)(P...), long long n, bool stride, cudaStream_t st, int *launches, const A &...args) {
+  long long blocks = (n + 127) / 128;
+  if (stride) blocks = std::min<long long>(blocks, (long long)sm_count() * 16);
+  k<<<(int)std::max<long long>(blocks, 1), 128, 0, st>>>(args...);
+  if (cudaError_t e = cudaGetLastError()) return e;
+  *launches += 1;
+  return cudaSuccess;
+}
 
 // Hbar for h = 1, 2, 3: the cost of a unit-duration segment in [start derivatives (h), end derivatives (h)]
 __constant__ double kHbar1[4] = {1, -1, -1, 1};
@@ -338,6 +365,14 @@ __device__ __forceinline__ int path_of(const long long *offset, int n_paths, lon
   return lo;
 }
 
+// every coefficient of one segment (axes, then yaw) is finite
+template <int DIM>
+__device__ __forceinline__ bool coeff_finite(const double *c) {
+  bool finite = true;
+  for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+  return finite;
+}
+
 // Coefficients of one axis of one segment from the derivatives d0 (start) and d1 (end), as Primitive1D holds them
 // (c[5-k] = k! p_k, p_k the coefficient of t^k).
 template <int H>
@@ -387,7 +422,6 @@ __global__ void __launch_bounds__(128) traj_coeff_kernel(TrajArgs A, long long n
       continue;
     }
     const double tau = A.seg_t[s];
-    bool finite = true;
 #pragma unroll
     for (int a = 0; a < DIM; a++) {
       double d0[H], d1[H];
@@ -407,21 +441,15 @@ __global__ void __launch_bounds__(128) traj_coeff_kernel(TrajArgs A, long long n
       }
       seg_coeff<HY>(tau, d0, d1, c + DIM * 6);
     }
-    for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
-    if (!finite) A.status[p] = 0;
+    if (!coeff_finite<DIM>(c)) A.status[p] = 0;
   }
 }
 
-// include/mpl_basis/math.h power / normalize_angle and Primitive1D's evaluators, in the host's operand order
+// include/mpl_basis/math.h power and Primitive1D's evaluators, in the host's operand order
 __device__ __forceinline__ double power(double t, int n) {
   double tn = 1;
   while (n > 0) { tn *= t; n--; }
   return tn;
-}
-__device__ __forceinline__ double normalize_angle(double angle) {
-  while (angle > kPi) angle -= 2.0 * kPi;
-  while (angle < -kPi) angle += 2.0 * kPi;
-  return angle;
 }
 __device__ __forceinline__ double pr_p(const double *c, double t) {
   return c[0] / 120 * power(t, 5) + c[1] / 24 * power(t, 4) + c[2] / 6 * power(t, 3) + c[3] / 2 * t * t + c[4] * t + c[5];
@@ -512,38 +540,24 @@ int order_of(int control) {  // h = N/2 of TrajSolver's PolySolver for this cont
   }
 }
 
-template <int DIM, int H, int HY>
-cudaError_t launch3(const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
-  traj_sweep_kernel<DIM, H, HY><<<(A.n_paths + 127) / 128, 128, 0, st>>>(A);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  if (n_wp > 0) {
-    const long long blocks = std::min<long long>((n_wp + 127) / 128, (long long)sm_count() * 16);
-    traj_coeff_kernel<DIM, H, HY><<<(int)blocks, 128, 0, st>>>(A, n_wp);
-    *launches += 1;
-    if (cudaError_t e = cudaGetLastError()) return e;
-  }
-  if (A.samples) {
-    const long long n = (long long)A.n_paths * (A.n_samples + 1);
-    const long long blocks = std::min<long long>((n + 127) / 128, (long long)sm_count() * 16);
-    traj_sample_kernel<DIM><<<(int)blocks, 128, 0, st>>>(A);
-    *launches += 1;
-    if (cudaError_t e = cudaGetLastError()) return e;
-  }
-  return cudaSuccess;
-}
-
-template <int DIM, int H>
-cudaError_t launch_yaw(int hy, const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
-  if (hy == 1) return launch3<DIM, H, 1>(A, n_wp, st, launches);
-  if (hy == 2) return launch3<DIM, H, 2>(A, n_wp, st, launches);
-  return launch3<DIM, H, 3>(A, n_wp, st, launches);
-}
-template <int DIM>
-cudaError_t launch_dim(int h, int hy, const TrajArgs &A, long long n_wp, cudaStream_t st, int *launches) {
-  if (h == 1) return launch_yaw<DIM, 1>(hy, A, n_wp, st, launches);
-  if (h == 2) return launch_yaw<DIM, 2>(hy, A, n_wp, st, launches);
-  return launch_yaw<DIM, 3>(hy, A, n_wp, st, launches);
+// control and yaw_control are VEL, ACC or JRK orders (mplx_traj_solve refuses SNP before any launch)
+cudaError_t launch_solve(int dim, int control, int yaw_control, const TrajArgs &A, long long n_wp, cudaStream_t st,
+                         int *launches) {
+  return with_dim(dim, [&](auto DIM) {
+    return with_order(control, [&](auto H) {
+      return with_order(yaw_control, [&](auto HY) {
+        if constexpr (H == 4 || HY == 4) {
+          return cudaErrorInvalidValue;
+        } else {
+          if (cudaError_t e = launch(traj_sweep_kernel<DIM, H, HY>, A.n_paths, false, st, launches, A)) return e;
+          if (n_wp > 0)
+            if (cudaError_t e = launch(traj_coeff_kernel<DIM, H, HY>, n_wp, true, st, launches, A, n_wp)) return e;
+          if (!A.samples) return cudaSuccess;
+          return launch(traj_sample_kernel<DIM>, (long long)A.n_paths * (A.n_samples + 1), true, st, launches, A);
+        }
+      });
+    });
+  });
 }
 
 }  // namespace
@@ -558,15 +572,10 @@ extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, 
   const int hy = (yaw_control == MPLX_VEL || yaw_control == MPLX_ACC || yaw_control == MPLX_JRK) ? mplx::order_of(yaw_control) : 0;
   if (hy == 0) return fail(MPLX_ERR_ARG, "yaw_control 0x%x: must be VEL, ACC or JRK", yaw_control);
   if (!dts && !(v > 0)) return fail(MPLX_ERR_ARG, "no segment times: dts is NULL and v <= 0");
-  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
-  if (!offset || !out || !out->status || !out->seg_t || !out->coeff) return fail(MPLX_ERR_ARG, "missing array");
-  if (out->samples && n_samples <= 0) return fail(MPLX_ERR_ARG, "samples with n_samples <= 0");
-  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
-  for (int p = 0; p < n_paths; p++)
-    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
-  const long long n_wp = offset[n_paths];
-  if (n_wp > 0 && !wps) return fail(MPLX_ERR_ARG, "missing array");
-  if (out->samples && (long long)n_paths * (n_samples + 1) >= ((long long)1 << 40)) return fail(MPLX_ERR_ARG, "too many samples");
+  long long n_wp = 0;
+  if (int r = mplx::check_batch(n_paths, offset, out && out->status && out->seg_t && out->coeff, wps != nullptr,
+                                out && out->samples, n_samples, n_wp))
+    return r;
   out->seconds = 0.0;
   if (n_paths == 0) return MPLX_OK;
   const int dim = c->dim;
@@ -591,20 +600,9 @@ extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, 
   mplx::TrajArgs A{n_paths, B.offset.p, B.wps.p, wp_control ? B.ctl.p : nullptr, dts ? B.dts.p : nullptr, v, control,
                    yaw_control, n_samples, B.status.p, B.mono.p, B.seg_t.p, B.taus.p, B.coeff.p,
                    out->samples ? B.samples.p : nullptr, B.fac.p, B.dpos.p, B.dyaw.p};
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  int launches = 0;
-  cudaError_t le = cudaEventRecord(e0, st);
-  if (le == cudaSuccess)
-    le = dim == 2 ? mplx::launch_dim<2>(h, hy, A, n_wp, st, &launches) : mplx::launch_dim<3>(h, hy, A, n_wp, st, &launches);
-  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
-  c->launches += launches;
-  if (le != cudaSuccess) {
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    CU(le);
-  }
+  TimedRun timed;
+  CU(timed.run(st, c->launches,
+               [&](int *launches) { return mplx::launch_solve(dim, control, yaw_control, A, n_wp, st, launches); }));
   CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
   if (n_wp > 0) {
     CU(cudaMemcpyAsync(out->seg_t, B.seg_t.p, sizeof(double) * n_wp, cudaMemcpyDeviceToHost, st));
@@ -612,11 +610,7 @@ extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, 
   }
   if (out->samples) CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  out->seconds = ms * 1e-3;
+  CU(timed.seconds(&out->seconds));
   return MPLX_OK;
 }
 
@@ -664,8 +658,8 @@ __device__ __forceinline__ int cubic_roots(double a, double b, double c, double 
   }
   const double theta = acos(R / sqrt(-Q * Q * Q));
   r[0] = 2 * sqrt(-Q) * cos(theta / 3) - a2 / 3;
-  r[1] = 2 * sqrt(-Q) * cos((theta + 2 * kPi) / 3) - a2 / 3;
-  r[2] = 2 * sqrt(-Q) * cos((theta + 4 * kPi) / 3) - a2 / 3;
+  r[1] = 2 * sqrt(-Q) * cos((theta + 2 * MPLX_PI) / 3) - a2 / 3;
+  r[2] = 2 * sqrt(-Q) * cos((theta + 4 * MPLX_PI) / 3) - a2 / 3;
   return 3;
 }
 __device__ __forceinline__ int quartic_roots(double a, double b, double c, double d, double e, double *r) {
@@ -827,6 +821,32 @@ struct ScaleArgs {
 
 __device__ __forceinline__ bool pos_finite(double x) { return isfinite(x) && x > 0; }
 
+// Trajectory's constructor for the path of W waypoints at slot b: taus[j+1] = t_j + taus[j].  Returns ok and
+// whether every segment time t_j is positive and finite.
+__device__ __forceinline__ bool seg_taus(const double *seg_t, double *taus, long long b, int W, bool ok) {
+  if (W > 0) taus[b] = 0.0;
+  for (int j = 0; j + 1 < W; j++) {
+    const double t = seg_t[b + j];
+    ok = ok && pos_finite(t);
+    taus[b + j + 1] = t + taus[b + j];
+  }
+  return ok;
+}
+
+// Lambda::getTau's running T += dT over nl lambda segments, left to right, into lT[0, nl].  Returns whether it
+// never decreases.
+__device__ __forceinline__ bool lam_sums(const double *lam, int nl, double *lT) {
+  double T = 0;
+  bool mono = true;
+  lT[0] = 0;
+  for (int k = 0; k < nl; k++) {
+    const double Tn = T + lam[k * 7 + 6];
+    mono = mono && Tn >= T;
+    lT[k + 1] = T = Tn;
+  }
+  return mono;
+}
+
 template <int DIM>
 __global__ void __launch_bounds__(128) scale_prep_kernel(ScaleArgs A) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -834,15 +854,8 @@ __global__ void __launch_bounds__(128) scale_prep_kernel(ScaleArgs A) {
   const long long b = A.offset[p];
   const int W = (int)(A.offset[p + 1] - b);
   const double *par = A.par + 3 * p;
-  bool ok = W >= 2 && pos_finite(par[1]) && pos_finite(par[2]) && (A.mode == MPLX_TRAJ_SCALE || pos_finite(par[0]));
-  // Trajectory's constructor: taus[j+1] = t_j + taus[j]
-  if (W > 0) A.taus[b] = 0.0;
-  for (int j = 0; j + 1 < W; j++) {
-    const double t = A.seg_t[b + j];
-    ok = ok && pos_finite(t);
-    A.taus[b + j + 1] = t + A.taus[b + j];
-  }
-  A.status[p] = ok ? 1 : 0;
+  const bool ok = W >= 2 && pos_finite(par[1]) && pos_finite(par[2]) && (A.mode == MPLX_TRAJ_SCALE || pos_finite(par[0]));
+  A.status[p] = seg_taus(A.seg_t, A.taus, b, W, ok) ? 1 : 0;
 }
 
 template <int DIM>
@@ -855,8 +868,7 @@ __global__ void __launch_bounds__(128) scale_cand_kernel(ScaleArgs A, long long 
     A.n_cand[s] = 0;
     if (j + 1 >= W) continue;
     const double *c = A.coeff + s * (DIM + 1) * 6;
-    bool finite = true;
-    for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+    const bool finite = coeff_finite<DIM>(c);
     if (!finite) A.status[p] = 0;  // every writer stores 0
     if (A.mode != MPLX_TRAJ_SCALE_DOWN || !finite) continue;
     const double t = A.seg_t[s], mv = A.par[3 * p], tau0 = A.taus[s];
@@ -968,16 +980,7 @@ __global__ void __launch_bounds__(128) scale_times_kernel(ScaleArgs A) {
   const int nl = A.n_knot[p] - 1;
   const double *lam = A.lam + b * NC * 7;
   double *lT = A.lam_T + b * NC;
-  // getTau's running T += dT, left to right
-  double T = 0;
-  bool mono = true;
-  lT[0] = 0;
-  for (int k = 0; k < nl; k++) {
-    const double Tn = T + lam[k * 7 + 6];
-    mono = mono && Tn >= T;
-    lT[k + 1] = T = Tn;
-  }
-  A.lam_mono[p] = mono ? 1 : 0;
+  A.lam_mono[p] = lam_sums(lam, nl, lT) ? 1 : 0;
   // Lambda::getT(taus[j]): the first segment with ti <= tau <= tf; the knots increase strictly from 0 and the
   // taus never decrease, so that segment's index never decreases along the path
   int k = 0;
@@ -1074,31 +1077,17 @@ __global__ void __launch_bounds__(128) scale_sample_kernel(ScaleArgs A) {
   }
 }
 
-template <int DIM>
-cudaError_t launch_scale(const ScaleArgs &A, long long n_wp, cudaStream_t st, int *launches) {
-  const int pb = (A.n_paths + 127) / 128;
-  auto grid = [](long long n) { return (int)std::min<long long>((n + 127) / 128, (long long)sm_count() * 16); };
-  scale_prep_kernel<DIM><<<pb, 128, 0, st>>>(A);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  scale_cand_kernel<DIM><<<grid(n_wp), 128, 0, st>>>(A, n_wp);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  scale_knot_kernel<DIM><<<pb, 128, 0, st>>>(A);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  scale_fit_kernel<DIM><<<grid(n_wp * kCand * DIM), 128, 0, st>>>(A, n_wp * kCand * DIM);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  scale_times_kernel<DIM><<<pb, 128, 0, st>>>(A);
-  *launches += 1;
-  if (cudaError_t e = cudaGetLastError()) return e;
-  if (A.samples) {
-    scale_sample_kernel<DIM><<<grid((long long)A.n_paths * (A.n_samples + 1)), 128, 0, st>>>(A);
-    *launches += 1;
-    if (cudaError_t e = cudaGetLastError()) return e;
-  }
-  return cudaSuccess;
+cudaError_t launch_scale(int dim, const ScaleArgs &A, long long n_wp, cudaStream_t st, int *launches) {
+  return with_dim(dim, [&](auto DIM) {
+    const long long n_slot = n_wp * kCand * DIM;
+    if (cudaError_t e = launch(scale_prep_kernel<DIM>, A.n_paths, false, st, launches, A)) return e;
+    if (cudaError_t e = launch(scale_cand_kernel<DIM>, n_wp, true, st, launches, A, n_wp)) return e;
+    if (cudaError_t e = launch(scale_knot_kernel<DIM>, A.n_paths, false, st, launches, A)) return e;
+    if (cudaError_t e = launch(scale_fit_kernel<DIM>, n_slot, true, st, launches, A, n_slot)) return e;
+    if (cudaError_t e = launch(scale_times_kernel<DIM>, A.n_paths, false, st, launches, A)) return e;
+    if (!A.samples) return cudaSuccess;
+    return launch(scale_sample_kernel<DIM>, (long long)A.n_paths * (A.n_samples + 1), true, st, launches, A);
+  });
 }
 
 }  // namespace
@@ -1110,15 +1099,10 @@ extern "C" int mplx_traj_scale(mplx_ctx *c, int n_paths, const int64_t *offset, 
   if (int r = mplx_bind(c)) return r;
   if (mode != MPLX_TRAJ_SCALE && mode != MPLX_TRAJ_SCALE_DOWN) return fail(MPLX_ERR_ARG, "mode %d: must be MPLX_TRAJ_SCALE or MPLX_TRAJ_SCALE_DOWN", mode);
   if (mode == MPLX_TRAJ_SCALE_DOWN && !mv) return fail(MPLX_ERR_ARG, "SCALE_DOWN without mv");
-  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
-  if (!offset || !ri || !rf || !out || !out->status || !out->total_t || !out->seg_T) return fail(MPLX_ERR_ARG, "missing array");
-  if (out->samples && n_samples <= 0) return fail(MPLX_ERR_ARG, "samples with n_samples <= 0");
-  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
-  for (int p = 0; p < n_paths; p++)
-    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
-  const long long n_wp = offset[n_paths];
-  if (n_wp > 0 && (!seg_t || !coeff)) return fail(MPLX_ERR_ARG, "missing array");
-  if (out->samples && (long long)n_paths * (n_samples + 1) >= ((long long)1 << 40)) return fail(MPLX_ERR_ARG, "too many samples");
+  long long n_wp = 0;
+  if (int r = mplx::check_batch(n_paths, offset, ri && rf && out && out->status && out->total_t && out->seg_T,
+                                seg_t && coeff, out && out->samples, n_samples, n_wp))
+    return r;
   out->seconds = 0.0;
   if (n_paths == 0) return MPLX_OK;
   const int dim = c->dim;
@@ -1149,20 +1133,8 @@ extern "C" int mplx_traj_scale(mplx_ctx *c, int n_paths, const int64_t *offset, 
   mplx::ScaleArgs A{n_paths, mode, n_samples, B.offset.p, B.seg_t.p, B.coeff.p, B.par.p, B.status.p, B.n_cand.p,
                     B.n_knot.p, B.taus.p, B.cand.p, B.cand_p.p, B.knot_t.p, B.knot_p.p, B.lam.p, B.lam_T.p,
                     B.total.p, B.seg_T.p, out->samples ? B.samples.p : nullptr, B.mono.p};
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  int launches = 0;
-  cudaError_t le = cudaEventRecord(e0, st);
-  if (le == cudaSuccess)
-    le = dim == 2 ? mplx::launch_scale<2>(A, n_wp, st, &launches) : mplx::launch_scale<3>(A, n_wp, st, &launches);
-  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
-  c->launches += launches;
-  if (le != cudaSuccess) {
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    CU(le);
-  }
+  TimedRun timed;
+  CU(timed.run(st, c->launches, [&](int *launches) { return mplx::launch_scale(dim, A, n_wp, st, launches); }));
   CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(out->total_t, B.total.p, sizeof(double) * n_paths, cudaMemcpyDeviceToHost, st));
   if (n_wp > 0) CU(cudaMemcpyAsync(out->seg_T, B.seg_T.p, sizeof(double) * n_wp, cudaMemcpyDeviceToHost, st));
@@ -1176,11 +1148,7 @@ extern "C" int mplx_traj_scale(mplx_ctx *c, int n_paths, const int64_t *offset, 
   CU(cudaStreamSynchronize(st));
   if (out->n_lambda)
     for (int p = 0; p < n_paths; p++) out->n_lambda[p] = out->status[p] == 1 ? nk[p] - 1 : 0;
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  out->seconds = ms * 1e-3;
+  CU(timed.seconds(&out->seconds));
   return MPLX_OK;
 }
 
@@ -1218,28 +1186,11 @@ __global__ void __launch_bounds__(128) check_path_kernel(const __grid_constant__
   if (p >= A.n_paths) return;
   const long long b = A.offset[p];
   const int W = (int)(A.offset[p + 1] - b);
-  bool ok = W >= 2;
-  // Trajectory's constructor: taus[j+1] = t_j + taus[j]
-  if (W > 0) A.taus[b] = 0.0;
-  for (int j = 0; j + 1 < W; j++) {
-    const double t = A.seg_t[b + j];
-    ok = ok && pos_finite(t);
-    A.taus[b + j + 1] = t + A.taus[b + j];
-  }
+  const bool ok = seg_taus(A.seg_t, A.taus, b, W, W >= 2);
   // Lambda::getTau's running T += dT, as mplx_traj_scale keeps it
   const int nl = A.lam ? A.n_lam[p] : 0;
   bool mono = true;
-  if (nl > 0) {
-    const double *lam = A.lam + b * NC * 7;
-    double *lT = A.lam_T + b * NC;
-    double T = 0;
-    lT[0] = 0;
-    for (int k = 0; k < nl; k++) {
-      const double Tn = T + lam[k * 7 + 6];
-      mono = mono && Tn >= T;
-      lT[k + 1] = T = Tn;
-    }
-  }
+  if (nl > 0) mono = lam_sums(A.lam + b * NC * 7, nl, A.lam_T + b * NC);
   A.lam_mono[p] = mono ? 1 : 0;
   const double total = nl > 0 ? A.total_in[p] : (W > 0 ? A.taus[b + W - 1] : 0.0);
   A.total[p] = total;
@@ -1336,8 +1287,7 @@ __global__ void __launch_bounds__(128) check_seg_kernel(const __grid_constant__ 
     bool fr = false, va = false;
     if (j + 1 < W) {
       const double *c = A.coeff + s * (DIM + 1) * 6;
-      bool finite = true;
-      for (int k = 0; k < (DIM + 1) * 6; k++) finite = finite && isfinite(c[k]);
+      const bool finite = coeff_finite<DIM>(c);
       if (!finite) A.form[p] = 0;  // every writer stores 0
       const double t = A.seg_t[s];
       if (finite && pos_finite(t)) {
@@ -1444,18 +1394,11 @@ __global__ void __launch_bounds__(128) check_sample_kernel(const __grid_constant
 
 cudaError_t launch_check(int dim, bool pot, const EnvParams &P, const CheckArgs &A, long long n_wp, cudaStream_t st,
                          int *launches) {
-  auto grid = [](long long n) { return (int)std::max<long long>(1, std::min<long long>((n + 127) / 128, (long long)sm_count() * 16)); };
   return with_dim(dim, [&](auto DIM) {
-    check_path_kernel<DIM><<<(A.n_paths + 127) / 128, 128, 0, st>>>(P, A);
-    *launches += 1;
-    if (cudaError_t e = cudaGetLastError()) return e;
-    check_seg_kernel<DIM><<<grid(n_wp), 128, 0, st>>>(P, A, n_wp);
-    *launches += 1;
-    if (cudaError_t e = cudaGetLastError()) return e;
+    if (cudaError_t e = launch(check_path_kernel<DIM>, A.n_paths, false, st, launches, P, A)) return e;
+    if (cudaError_t e = launch(check_seg_kernel<DIM>, n_wp, true, st, launches, P, A, n_wp)) return e;
     return with_bool(pot, [&](auto POT) {
-      check_sample_kernel<DIM, POT><<<grid(32LL * A.n_paths), 128, 0, st>>>(P, A);
-      *launches += 1;
-      return cudaGetLastError();
+      return launch(check_sample_kernel<DIM, POT>, 32LL * A.n_paths, true, st, launches, P, A);
     });
   });
 }
@@ -1469,17 +1412,13 @@ extern "C" int mplx_traj_check(mplx_ctx *c, int n_paths, const int64_t *offset, 
   if (int r = mplx_bind(c)) return r;
   if (!c->has_map) return fail(MPLX_ERR_ARG, "no map: call mplx_set_map first");
   if (!c->has_params) return fail(MPLX_ERR_ARG, "no params: call mplx_set_params first");
-  if (n_paths < 0) return fail(MPLX_ERR_ARG, "n_paths < 0");
-  if (!offset || !out || !out->status || !out->cost) return fail(MPLX_ERR_ARG, "missing array");
+  long long n_wp = 0;
+  if (int r = mplx::check_batch(n_paths, offset, out && out->status && out->cost, seg_t && coeff, false, 0, n_wp))
+    return r;
   if (out->seg_valid && !control) return fail(MPLX_ERR_ARG, "seg_valid without control");
   const bool scaled = lambda != nullptr;
   if ((total_t != nullptr) != scaled || (n_lambda != nullptr) != scaled)
     return fail(MPLX_ERR_ARG, "total_t, n_lambda and lambda go together");
-  if (offset[0] != 0) return fail(MPLX_ERR_ARG, "offset[0] must be 0");
-  for (int p = 0; p < n_paths; p++)
-    if (offset[p + 1] < offset[p]) return fail(MPLX_ERR_ARG, "offset decreases at path %d", p);
-  const long long n_wp = offset[n_paths];
-  if (n_wp > 0 && (!seg_t || !coeff)) return fail(MPLX_ERR_ARG, "missing array");
   const int dim = c->dim;
   const long long NC = (long long)mplx::kCand * dim;
   if (scaled)
@@ -1518,28 +1457,15 @@ extern "C" int mplx_traj_check(mplx_ctx *c, int n_paths, const int64_t *offset, 
                     scaled ? B.n_knot.p : nullptr, out->seg_valid ? B.ctl.p : nullptr, B.status.p, B.n_pts.p, B.form.p,
                     B.mono.p, B.taus.p, B.lam_T.p, B.total.p, B.cost.p, out->seg_free ? B.seg_free.p : nullptr,
                     out->seg_valid ? B.seg_valid.p : nullptr};
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  int launches = 0;
-  cudaError_t le = cudaEventRecord(e0, st);
-  if (le == cudaSuccess) le = mplx::launch_check(dim, c->P.pot != nullptr, c->P, A, n_wp, st, &launches);
-  if (le == cudaSuccess) le = cudaEventRecord(e1, st);
-  c->launches += launches;
-  if (le != cudaSuccess) {
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    CU(le);
-  }
+  TimedRun timed;
+  CU(timed.run(st, c->launches, [&](int *launches) {
+    return mplx::launch_check(dim, c->P.pot != nullptr, c->P, A, n_wp, st, launches);
+  }));
   CU(cudaMemcpyAsync(out->status, B.status.p, sizeof(int32_t) * n_paths, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(out->cost, B.cost.p, sizeof(double) * n_paths, cudaMemcpyDeviceToHost, st));
   if (n_wp > 0 && out->seg_free) CU(cudaMemcpyAsync(out->seg_free, B.seg_free.p, (size_t)n_wp, cudaMemcpyDeviceToHost, st));
   if (n_wp > 0 && out->seg_valid) CU(cudaMemcpyAsync(out->seg_valid, B.seg_valid.p, (size_t)n_wp, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  out->seconds = ms * 1e-3;
+  CU(timed.seconds(&out->seconds));
   return MPLX_OK;
 }

@@ -504,6 +504,19 @@ void put_waypoints(const Trajectory<Dim> &traj, double *waypoints) {
     o[4 * Dim] = w.yaw; o[4 * Dim + 1] = w.t;
   }
 }
+/// Trajectory<Dim> of n_seg segments with durations seg_t and coefficients coeff (mplh_traj_solve's layout), each
+/// segment with the control flag `control`
+template <int Dim>
+Trajectory<Dim> make_trajectory(int n_seg, const double *seg_t, const double *coeff, int control) {
+  vec_E<Primitive<Dim>> prs;
+  for (int j = 0; j < n_seg; j++) {
+    vec_E<Vecf<6>> cs(Dim + 1);
+    for (int a = 0; a <= Dim; a++)
+      for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)j * (Dim + 1) + a) * 6 + k];
+    prs.push_back(Primitive<Dim>(cs, seg_t[j], control));
+  }
+  return Trajectory<Dim>(prs);
+}
 template <typename F>
 int with_traj_dim(int dim, F &&f) {
   try {
@@ -576,14 +589,7 @@ int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coef
   if (n_seg < 0 || (n_seg > 0 && (!seg_t || !coeff)) || (samples && n_samples < 1)) { g_err = "bad argument"; return 1; }
   return with_traj_dim(dim, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
-    vec_E<Primitive<Dim>> prs;
-    for (int j = 0; j < n_seg; j++) {
-      vec_E<Vecf<6>> cs(Dim + 1);
-      for (int a = 0; a <= Dim; a++)
-        for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)j * (Dim + 1) + a) * 6 + k];
-      prs.push_back(Primitive<Dim>(cs, seg_t[j], control));
-    }
-    const Trajectory<Dim> traj(prs);
+    const Trajectory<Dim> traj = make_trajectory<Dim>(n_seg, seg_t, coeff, control);
     if (samples) put_samples<Dim>(traj, n_samples, samples);
     if (waypoints) put_waypoints<Dim>(traj, waypoints);
   });
@@ -593,16 +599,23 @@ int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coef
 /* ---- Trajectory time scaling (mpl_host.hpp): one path on the host ------------------------------------------ */
 
 namespace {
+/// whether mplx_traj_check evaluates this path at all: at least one segment, every segment time finite and
+/// > 0, every coefficient finite
+template <int Dim>
+bool checkable(int n_seg, const double *seg_t, const double *coeff) {
+  if (n_seg < 1) return false;
+  for (int j = 0; j < n_seg; j++)
+    if (!(std::isfinite(seg_t[j]) && seg_t[j] > 0)) return false;
+  for (size_t k = 0; k < (size_t)n_seg * (Dim + 1) * 6; k++)
+    if (!std::isfinite(coeff[k])) return false;
+  return true;
+}
+
 /// whether mplx_traj_scale would scale this path (status 1 or 2) rather than refuse it (status 0)
 template <int Dim>
 bool scalable(int n_seg, const double *seg_t, const double *coeff, int mode, double mv, double ri, double rf) {
   auto pos = [](double x) { return std::isfinite(x) && x > 0; };
-  if (n_seg < 1 || !pos(ri) || !pos(rf) || (mode == MPLX_TRAJ_SCALE_DOWN && !pos(mv))) return false;
-  for (int j = 0; j < n_seg; j++)
-    if (!pos(seg_t[j])) return false;
-  for (size_t k = 0; k < (size_t)n_seg * (Dim + 1) * 6; k++)
-    if (!std::isfinite(coeff[k])) return false;
-  return true;
+  return pos(ri) && pos(rf) && (mode != MPLX_TRAJ_SCALE_DOWN || pos(mv)) && checkable<Dim>(n_seg, seg_t, coeff);
 }
 }  // namespace
 
@@ -634,14 +647,7 @@ int mplh_traj_scale(int dim, int n_seg, const double *seg_t, const double *coeff
     if (lambda) std::fill(lambda, lambda + n_slot * 7, 0.0);
     if (samples) std::fill(samples, samples + (size_t)(n_samples + 1) * (4 * Dim + 3), 0.0);
     if (!scalable<Dim>(n_seg, seg_t, coeff, mode, mv, ri, rf)) return;
-    vec_E<Primitive<Dim>> prs;
-    for (int j = 0; j < n_seg; j++) {
-      vec_E<Vecf<6>> cs(Dim + 1);
-      for (int a = 0; a <= Dim; a++)
-        for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)j * (Dim + 1) + a) * 6 + k];
-      prs.push_back(Primitive<Dim>(cs, seg_t[j], control));
-    }
-    Trajectory<Dim> traj(prs);
+    Trajectory<Dim> traj = make_trajectory<Dim>(n_seg, seg_t, coeff, control);
     const bool scaled = mode == MPLX_TRAJ_SCALE ? traj.scale(ri, rf) : traj.scale_down(mv, ri, rf);
     *status = scaled ? 1 : 2;
     *total_t = traj.getTotalTime();
@@ -677,18 +683,6 @@ struct CheckEnv : MPL::env_map_host<Dim> {  // the map queries only: get_succ is
   using MPL::env_map_host<Dim>::env_map_host;
   void get_succ(const Waypoint<Dim> &, vec_E<Waypoint<Dim>> &, std::vector<decimal_t> &, std::vector<int> &) const override {}
 };
-
-/// whether mplx_traj_check evaluates this path at all: at least one segment, every segment time finite and
-/// > 0, every coefficient finite
-template <int Dim>
-bool checkable(int n_seg, const double *seg_t, const double *coeff) {
-  if (n_seg < 1) return false;
-  for (int j = 0; j < n_seg; j++)
-    if (!(std::isfinite(seg_t[j]) && seg_t[j] > 0)) return false;
-  for (size_t k = 0; k < (size_t)n_seg * (Dim + 1) * 6; k++)
-    if (!std::isfinite(coeff[k])) return false;
-  return true;
-}
 }  // namespace
 
 extern "C" {
@@ -750,15 +744,8 @@ int mplh_traj_check(int dim, const int8_t *map, const int32_t *mdim, const doubl
         if (seg_valid) seg_valid[b + j] = 0;
       }
       if (!checkable<Dim>(S, seg_t + b, coeff + b * (Dim + 1) * 6)) return;
-      const int ctl = control ? control[p] : Control::NONE;
-      vec_E<Primitive<Dim>> prs;
-      for (int j = 0; j < S; j++) {
-        vec_E<Vecf<6>> cs(Dim + 1);
-        for (int a = 0; a <= Dim; a++)
-          for (int k = 0; k < 6; k++) cs[a](k) = coeff[((size_t)(b + j) * (Dim + 1) + a) * 6 + k];
-        prs.push_back(Primitive<Dim>(cs, seg_t[b + j], ctl));
-      }
-      Trajectory<Dim> traj(prs);
+      Trajectory<Dim> traj =
+          make_trajectory<Dim>(S, seg_t + b, coeff + b * (Dim + 1) * 6, control ? control[p] : Control::NONE);
       if (scaled && n_lambda[p] > 0) {
         Lambda lam;
         for (int k = 0; k < n_lambda[p]; k++) {

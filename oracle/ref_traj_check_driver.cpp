@@ -5,7 +5,7 @@
 // can be checked against it.  A scaled path gets its lambda segments and total time assigned to the reference's
 // Trajectory members.  Paths and segments where the reference is undefined (mplh_traj_check's status 0, a sample
 // count above MPLX_SAMPLE_N_MAX) are not evaluated.  TEST INFRASTRUCTURE.
-// Build: make -C oracle -f traj_check.mk ref -> oracle/_ref/libmplref_traj_check.so (git-ignored), run by build().
+// Build: make -C oracle -f traj.mk ref -> oracle/_ref/libmplref_traj_check.so (git-ignored), run by build().
 #include <mpl_basis/trajectory.h>
 #include <mpl_planner/env/env_map.h>
 

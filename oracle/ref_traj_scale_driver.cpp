@@ -3,7 +3,7 @@
 // the product's mplh_traj_scale and mplh_solve (host/mpl_host_capi.cpp), so that the host restatement can be
 // checked against it.  Trajectory::scale is called directly; scale_down, which does not compile in the reference,
 // is run as the product defines it, on the reference's own classes.  TEST INFRASTRUCTURE.
-// Build: make -C oracle -f traj_scale.mk ref -> oracle/_ref/libmplref_traj_scale.so (git-ignored), run by build().
+// Build: make -C oracle -f traj.mk ref -> oracle/_ref/libmplref_traj_scale.so (git-ignored), run by build().
 #include <mpl_basis/trajectory.h>
 
 #include <algorithm>

@@ -412,7 +412,13 @@ def test_batch_independence_and_launches(solvers):
         l0 = e.launch_count()
         e.traverse_trajectories(paths[:n], ctl[:n])
         launches.append(e.launch_count() - l0)
-    assert launches == [3, 3, 3]
+    # a batch in which no path has a segment has no waypoint slot: the segment kernel runs on one block
+    empty = dict(seg_t=np.zeros(0), coeff=np.zeros((0, dim + 1, 6)))
+    l0 = e.launch_count()
+    out, _ = e.traverse_trajectories([empty, empty], ctl[:2])
+    launches.append(e.launch_count() - l0)
+    assert [(o["status"], o["cost"]) for o in out] == [(0, 0.0), (0, 0.0)]
+    assert launches == [3, 3, 3, 3]
     e.close()
 
 

@@ -163,6 +163,15 @@ def test_status_classes(solvers):
         if o["status"] == 0:
             assert o["total_t"] == 0 and not o["seg_T"].any() and not o["samples"].any() and len(o["lambda"]) == 0
     assert out[4]["total_t"] > 0 and out[4]["seg_T"].all() and len(out[4]["lambda"]) == 0
+    # a batch in which no path has a segment has no waypoint slot: every kernel still runs, on one block
+    for mode in (SCALE, SCALE_DOWN):
+        for ns, with_lambda in ((0, False), (NS, True)):
+            l0 = s.launch_count()
+            out, _ = s.scale([empty, empty], mode, mv=0.5, ri=1.0, rf=1.0, n_samples=ns, with_lambda=with_lambda)
+            assert s.launch_count() - l0 == 5 + (ns > 0)
+            for o in out:
+                assert o["status"] == 0 and o["total_t"] == 0 and not o["seg_T"].any()
+                assert not o.get("samples", np.zeros(1)).any() and len(o.get("lambda", [])) == 0
 
 
 def test_refusals(solvers):

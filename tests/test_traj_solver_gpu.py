@@ -149,6 +149,11 @@ def test_batch_edge_cases(solvers):
         same_result(res[p], solve_alone(s, paths, 0x07, 0x01, dts, None, p), p)
     one, _ = s.solve(paths[:1], 0x07, dts=dts[:1], n_samples=NS)
     same_result(one[0], res[0], "one path")
+    # no path with a segment and no waypoint slot: the sweep and the samples run, the coefficient kernel does not
+    l0 = s.launch_count()
+    res, _ = s.solve([np.zeros((0, 3)), np.zeros((0, 3))], 0x07, n_samples=NS)
+    assert s.launch_count() - l0 == 2
+    assert [r["status"] for r in res] == [0, 0] and not any(r["samples"].any() for r in res)
 
 
 def test_allocated_zero_length_segment(solvers):

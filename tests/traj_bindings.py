@@ -1,6 +1,6 @@
 """TrajSolver bindings for the tests: the product's host restatement (planner.traj_solve) and the REFERENCE's
-own TrajSolver (oracle/_ref/libmplref_traj.so: src/mpl_traj_solver compiled against oracle/shim_traj), with
-the same signature (mplh_traj_solve, host/mpl_host_capi.cpp)."""
+own TrajSolver (oracle/_ref/libmplref_traj.so, built by oracle/traj.mk: src/mpl_traj_solver compiled against
+oracle/shim_traj), with the same signature (mplh_traj_solve, host/mpl_host_capi.cpp)."""
 from pathlib import Path
 
 from motion_primitive_library_b200.planner import load_traj_solve_fn, run_traj_solve, traj_solve  # noqa: F401

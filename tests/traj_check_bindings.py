@@ -1,6 +1,6 @@
 """Trajectory-check bindings for the tests: the product's host restatement (planner.traj_check) and the
 REFERENCE's own env_map::traverse_trajectory / is_free and validate_primitive (oracle/_ref/libmplref_traj_check.so,
-built by oracle/traj_check.mk), with the same signature (mplh_traj_check in host/mpl_host_capi.cpp)."""
+built by oracle/traj.mk), with the same signature (mplh_traj_check in host/mpl_host_capi.cpp)."""
 import numpy as np
 
 from motion_primitive_library_b200 import planner as P

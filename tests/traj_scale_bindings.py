@@ -1,6 +1,6 @@
 """Trajectory time-scaling bindings for the tests: the product's host restatement (planner.traj_scale,
 planner.solve_roots) and the REFERENCE's own Trajectory::scale, scale_down steps and math.h solve
-(oracle/_ref/libmplref_traj_scale.so, built by oracle/traj_scale.mk), with the same signatures (mplh_traj_scale,
+(oracle/_ref/libmplref_traj_scale.so, built by oracle/traj.mk), with the same signatures (mplh_traj_scale,
 mplh_solve in host/mpl_host_capi.cpp)."""
 import numpy as np
 
