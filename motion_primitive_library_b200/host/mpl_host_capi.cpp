@@ -6,94 +6,74 @@
 
 static thread_local std::string g_err;
 
+namespace {
+/// A MapPlanner with the GPU env on map mu (map_planner.cpp:14-18), a's control and a's speculation (0 = the
+/// library default)
+template <int Dim>
+std::unique_ptr<MPL::MapPlanner<Dim>> gpu_planner(const mplh_plan_args *a, const std::shared_ptr<MPL::MapUtil<Dim>> &mu) {
+  auto planner = std::make_unique<MPL::MapPlanner<Dim>>(false);
+  planner->setMapUtil(mu, a->device);
+  planner->setControl(a->control);
+  if (a->speculate > 0) planner->setSpeculation(a->speculate);
+  return planner;
+}
+
+/// a's potential map and its two weights, when a has one
+template <int Dim>
+void set_potential(MPL::MapPlanner<Dim> &planner, const mplh_plan_args *a) {
+  if (!a->potential) return;
+  planner.gpu_env()->set_potential_map(std::vector<int8_t>(a->potential, a->potential + mplh::n_cells<Dim>(a)));
+  planner.setPotentialWeight(a->potential_weight);
+  planner.setGradientWeight(a->gradient_weight);
+}
+}  // namespace
+
 extern "C" {
 const char *mplh_last_error(void) { return g_err.c_str(); }
 
 int mplh_plan(const mplh_plan_args *a, mplh_plan_result *r, uint64_t *closed_keys, int cap_closed, int32_t *actions,
               int cap_actions) {
-  try {
-    *r = mplh_plan_result{};
-    auto go = [&](auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      MPL::MapPlanner<Dim> planner(false);
-      planner.setMapUtil(mplh::make_map<Dim>(a), a->device);  // installs env_map_gpu (map_planner.cpp:14-18)
-      planner.setControl(a->control);
-      if (a->speculate > 0) planner.setSpeculation(a->speculate);  // 0 = the library default
-      if (a->potential) {
-        size_t n = 1;
-        for (int k = 0; k < Dim; k++) n *= (size_t)a->mdim[k];
-        planner.gpu_env()->set_potential_map(std::vector<int8_t>(a->potential, a->potential + n));
-        planner.setPotentialWeight(a->potential_weight);
-        planner.setGradientWeight(a->gradient_weight);
-      }
-      mplh::run<Dim>(planner, a, r, closed_keys, cap_closed, actions, cap_actions);
-      r->gpu_nodes = planner.gpu_env()->stats_nodes();
-      r->gpu_calls = planner.gpu_env()->stats_calls();
-      r->gpu_launches = planner.gpu_env()->launches();
-    };
-    if (a->dim == 2) go(std::integral_constant<int, 2>());
-    else if (a->dim == 3) go(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
+  *r = mplh_plan_result{};
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    auto planner = gpu_planner<Dim>(a, mplh::make_map<Dim>(a));
+    set_potential(*planner, a);
+    mplh::run<Dim>(*planner, a, r, closed_keys, cap_closed, actions, cap_actions);
+    r->gpu_nodes = planner->gpu_env()->stats_nodes();
+    r->gpu_calls = planner->gpu_env()->stats_calls();
+    r->gpu_launches = planner->gpu_env()->launches();
+  });
 }
 
 /* mplh_plan that also returns the nodes A* expanded, in pop order (graph_search.h:66-75): the replay
  * frontier of the benchmark.  *n_trace = nodes recorded (<= cap_trace). */
 int mplh_plan_trace(const mplh_plan_args *a, mplh_plan_result *r, mplx_waypoint *trace, int cap_trace, int32_t *n_trace) {
-  try {
-    *r = mplh_plan_result{};
+  *r = mplh_plan_result{};
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
     std::vector<mplx_waypoint> tr;
-    auto go = [&](auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      MPL::MapPlanner<Dim> planner(false);
-      planner.setMapUtil(mplh::make_map<Dim>(a), a->device);
-      planner.setControl(a->control);
-      if (a->speculate > 0) planner.setSpeculation(a->speculate);  // 0 = the library default
-      planner.gpu_env()->set_trace(&tr);
-      std::vector<uint64_t> closed(1);
-      std::vector<int32_t> actions(1);
-      mplh::run<Dim>(planner, a, r, closed.data(), 0, actions.data(), 0);
-      planner.gpu_env()->set_trace(nullptr);
-    };
-    if (a->dim == 2) go(std::integral_constant<int, 2>());
-    else if (a->dim == 3) go(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
+    auto planner = gpu_planner<Dim>(a, mplh::make_map<Dim>(a));
+    planner->gpu_env()->set_trace(&tr);
+    std::vector<uint64_t> closed(1);
+    std::vector<int32_t> actions(1);
+    mplh::run<Dim>(*planner, a, r, closed.data(), 0, actions.data(), 0);
+    planner->gpu_env()->set_trace(nullptr);
     const int n = (int)std::min<std::size_t>(tr.size(), (std::size_t)cap_trace);
-    for (int i = 0; i < n; i++) trace[i] = tr[i];
+    std::copy(tr.begin(), tr.begin() + n, trace);
     if (n_trace) *n_trace = n;
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
+  });
 }
 
 /* MapPlanner::plan() with the GPU env, then the recovered Trajectory (include/mpl_basis/trajectory.h):
  * sample(N), getTotalTime / J / Jyaw, getWaypoints and evaluate(t); layouts in plan_capi.hpp. */
 int mplh_plan_trajectory(const mplh_plan_args *a, int N, mplh_plan_result *r, double *samples, double *totals,
                          double *waypoints, int cap_wp, int32_t *n_wp, double *mids) {
-  try {
-    *r = mplh_plan_result{};
-    auto go = [&](auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      MPL::MapPlanner<Dim> planner(false);
-      planner.setMapUtil(mplh::make_map<Dim>(a), a->device);
-      planner.setControl(a->control);
-      if (a->speculate > 0) planner.setSpeculation(a->speculate);  // 0 = the library default
-      mplh::run_trajectory<Dim>(planner, a, N, r, samples, totals, waypoints, cap_wp, n_wp, mids);
-    };
-    if (a->dim == 2) go(std::integral_constant<int, 2>());
-    else if (a->dim == 3) go(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
+  *r = mplh_plan_result{};
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    auto planner = gpu_planner<Dim>(a, mplh::make_map<Dim>(a));
+    mplh::run_trajectory<Dim>(*planner, a, N, r, samples, totals, waypoints, cap_wp, n_wp, mids);
+  });
 }
 
 /* MapPlanner::plan() followed by MapPlanner::iterativePlan() (map_planner.cpp:393-433) with the GPU
@@ -103,33 +83,15 @@ int mplh_plan_trajectory(const mplh_plan_args *a, int N, mplh_plan_result *r, do
 int mplh_iterative_plan(const mplh_plan_args *a, const double *search_radius, int max_iter, mplh_plan_result *first,
                         mplh_plan_result *last, int32_t *info, uint64_t *closed_keys, int cap_closed, int32_t *actions,
                         int cap_actions) {
-  try {
-    *first = mplh_plan_result{};
-    *last = mplh_plan_result{};
-    auto go = [&](auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      MPL::MapPlanner<Dim> planner(false);
-      planner.setMapUtil(mplh::make_map<Dim>(a), a->device);
-      planner.setControl(a->control);
-      if (a->speculate > 0) planner.setSpeculation(a->speculate);  // 0 = the library default
-      if (a->potential) {
-        size_t n = 1;
-        for (int k = 0; k < Dim; k++) n *= (size_t)a->mdim[k];
-        planner.gpu_env()->set_potential_map(std::vector<int8_t>(a->potential, a->potential + n));
-        planner.setPotentialWeight(a->potential_weight);
-        planner.setGradientWeight(a->gradient_weight);
-      }
-      mplh::run_iterative<Dim>(planner, a, search_radius, max_iter, first, last, info, closed_keys, cap_closed, actions,
-                               cap_actions);
-    };
-    if (a->dim == 2) go(std::integral_constant<int, 2>());
-    else if (a->dim == 3) go(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
+  *first = mplh_plan_result{};
+  *last = mplh_plan_result{};
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    auto planner = gpu_planner<Dim>(a, mplh::make_map<Dim>(a));
+    set_potential(*planner, a);
+    mplh::run_iterative<Dim>(*planner, a, search_radius, max_iter, first, last, info, closed_keys, cap_closed, actions,
+                             cap_actions);
+  });
 }
 
 /* A scripted LPA* session (plan_capi_types.h: PLAN / LINK / BLOCK / CLEAR / SUBTREE steps) on one
@@ -138,24 +100,12 @@ int mplh_iterative_plan(const mplh_plan_args *a, const double *search_radius, in
  * the trajectory found by PLAN step k go to actions[k*cap_actions ...]. */
 int mplh_lpa_run(const mplh_plan_args *a, const mplh_lpa_step *steps, int n_steps, mplh_lpa_out *outs,
                  int32_t *actions, int cap_actions) {
-  try {
-    auto go = [&](auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      MPL::MapPlanner<Dim> planner(false);
-      auto mu = mplh::make_map<Dim>(a);
-      planner.setMapUtil(mu, a->device);
-      planner.setControl(a->control);
-      if (a->speculate > 0) planner.setSpeculation(a->speculate);  // 0 = the library default
-      mplh::run_lpa<Dim>(planner, mu, a, steps, n_steps, outs, actions, cap_actions);
-    };
-    if (a->dim == 2) go(std::integral_constant<int, 2>());
-    else if (a->dim == 3) go(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
+    constexpr int Dim = decltype(dimtag)::value;
+    auto mu = mplh::make_map<Dim>(a);
+    auto planner = gpu_planner<Dim>(a, mu);
+    mplh::run_lpa<Dim>(*planner, mu, a, steps, n_steps, outs, actions, cap_actions);
+  });
 }
 
 /* Lock-step batched A* over many (start, goal) pairs on one map (MPL::MultiQueryPlanner) as a
@@ -175,6 +125,12 @@ struct BatchSession {
   std::vector<int32_t> actions;
   std::vector<uint64_t> closed;
 };
+/// the Dim of a MultiQueryPlanner<Dim>, for the bodies with_session runs
+template <class Q>
+struct mq_dim;
+template <int Dim>
+struct mq_dim<MPL::MultiQueryPlanner<Dim>> : std::integral_constant<int, Dim> {};
+
 template <int Dim>
 MPL::MultiQueryPlanner<Dim> *open_mq(const mplh_plan_args *a) {
   auto *mq = new MPL::MultiQueryPlanner<Dim>(mplh::make_map<Dim>(a), a->device);
@@ -187,106 +143,106 @@ MPL::MultiQueryPlanner<Dim> *open_mq(const mplh_plan_args *a) {
   e.set_dt(a->T); e.set_w(a->w); e.set_wyaw(a->wyaw);
   e.set_tol_pos(a->tol_pos); e.set_tol_vel(a->tol_vel); e.set_tol_acc(a->tol_acc);
   if (a->potential) {
-    size_t n = 1;
-    for (int k = 0; k < Dim; k++) n *= (size_t)a->mdim[k];
-    e.set_potential_map(std::vector<int8_t>(a->potential, a->potential + n));
+    e.set_potential_map(std::vector<int8_t>(a->potential, a->potential + mplh::n_cells<Dim>(a)));
     e.set_potential_weight(a->potential_weight);
     e.set_gradient_weight(a->gradient_weight);
   }
   return mq;
 }
-template <int Dim>
-void plan_mq(MPL::MultiQueryPlanner<Dim> *mq, int control, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q,
-             double eps, int max_num, mplh_query_result *out, double *totals) {
-  vec_E<Waypoint<Dim>> S, G;
-  for (int q = 0; q < n_q; q++) {
-    S.push_back(mplh::wp_from<Dim>(starts[q], control));
-    G.push_back(mplh::wp_from<Dim>(goals[q], control));
+
+/// Runs f(mq, s) on the session s and its MPL::MultiQueryPlanner<Dim> mq and returns 0.  A null handle, or
+/// ok == false, returns 1 with `refusal`; an exception thrown by f returns 1 with its message.
+template <typename F>
+int with_session(void *session, F &&f, bool ok = true, const char *refusal = "null session") {
+  BatchSession *s = (BatchSession *)session;
+  if (!s || !s->mq || !ok) {
+    g_err = refusal;
+    return 1;
   }
-  auto t0 = std::chrono::steady_clock::now();
-  auto res = mq->plan(S, G, eps, max_num);
-  const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-  for (int q = 0; q < n_q; q++) {
-    out[q].valid = res[q].valid ? 1 : 0;
-    out[q].cost = res[q].cost;
-    out[q].expanded = res[q].expanded;
-    out[q].n_closed = (int)res[q].n_closed;
-    out[q].n_actions = (int)res[q].actions.size();
-  }
-  if (totals) {
-    totals[0] = (double)mq->iterations(); totals[1] = (double)mq->nodes_expanded(); totals[2] = secs;
-    totals[3] = mq->t_pop(); totals[4] = mq->t_device(); totals[5] = mq->t_relax(); totals[6] = 0.0;
-  }
+  return mplh::with_dim(s->dim, g_err, 1, [&](auto dimtag) {
+    f(*(MPL::MultiQueryPlanner<decltype(dimtag)::value> *)s->mq, *s);
+  });
+}
+
+/// mplh_batch_plan, and with keep mplh_batch_plan_keep
+int batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps, int max_num,
+               bool keep, bool collect_closed, mplh_query_result *out, double *totals) {
+  return with_session(session, [&](auto &mq, BatchSession &s) {
+    constexpr int Dim = mq_dim<std::decay_t<decltype(mq)>>::value;
+    mq.setCollectClosed(keep && collect_closed);
+    // the session's later plans must not keep collecting, whatever plan() does
+    struct Reset {
+      decltype(mq) p;
+      ~Reset() { p.setCollectClosed(false); }
+    } reset{mq};
+    vec_E<Waypoint<Dim>> S, G;
+    for (int q = 0; q < n_q; q++) {
+      S.push_back(mplh::wp_from<Dim>(starts[q], s.control));
+      G.push_back(mplh::wp_from<Dim>(goals[q], s.control));
+    }
+    auto t0 = std::chrono::steady_clock::now();
+    auto res = mq.plan(S, G, eps, max_num);
+    const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    if (keep) {
+      s.aoff.assign((size_t)n_q + 1, 0);
+      s.coff.assign((size_t)n_q + 1, 0);
+      s.actions.clear();
+      s.closed.clear();
+    }
+    for (int q = 0; q < n_q; q++) {
+      out[q].valid = res[q].valid ? 1 : 0;
+      out[q].cost = res[q].cost;
+      out[q].expanded = res[q].expanded;
+      out[q].n_closed = (int)res[q].n_closed;
+      out[q].n_actions = (int)res[q].actions.size();
+      if (!keep) continue;
+      s.actions.insert(s.actions.end(), res[q].actions.begin(), res[q].actions.end());
+      s.closed.insert(s.closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
+      s.aoff[q + 1] = (int64_t)s.actions.size();
+      s.coff[q + 1] = (int64_t)s.closed.size();
+    }
+    if (totals) {
+      totals[0] = (double)mq.iterations(); totals[1] = (double)mq.nodes_expanded(); totals[2] = secs;
+      totals[3] = mq.t_pop(); totals[4] = mq.t_device(); totals[5] = mq.t_relax(); totals[6] = 0.0;
+    }
+  });
 }
 }  // namespace
 extern "C" {
 
 void *mplh_batch_open(const mplh_plan_args *a) {
-  try {
-    if (a->dim != 2 && a->dim != 3) throw std::runtime_error("dim must be 2 or 3");
-    BatchSession *s = new BatchSession();
-    s->dim = a->dim;
-    s->control = a->control;
-    s->mq = a->dim == 2 ? (void *)open_mq<2>(a) : (void *)open_mq<3>(a);
-    return s;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return nullptr;
-  }
+  BatchSession *s = nullptr;
+  mplh::with_dim(a->dim, g_err, 1, [&](auto dimtag) {
+    s = new BatchSession{a->dim, a->control, open_mq<decltype(dimtag)::value>(a)};
+  });
+  return s;
 }
 
 int mplh_batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps, int max_num,
                     mplh_query_result *out, double *totals) {
-  try {
-    BatchSession *s = (BatchSession *)session;
-    if (!s || !s->mq) throw std::runtime_error("null session");
-    if (s->dim == 2) plan_mq<2>((MPL::MultiQueryPlanner<2> *)s->mq, s->control, starts, goals, n_q, eps, max_num, out, totals);
-    else plan_mq<3>((MPL::MultiQueryPlanner<3> *)s->mq, s->control, starts, goals, n_q, eps, max_num, out, totals);
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 1;
-  }
+  return batch_plan(session, starts, goals, n_q, eps, max_num, false, false, out, totals);
 }
 
 /* MapUtil::setCells on the session's map: cells (n x dim cell coordinates) get values[k], a later entry
  * for the same cell winning.  The next mplh_batch_plan sends only these voxels to the device and keeps
  * the potential map.  A cell outside the map fails the call with nothing changed. */
 int mplh_batch_update_cells(void *session, const int32_t *cells, const int8_t *values, int n) {
-  try {
-    BatchSession *s = (BatchSession *)session;
-    if (!s || !s->mq) throw std::runtime_error("null session");
+  return with_session(session, [&](auto &mq, BatchSession &) {
+    constexpr int Dim = mq_dim<std::decay_t<decltype(mq)>>::value;
     if (n < 0 || (n > 0 && (!cells || !values))) throw std::runtime_error("cells/values missing");
-    auto go = [&](auto *mq, auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      vec_E<Veci<Dim>> pns(n);
-      for (int i = 0; i < n; i++)
-        for (int d = 0; d < Dim; d++) pns[i](d) = cells[(size_t)i * Dim + d];
-      mq->map_util().setCells(pns, std::vector<int8_t>(values, values + n));
-    };
-    if (s->dim == 2) go((MPL::MultiQueryPlanner<2> *)s->mq, std::integral_constant<int, 2>());
-    else go((MPL::MultiQueryPlanner<3> *)s->mq, std::integral_constant<int, 3>());
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 1;
-  }
+    vec_E<Veci<Dim>> pns(n);
+    for (int i = 0; i < n; i++)
+      for (int d = 0; d < Dim; d++) pns[i](d) = cells[(size_t)i * Dim + d];
+    mq.map_util().setCells(pns, std::vector<int8_t>(values, values + n));
+  });
 }
 
 /* Grid transfers of the session's env so far: *full = whole-grid uploads, *delta = sparse updates. */
 int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq) {
-    g_err = "null session";
-    return 1;
-  }
-  auto put = [&](const auto &env) {
-    if (full) *full = env.full_uploads();
-    if (delta) *delta = env.delta_uploads();
-  };
-  if (s->dim == 2) put(((MPL::MultiQueryPlanner<2> *)s->mq)->env());
-  else put(((MPL::MultiQueryPlanner<3> *)s->mq)->env());
-  return 0;
+  return with_session(session, [&](auto &mq, BatchSession &) {
+    if (full) *full = mq.env().full_uploads();
+    if (delta) *delta = mq.env().delta_uploads();
+  });
 }
 
 /* Which loop the session's plans run (MultiQueryPlanner::Path): 0 = automatic (a device search once the
@@ -295,27 +251,15 @@ int mplh_batch_map_uploads(void *session, int64_t *full, int64_t *delta) {
  * mplx_plan_batch_grow), 1 = always lock-step, 2 = the occupancy device search whenever the plan allows it,
  * 3 = the cost-term device search for every plan, 4 = the growing device search for every plan. */
 int mplh_batch_set_path(void *session, int path) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq || path < 0 || path > 4) {
-    g_err = "null session or path not in 0..4";
-    return 1;
-  }
-  if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setPath(path);
-  else ((MPL::MultiQueryPlanner<3> *)s->mq)->setPath(path);
-  return 0;
+  return with_session(session, [&](auto &mq, BatchSession &) { mq.setPath(path); }, path >= 0 && path <= 4,
+                      "null session or path not in 0..4");
 }
 
 /* Diagnostics: the first and the largest arena capacity (records) of the session's growing device searches;
  * 0 = automatic (mplx_plan_batch_grow).  Negative values fail. */
 int mplh_batch_set_grow_caps(void *session, int64_t first_cap, int64_t max_cap) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq || first_cap < 0 || max_cap < 0) {
-    g_err = "null session or negative capacity";
-    return 1;
-  }
-  if (s->dim == 2) ((MPL::MultiQueryPlanner<2> *)s->mq)->setGrowCaps(first_cap, max_cap);
-  else ((MPL::MultiQueryPlanner<3> *)s->mq)->setGrowCaps(first_cap, max_cap);
-  return 0;
+  return with_session(session, [&](auto &mq, BatchSession &) { mq.setGrowCaps(first_cap, max_cap); },
+                      first_cap >= 0 && max_cap >= 0, "null session or negative capacity");
 }
 
 /* The growing device search of the session's last plan (all 0 when it ran another path): kernel launches,
@@ -323,40 +267,24 @@ int mplh_batch_set_grow_caps(void *session, int64_t first_cap, int64_t max_cap) 
  * handed to the lock-step loop.  Any pointer may be NULL. */
 int mplh_batch_grow_stats(void *session, int32_t *rounds, int64_t *reruns, int64_t *first_cap, int64_t *last_cap,
                           int32_t *lockstep) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq) {
-    g_err = "null session";
-    return 1;
-  }
-  auto put = [&](const auto *mq) {
-    if (rounds) *rounds = mq->growRounds();
-    if (reruns) *reruns = mq->growReruns();
-    if (first_cap) *first_cap = mq->growFirstCap();
-    if (last_cap) *last_cap = mq->growLastCap();
-    if (lockstep) *lockstep = mq->growLockstep();
-  };
-  if (s->dim == 2) put((const MPL::MultiQueryPlanner<2> *)s->mq);
-  else put((const MPL::MultiQueryPlanner<3> *)s->mq);
-  return 0;
+  return with_session(session, [&](const auto &mq, BatchSession &) {
+    if (rounds) *rounds = mq.growRounds();
+    if (reruns) *reruns = mq.growReruns();
+    if (first_cap) *first_cap = mq.growFirstCap();
+    if (last_cap) *last_cap = mq.growLastCap();
+    if (lockstep) *lockstep = mq.growLockstep();
+  });
 }
 
 /* The last plan of the session: *device = 1 when it ran the occupancy device search, 2 when it ran the
  * cost-term device search, 3 when it ran the growing device search (then *slots and *arena_bytes describe
  * its (first round's) arenas), 0 when it ran the lock-step loop. */
 int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t *arena_bytes) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq) {
-    g_err = "null session";
-    return 1;
-  }
-  auto put = [&](const auto *mq) {
-    if (device) *device = mq->lastDevicePath();
-    if (slots) *slots = mq->searchSlots();
-    if (arena_bytes) *arena_bytes = mq->searchArenaBytes();
-  };
-  if (s->dim == 2) put((const MPL::MultiQueryPlanner<2> *)s->mq);
-  else put((const MPL::MultiQueryPlanner<3> *)s->mq);
-  return 0;
+  return with_session(session, [&](const auto &mq, BatchSession &) {
+    if (device) *device = mq.lastDevicePath();
+    if (slots) *slots = mq.searchSlots();
+    if (arena_bytes) *arena_bytes = mq.searchArenaBytes();
+  });
 }
 
 /* mplh_batch_plan that keeps every query's trajectory (action ids) and, with collect_closed, closed set
@@ -364,52 +292,7 @@ int mplh_batch_last_path(void *session, int32_t *device, int32_t *slots, int64_t
  * them, whatever max_num is. */
 int mplh_batch_plan_keep(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
                          int max_num, int collect_closed, mplh_query_result *out, double *totals) {
-  try {
-    BatchSession *s = (BatchSession *)session;
-    if (!s || !s->mq) throw std::runtime_error("null session");
-    auto go = [&](auto *mq, auto dimtag) {
-      constexpr int Dim = decltype(dimtag)::value;
-      mq->setCollectClosed(collect_closed != 0);
-      // the session's later plans must not keep collecting, whatever plan() does
-      struct Reset {
-        decltype(mq) p;
-        ~Reset() { p->setCollectClosed(false); }
-      } reset{mq};
-      vec_E<Waypoint<Dim>> S, G;
-      for (int q = 0; q < n_q; q++) {
-        S.push_back(mplh::wp_from<Dim>(starts[q], s->control));
-        G.push_back(mplh::wp_from<Dim>(goals[q], s->control));
-      }
-      auto t0 = std::chrono::steady_clock::now();
-      auto res = mq->plan(S, G, eps, max_num);
-      const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      s->aoff.assign((size_t)n_q + 1, 0);
-      s->coff.assign((size_t)n_q + 1, 0);
-      s->actions.clear();
-      s->closed.clear();
-      for (int q = 0; q < n_q; q++) {
-        out[q].valid = res[q].valid ? 1 : 0;
-        out[q].cost = res[q].cost;
-        out[q].expanded = res[q].expanded;
-        out[q].n_closed = (int)res[q].n_closed;
-        out[q].n_actions = (int)res[q].actions.size();
-        s->actions.insert(s->actions.end(), res[q].actions.begin(), res[q].actions.end());
-        s->closed.insert(s->closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
-        s->aoff[q + 1] = (int64_t)s->actions.size();
-        s->coff[q + 1] = (int64_t)s->closed.size();
-      }
-      if (totals) {
-        totals[0] = (double)mq->iterations(); totals[1] = (double)mq->nodes_expanded(); totals[2] = secs;
-        totals[3] = mq->t_pop(); totals[4] = mq->t_device(); totals[5] = mq->t_relax(); totals[6] = 0.0;
-      }
-    };
-    if (s->dim == 2) go((MPL::MultiQueryPlanner<2> *)s->mq, std::integral_constant<int, 2>());
-    else go((MPL::MultiQueryPlanner<3> *)s->mq, std::integral_constant<int, 3>());
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 1;
-  }
+  return batch_plan(session, starts, goals, n_q, eps, max_num, true, collect_closed != 0, out, totals);
 }
 
 /* Copies what the last mplh_batch_plan_keep kept: query q's action ids at actions[action_offset[q],
@@ -417,66 +300,28 @@ int mplh_batch_plan_keep(void *session, const mplx_waypoint *starts, const mplx_
  * that is too small fails the call with nothing written. */
 int mplh_batch_kept(void *session, int64_t *action_offset, int32_t *actions, int64_t cap_actions,
                     int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq) {
-    g_err = "null session";
-    return 1;
-  }
-  if (!action_offset || (!actions && !s->actions.empty()) || (closed_keys && !closed_offset)) {
-    g_err = "missing output array";
-    return 1;
-  }
-  if ((int64_t)s->actions.size() > cap_actions || (closed_keys && (int64_t)s->closed.size() > cap_closed)) {
-    g_err = (int64_t)s->actions.size() > cap_actions ? "action capacity too small" : "closed capacity too small";
-    return 1;
-  }
-  std::copy(s->aoff.begin(), s->aoff.end(), action_offset);
-  std::copy(s->actions.begin(), s->actions.end(), actions);
-  if (closed_keys) {
-    std::copy(s->coff.begin(), s->coff.end(), closed_offset);
-    std::copy(s->closed.begin(), s->closed.end(), closed_keys);
-  }
-  return 0;
-}
-
-/* mplh_batch_plan that also returns every query's trajectory (action ids, query q's at
- * actions[action_offset[q], action_offset[q+1])) and closed set (sorted lattice keys, likewise with
- * closed_offset; closed_keys NULL = skip).  A capacity that is too small fails the call. */
-int mplh_batch_plan_detail(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps,
-                           int max_num, mplh_query_result *out, double *totals, int64_t *action_offset, int32_t *actions,
-                           int64_t cap_actions, int64_t *closed_offset, uint64_t *closed_keys, int64_t cap_closed) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s || !s->mq || !action_offset || !actions || (closed_keys && !closed_offset)) {
-    g_err = !s || !s->mq ? "null session" : "missing output array";
-    return 1;
-  }
-  const int rc = mplh_batch_plan_keep(session, starts, goals, n_q, eps, max_num, closed_keys != nullptr, out, totals);
-  if (rc) return rc;
-  return mplh_batch_kept(session, action_offset, actions, cap_actions, closed_offset, closed_keys, cap_closed);
+  return with_session(session, [&](const auto &, BatchSession &s) {
+    if (!action_offset || (!actions && !s.actions.empty()) || (closed_keys && !closed_offset))
+      throw std::runtime_error("missing output array");
+    if ((int64_t)s.actions.size() > cap_actions) throw std::runtime_error("action capacity too small");
+    if (closed_keys && (int64_t)s.closed.size() > cap_closed) throw std::runtime_error("closed capacity too small");
+    std::copy(s.aoff.begin(), s.aoff.end(), action_offset);
+    std::copy(s.actions.begin(), s.actions.end(), actions);
+    if (closed_keys) {
+      std::copy(s.coff.begin(), s.coff.end(), closed_offset);
+      std::copy(s.closed.begin(), s.closed.end(), closed_keys);
+    }
+  });
 }
 
 /* Frees the session incl. the search states it kept; seconds spent are returned in *release_seconds. */
 int mplh_batch_close(void *session, double *release_seconds) {
-  BatchSession *s = (BatchSession *)session;
-  if (!s) return 0;
+  if (!session) return 0;
   auto t0 = std::chrono::steady_clock::now();
-  if (s->dim == 2) delete (MPL::MultiQueryPlanner<2> *)s->mq;
-  else delete (MPL::MultiQueryPlanner<3> *)s->mq;
-  delete s;
+  with_session(session, [](auto &mq, BatchSession &) { delete &mq; });
+  delete (BatchSession *)session;
   if (release_seconds) *release_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   return 0;
-}
-
-/* One-shot form: open, plan one set, close.  totals[6] = seconds spent freeing the search states. */
-int mplh_plan_batch(const mplh_plan_args *a, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q,
-                    mplh_query_result *out, double *totals) {
-  void *s = mplh_batch_open(a);
-  if (!s) return 1;
-  const int rc = mplh_batch_plan(s, starts, goals, n_q, a->eps, a->max_num, out, totals);
-  double rel = 0;
-  mplh_batch_close(s, &rel);
-  if (totals) totals[6] = rel;
-  return rc;
 }
 }
 
@@ -486,23 +331,12 @@ namespace {
 template <int Dim>
 void put_samples(const Trajectory<Dim> &traj, int n_samples, double *samples) {
   const auto cmds = traj.sample(n_samples);
-  const int W = 4 * Dim + 3;
-  for (int i = 0; i <= n_samples; i++) {
-    double *o = samples + (size_t)i * W;
-    for (int d = 0; d < Dim; d++) { o[d] = cmds[i].pos(d); o[Dim + d] = cmds[i].vel(d); o[2 * Dim + d] = cmds[i].acc(d); o[3 * Dim + d] = cmds[i].jrk(d); }
-    o[4 * Dim] = cmds[i].yaw; o[4 * Dim + 1] = cmds[i].yaw_dot; o[4 * Dim + 2] = cmds[i].t;
-  }
+  for (int i = 0; i <= n_samples; i++) mplh::put_command_row<Dim>(samples, i, cmds[i]);
 }
 template <int Dim>
 void put_waypoints(const Trajectory<Dim> &traj, double *waypoints) {
-  const int V = 4 * Dim + 2;
   const auto ws = traj.getWaypoints();
-  for (std::size_t i = 0; i < ws.size(); i++) {
-    double *o = waypoints + i * V;
-    const Waypoint<Dim> &w = ws[i];
-    for (int d = 0; d < Dim; d++) { o[d] = w.pos(d); o[Dim + d] = w.vel(d); o[2 * Dim + d] = w.acc(d); o[3 * Dim + d] = w.jrk(d); }
-    o[4 * Dim] = w.yaw; o[4 * Dim + 1] = w.t;
-  }
+  for (std::size_t i = 0; i < ws.size(); i++) mplh::put_waypoint_row<Dim>(waypoints, i, ws[i]);
 }
 /// Trajectory<Dim> of n_seg segments with durations seg_t and coefficients coeff (mplh_traj_solve's layout), each
 /// segment with the control flag `control`
@@ -517,18 +351,6 @@ Trajectory<Dim> make_trajectory(int n_seg, const double *seg_t, const double *co
   }
   return Trajectory<Dim>(prs);
 }
-template <typename F>
-int with_traj_dim(int dim, F &&f) {
-  try {
-    if (dim == 2) f(std::integral_constant<int, 2>());
-    else if (dim == 3) f(std::integral_constant<int, 3>());
-    else { g_err = "dim must be 2 or 3"; return 1; }
-    return 0;
-  } catch (const std::exception &e) {
-    g_err = e.what();
-    return 2;
-  }
-}
 }  // namespace
 
 extern "C" {
@@ -538,26 +360,20 @@ extern "C" {
  *   *n_seg     segments of the solved trajectory (0 when it is empty)
  *   seg_t      [n_wp - 1] getDts(): the segment times used
  *   coeff      [n_seg * (dim + 1) * 6] segment j's Primitive1D coefficients, highest order first, axes then yaw
- *   samples    [(n_samples + 1) * (4 dim + 3)] Trajectory::sample(n_samples) rows {pos, vel, acc, jrk, yaw, yaw_dot, t}
- *   waypoints  [(n_seg + 1) * (4 dim + 2)] Trajectory::getWaypoints() rows {pos, vel, acc, jrk, yaw, t}
+ *   samples    [(n_samples + 1) * (4 dim + 3)] Trajectory::sample(n_samples) as command rows (traj_rows.hpp)
+ *   waypoints  [(n_seg + 1) * (4 dim + 2)] Trajectory::getWaypoints() as waypoint rows (traj_rows.hpp)
  * 1: bad argument (dim, n_wp < 0, samples with n_samples < 1, missing wps); 2: solve() threw (no segment times). */
 int mplh_traj_solve(int dim, int control, int yaw_control, const mplx_waypoint *wps, const uint8_t *wp_control, int n_wp,
                     const double *dts, double v, int n_samples, int32_t *n_seg, double *seg_t, double *coeff,
                     double *samples, double *waypoints) {
   if (n_wp < 0 || (n_wp > 0 && !wps) || !n_seg || (samples && n_samples < 1)) { g_err = "bad argument"; return 1; }
   *n_seg = 0;
-  return with_traj_dim(dim, [&](auto dimtag) {
+  return mplh::with_dim(dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     MPL::TrajSolver<Dim> solver(control, yaw_control);
     if (wp_control) {
-      vec_E<Waypoint<Dim>> ws(n_wp);
-      for (int i = 0; i < n_wp; i++) {
-        ws[i].control = wp_control[i];
-        for (int d = 0; d < Dim; d++) {
-          ws[i].pos(d) = wps[i].pos[d]; ws[i].vel(d) = wps[i].vel[d]; ws[i].acc(d) = wps[i].acc[d]; ws[i].jrk(d) = wps[i].jrk[d];
-        }
-        ws[i].yaw = wps[i].yaw;
-      }
+      vec_E<Waypoint<Dim>> ws;
+      for (int i = 0; i < n_wp; i++) ws.push_back(mplh::wp_from<Dim>(wps[i], wp_control[i]));
       solver.setWaypoints(ws);
     } else {
       vec_E<Vecf<Dim>> path(n_wp);
@@ -587,7 +403,7 @@ int mplh_traj_solve(int dim, int control, int yaw_control, const mplx_waypoint *
 int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coeff, int control, int n_samples,
                      double *samples, double *waypoints) {
   if (n_seg < 0 || (n_seg > 0 && (!seg_t || !coeff)) || (samples && n_samples < 1)) { g_err = "bad argument"; return 1; }
-  return with_traj_dim(dim, [&](auto dimtag) {
+  return mplh::with_dim(dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     const Trajectory<Dim> traj = make_trajectory<Dim>(n_seg, seg_t, coeff, control);
     if (samples) put_samples<Dim>(traj, n_samples, samples);
@@ -637,7 +453,7 @@ int mplh_traj_scale(int dim, int n_seg, const double *seg_t, const double *coeff
     g_err = "bad argument";
     return 1;
   }
-  return with_traj_dim(dim, [&](auto dimtag) {
+  return mplh::with_dim(dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     const size_t n_slot = (size_t)(n_seg + 1) * 5 * Dim;
     *status = 0;
@@ -710,7 +526,7 @@ int mplh_traj_check(int dim, const int8_t *map, const int32_t *mdim, const doubl
       return 1;
     }
   if (offset[n_paths] > 0 && (!seg_t || !coeff)) { g_err = "bad argument"; return 1; }
-  return with_traj_dim(dim, [&](auto dimtag) {
+  return mplh::with_dim(dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     auto mu = std::make_shared<MPL::MapUtil<Dim>>();
     Vecf<Dim> ori;

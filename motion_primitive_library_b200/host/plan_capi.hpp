@@ -4,8 +4,29 @@
 #include "mpl_host.hpp"
 
 #include "plan_capi_types.h"
+#include "traj_rows.hpp"
 
 namespace mplh {
+// Runs f(std::integral_constant<int, Dim>()) for dim 2 or 3 and returns 0.  Any other dim returns 1 with
+// "dim must be 2 or 3" in err; an exception thrown by f returns `thrown` with its message in err.
+template <typename F>
+int with_dim(int dim, std::string &err, int thrown, F &&f) {
+  try {
+    if (dim == 2) f(std::integral_constant<int, 2>());
+    else if (dim == 3) f(std::integral_constant<int, 3>());
+    else { err = "dim must be 2 or 3"; return 1; }
+    return 0;
+  } catch (const std::exception &e) {
+    err = e.what();
+    return thrown;
+  }
+}
+template <int Dim>
+size_t n_cells(const mplh_plan_args *a) {
+  size_t n = 1;
+  for (int k = 0; k < Dim; k++) n *= (size_t)a->mdim[k];
+  return n;
+}
 template <int Dim>
 Waypoint<Dim> wp_from(const mplx_waypoint &p, int control) {
   Waypoint<Dim> w(control);
@@ -16,9 +37,9 @@ Waypoint<Dim> wp_from(const mplx_waypoint &p, int control) {
 template <int Dim>
 std::shared_ptr<MPL::MapUtil<Dim>> make_map(const mplh_plan_args *a) {
   auto mu = std::make_shared<MPL::MapUtil<Dim>>();
-  Vecf<Dim> ori; Veci<Dim> dim; size_t n = 1;
-  for (int k = 0; k < Dim; k++) { ori(k) = a->origin[k]; dim(k) = a->mdim[k]; n *= (size_t)a->mdim[k]; }
-  mu->setMap(ori, dim, MPL::Tmap(a->map, a->map + n), a->res);
+  Vecf<Dim> ori; Veci<Dim> dim;
+  for (int k = 0; k < Dim; k++) { ori(k) = a->origin[k]; dim(k) = a->mdim[k]; }
+  mu->setMap(ori, dim, MPL::Tmap(a->map, a->map + n_cells<Dim>(a)), a->res);
   return mu;
 }
 // Configure `planner` (whose env is already installed) from the flat args.
@@ -92,10 +113,9 @@ void run_iterative(MPL::MapPlanner<Dim> &planner, const mplh_plan_args *a, const
   export_result<Dim>(planner, ok, last, closed_keys, cap_closed, actions, cap_actions);
 }
 
-// plan(), then describe the recovered trajectory: samples = Trajectory::sample(N) as (N+1) rows of
-// {pos, vel, acc, jrk (Dim each), yaw, yaw_dot, t}; totals = {getTotalTime(), J(control), Jyaw(), #segments};
-// waypoints = getWaypoints() as rows of {pos, vel, acc, jrk (Dim each), yaw, t}; mids = evaluate(t) (the
-// Waypoint overload) at the N+1 sample times, same row layout as waypoints.
+// plan(), then describe the recovered trajectory: samples = Trajectory::sample(N) as N+1 command rows
+// (traj_rows.hpp); totals = {getTotalTime(), J(control), Jyaw(), #segments}; waypoints = getWaypoints() as
+// waypoint rows; mids = evaluate(t) (the Waypoint overload) at the N+1 sample times, as waypoint rows.
 template <int Dim>
 void run_trajectory(MPL::MapPlanner<Dim> &planner, const mplh_plan_args *a, int N, mplh_plan_result *r, double *samples,
                     double *totals, double *waypoints, int cap_wp, int32_t *n_wp, double *mids) {
@@ -109,22 +129,12 @@ void run_trajectory(MPL::MapPlanner<Dim> &planner, const mplh_plan_args *a, int 
   totals[2] = traj.Jyaw();
   totals[3] = (double)traj.segs.size();
   const auto cmds = traj.sample(N);
-  const int W = 4 * Dim + 3;
-  for (int i = 0; i <= N; i++) {
-    double *o = samples + (size_t)i * W;
-    for (int d = 0; d < Dim; d++) { o[d] = cmds[i].pos(d); o[Dim + d] = cmds[i].vel(d); o[2 * Dim + d] = cmds[i].acc(d); o[3 * Dim + d] = cmds[i].jrk(d); }
-    o[4 * Dim] = cmds[i].yaw; o[4 * Dim + 1] = cmds[i].yaw_dot; o[4 * Dim + 2] = cmds[i].t;
-  }
-  const int V = 4 * Dim + 2;
-  auto put = [&](double *o, const Waypoint<Dim> &w) {
-    for (int d = 0; d < Dim; d++) { o[d] = w.pos(d); o[Dim + d] = w.vel(d); o[2 * Dim + d] = w.acc(d); o[3 * Dim + d] = w.jrk(d); }
-    o[4 * Dim] = w.yaw; o[4 * Dim + 1] = w.t;
-  };
+  for (int i = 0; i <= N; i++) put_command_row<Dim>(samples, i, cmds[i]);
   const auto ws = traj.getWaypoints();
   *n_wp = (int)ws.size();
-  for (int i = 0; i < (int)ws.size() && i < cap_wp; i++) put(waypoints + (size_t)i * V, ws[i]);
+  for (int i = 0; i < (int)ws.size() && i < cap_wp; i++) put_waypoint_row<Dim>(waypoints, i, ws[i]);
   const decimal_t dt = traj.getTotalTime() / N;
-  for (int i = 0; i <= N; i++) put(mids + (size_t)i * V, traj.evaluate(i * dt));
+  for (int i = 0; i <= N; i++) put_waypoint_row<Dim>(mids, i, traj.evaluate(i * dt));
 }
 
 inline void fnv(uint64_t &h, const void *p, size_t n) {
@@ -155,14 +165,7 @@ void snapshot(MPL::MapPlanner<Dim> &planner, mplh_lpa_out *o) {
 template <int Dim>
 void run_lpa(MPL::MapPlanner<Dim> &planner, const std::shared_ptr<MPL::MapUtil<Dim>> &mu, const mplh_plan_args *a,
              const mplh_lpa_step *steps, int n_steps, mplh_lpa_out *outs, int32_t *actions, int cap_actions) {
-  vec_E<VecDf> U;
-  for (int i = 0; i < a->nU; i++) U.push_back(VecDf(a->U + (size_t)i * a->udim, a->U + (size_t)(i + 1) * a->udim));
-  planner.setU(U);
-  planner.setVmax(a->v_max); planner.setAmax(a->a_max); planner.setJmax(a->j_max); planner.setYawmax(a->yaw_max);
-  planner.setDt(a->T); planner.setW(a->w); planner.setWyaw(a->wyaw); planner.setEpsilon(a->eps);
-  planner.setTol(a->tol_pos, a->tol_vel, a->tol_acc);
-  planner.setMaxNum(a->max_num);
-  planner.setHeurIgnoreDynamics(a->heur_ignore_dynamics != 0);
+  configure<Dim>(planner, a);
   planner.setLPAstar(true);
   Waypoint<Dim> start = wp_from<Dim>(a->start, a->control);
   const Waypoint<Dim> goal = wp_from<Dim>(a->goal, a->control);

@@ -1,6 +1,7 @@
 """ctypes binding of libmpl_host.so: the C++ host planner (MPL::MapPlanner with the GPU env,
 MPL::MultiQueryPlanner) behind flat C structs.  See host/plan_capi.hpp."""
 import ctypes as C
+import functools
 from pathlib import Path
 
 import numpy as np
@@ -54,12 +55,89 @@ WAYPOINT_DTYPE = np.dtype(
 )
 
 
-def load_fn(path, fn):
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.POINTER(PlanArgs), C.POINTER(PlanResult), C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    f.restype = C.c_int
-    return L, f
+_vp, _i, _i64, _d = C.c_void_p, C.c_int, C.c_int64, C.c_double
+_i32p, _i64p, _argp, _resp = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PlanArgs), C.POINTER(PlanResult)
+# (argtypes, restype) of every function libmpl_host.so exports (host/mpl_host_capi.cpp)
+SIGNATURES = {
+    "mplh_last_error": ([], C.c_char_p),
+    "mplh_plan": ([_argp, _resp, _vp, _i, _vp, _i], _i),
+    "mplh_plan_trace": ([_argp, _resp, _vp, _i, _i32p], _i),
+    "mplh_plan_trajectory": ([_argp, _i, _resp, _vp, _vp, _vp, _i, _i32p, _vp], _i),
+    "mplh_iterative_plan": ([_argp, _vp, _i, _resp, _resp, _vp, _vp, _i, _vp, _i], _i),
+    "mplh_lpa_run": ([_argp, C.POINTER(LpaStep), _i, C.POINTER(LpaOut), _vp, _i], _i),
+    "mplh_batch_open": ([_argp], _vp),
+    "mplh_batch_plan": ([_vp, _vp, _vp, _i, _d, _i, _vp, _vp], _i),
+    "mplh_batch_plan_keep": ([_vp, _vp, _vp, _i, _d, _i, _i, _vp, _vp], _i),
+    "mplh_batch_kept": ([_vp, _vp, _vp, _i64, _vp, _vp, _i64], _i),
+    "mplh_batch_update_cells": ([_vp, _vp, _vp, _i], _i),
+    "mplh_batch_map_uploads": ([_vp, _i64p, _i64p], _i),
+    "mplh_batch_set_path": ([_vp, _i], _i),
+    "mplh_batch_set_grow_caps": ([_vp, _i64, _i64], _i),
+    "mplh_batch_grow_stats": ([_vp, _i32p, _i64p, _i64p, _i64p, _i32p], _i),
+    "mplh_batch_last_path": ([_vp, _i32p, _i32p, _i64p], _i),
+    "mplh_batch_close": ([_vp, C.POINTER(_d)], _i),
+    "mplh_traj_solve": ([_i, _i, _i, _vp, _vp, _i, _vp, _d, _i, _i32p, _vp, _vp, _vp, _vp], _i),
+    "mplh_traj_sample": ([_i, _i, _vp, _vp, _i, _i, _vp, _vp], _i),
+    "mplh_traj_scale": ([_i, _i, _vp, _vp, _i, _i, _d, _d, _d, _i, _i32p, C.POINTER(_d), _vp, _i32p, _vp, _vp], _i),
+    "mplh_solve": ([_d] * 5 + [_i32p, _vp], _i),
+    "mplh_traj_check": ([_i, _vp, _vp, _vp, _d, _vp, _d, _d, _vp, _d, _d, _d, _d, _i, _vp, _vp, _vp, _vp, _vp, _vp,
+                         _vp, _i, _vp, _vp, _vp, _vp], _i),
+}
+# the reference's mplh_traj_scale, with a trailing per-row flags array
+SIGNATURES["reft_traj_scale"] = (SIGNATURES["mplh_traj_scale"][0] + [_vp], _i)
+
+
+@functools.cache
+def _lib():
+    """libmpl_host.so, opened once, with every function declared from SIGNATURES."""
+    if not LIB.exists():
+        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
+    lib = C.CDLL(str(LIB))
+    for name, (argtypes, restype) in SIGNATURES.items():
+        if name.startswith("mplh_"):
+            f = getattr(lib, name)
+            f.argtypes, f.restype = argtypes, restype
+    return lib
+
+
+def _host():
+    """(libmpl_host.so, its mplh_plan), the pair callers of earlier versions unpack."""
+    lib = _lib()
+    return lib, lib.mplh_plan
+
+
+def bind(path, name, like=None):
+    """(lib, fn): the function `name` of the shared library at `path`, declared with the signature of `like`
+    (default `name`) in SIGNATURES: a driver function that mirrors an mplh_* entry point."""
+    lib = C.CDLL(str(path))
+    fn = getattr(lib, name)
+    fn.argtypes, fn.restype = SIGNATURES[like or name]
+    return lib, fn
+
+
+# the loaders of earlier versions, kept as public names: bind() with the mirrored entry point fixed
+load_fn = functools.partial(bind, like="mplh_plan")
+load_lpa_fn = functools.partial(bind, like="mplh_lpa_run")
+load_traj_fn = functools.partial(bind, like="mplh_plan_trajectory")
+load_iter_fn = functools.partial(bind, like="mplh_iterative_plan")
+load_traj_solve_fn = functools.partial(bind, like="mplh_traj_solve")
+load_solve_fn = functools.partial(bind, like="mplh_solve")
+load_traj_check_fn = functools.partial(bind, like="mplh_traj_check")
+
+
+def load_traj_scale_fn(path, fn, flags=False):
+    """bind() with mplh_traj_scale's signature, plus the reference driver's trailing per-row flags when `flags`."""
+    return bind(path, fn, "reft_traj_scale" if flags else "mplh_traj_scale")
+
+
+def _check(lib, rc):
+    """Raise RuntimeError with lib's mplh_last_error() when rc is nonzero."""
+    if rc != 0:
+        err = getattr(lib, "mplh_last_error", None)
+        if err is None:
+            raise RuntimeError(f"call failed rc={rc}")
+        err.restype = C.c_char_p
+        raise RuntimeError(err().decode())
 
 
 def make_args(dim, control, grid, mdim, origin, res, U, start, goal, T=1.0, w=10.0, wyaw=1.0, eps=1.0, v_max=-1.0,
@@ -99,10 +177,7 @@ def run_plan(fn, lib, args, cap=1 << 21):
     r = PlanResult()
     closed = np.zeros(cap, dtype=np.uint64)
     actions = np.zeros(65536, dtype=np.int32)
-    rc = fn(C.byref(args), C.byref(r), closed.ctypes.data, cap, actions.ctypes.data, actions.size)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"plan failed rc={rc}")
+    _check(lib, fn(C.byref(args), C.byref(r), closed.ctypes.data, cap, actions.ctypes.data, actions.size))
     out = {k: getattr(r, k) for k, _ in PlanResult._fields_}
     out["closed"] = closed[: min(r.n_closed, cap)].copy()
     out["actions"] = actions[: r.n_actions].copy()
@@ -127,10 +202,7 @@ def run_lpa(fn, lib, args, script, cap_actions=4096):
             steps[k].n = int(st[1])
     outs = (LpaOut * len(script))()
     actions = np.full((len(script), cap_actions), -1, dtype=np.int32)
-    rc = fn(C.byref(args), steps, len(script), outs, actions.ctypes.data, cap_actions)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"lpa session failed rc={rc}")
+    _check(lib, fn(C.byref(args), steps, len(script), outs, actions.ctypes.data, cap_actions))
     res = []
     for k in range(len(script)):
         d = {name: getattr(outs[k], name) for name, _ in LpaOut._fields_}
@@ -140,32 +212,12 @@ def run_lpa(fn, lib, args, script, cap_actions=4096):
     return res
 
 
-def load_lpa_fn(path, fn):
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.POINTER(PlanArgs), C.POINTER(LpaStep), C.c_int, C.POINTER(LpaOut), C.c_void_p, C.c_int]
-    f.restype = C.c_int
-    return L, f
-
-
 def lpa_session(args, script):
     """MPL::MapPlanner with setLPAstar(true) and the GPU env: plan / getLinkedNodes / updateBlockedNodes /
     updateClearedNodes / getSubStateSpace as scripted; expansion, the linked-voxel walk and the
     is_free(pr) re-validation run on the device."""
-    if not LIB.exists():
-        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
-    lib, fn = load_lpa_fn(LIB, "mplh_lpa_run")
-    lib.mplh_last_error.restype = C.c_char_p
-    return run_lpa(fn, lib, args, script)
-
-
-def load_traj_fn(path, fn):
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.POINTER(PlanArgs), C.c_int, C.POINTER(PlanResult), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                  C.POINTER(C.c_int32), C.c_void_p]
-    f.restype = C.c_int
-    return L, f
+    lib = _lib()
+    return run_lpa(lib.mplh_lpa_run, lib, args, script)
 
 
 def run_trajectory(fn, lib, args, n_samples=50, cap_wp=4096):
@@ -179,11 +231,8 @@ def run_trajectory(fn, lib, args, n_samples=50, cap_wp=4096):
     wps = np.zeros((cap_wp, 4 * dim + 2))
     mids = np.zeros((n_samples + 1, 4 * dim + 2))
     n_wp = C.c_int32(0)
-    rc = fn(C.byref(args), n_samples, C.byref(r), samples.ctypes.data, totals.ctypes.data, wps.ctypes.data, cap_wp,
-            C.byref(n_wp), mids.ctypes.data)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"trajectory failed rc={rc}")
+    _check(lib, fn(C.byref(args), n_samples, C.byref(r), samples.ctypes.data, totals.ctypes.data, wps.ctypes.data,
+                   cap_wp, C.byref(n_wp), mids.ctypes.data))
     out = {k: getattr(r, k) for k, _ in PlanResult._fields_}
     out.update(commands=samples, total_time=totals[0], J=totals[1], Jyaw=totals[2], segments=int(totals[3]),
                waypoints=wps[: min(n_wp.value, cap_wp)].copy(), evaluated=mids)
@@ -192,20 +241,8 @@ def run_trajectory(fn, lib, args, n_samples=50, cap_wp=4096):
 
 def plan_trajectory(args, n_samples=50):
     """MPL::MapPlanner::plan() with the GPU env + the recovered Trajectory (sample / waypoints / efforts)."""
-    if not LIB.exists():
-        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
-    lib, fn = load_traj_fn(LIB, "mplh_plan_trajectory")
-    lib.mplh_last_error.restype = C.c_char_p
-    return run_trajectory(fn, lib, args, n_samples)
-
-
-def load_iter_fn(path, fn):
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_int, C.POINTER(PlanResult), C.POINTER(PlanResult), C.c_void_p,
-                  C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    f.restype = C.c_int
-    return L, f
+    lib = _lib()
+    return run_trajectory(lib.mplh_plan_trajectory, lib, args, n_samples)
 
 
 def run_iterative(fn, lib, args, search_radius, max_iter=3, cap=1 << 21):
@@ -218,11 +255,8 @@ def run_iterative(fn, lib, args, search_radius, max_iter=3, cap=1 << 21):
     rad[: len(search_radius)] = search_radius
     closed = np.zeros(cap, dtype=np.uint64)
     actions = np.zeros(65536, dtype=np.int32)
-    rc = fn(C.byref(args), rad.ctypes.data, int(max_iter), C.byref(first), C.byref(last), info.ctypes.data,
-            closed.ctypes.data, cap, actions.ctypes.data, actions.size)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"iterative plan failed rc={rc}")
+    _check(lib, fn(C.byref(args), rad.ctypes.data, int(max_iter), C.byref(first), C.byref(last), info.ctypes.data,
+                   closed.ctypes.data, cap, actions.ctypes.data, actions.size))
     f = {k: getattr(first, k) for k, _ in PlanResult._fields_}
     l = {k: getattr(last, k) for k, _ in PlanResult._fields_}
     l["closed"] = closed[: min(last.n_closed, cap)].copy()
@@ -233,68 +267,23 @@ def run_iterative(fn, lib, args, search_radius, max_iter=3, cap=1 << 21):
 
 def iterative_plan(args, search_radius, max_iter=3):
     """MPL::MapPlanner::plan() + iterativePlan() with the GPU env (tunnels built on the device)."""
-    if not LIB.exists():
-        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
-    lib, fn = load_iter_fn(LIB, "mplh_iterative_plan")
-    lib.mplh_last_error.restype = C.c_char_p
-    return run_iterative(fn, lib, args, search_radius, max_iter)
-
-
-def _host():
-    if not LIB.exists():
-        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
-    lib, fn = load_fn(LIB, "mplh_plan")
-    lib.mplh_last_error.restype = C.c_char_p
-    lib.mplh_plan_batch.argtypes = [C.POINTER(PlanArgs), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.mplh_plan_batch.restype = C.c_int
-    lib.mplh_batch_open.argtypes = [C.POINTER(PlanArgs)]
-    lib.mplh_batch_open.restype = C.c_void_p
-    lib.mplh_batch_plan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_void_p, C.c_void_p]
-    lib.mplh_batch_plan.restype = C.c_int
-    lib.mplh_batch_close.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
-    lib.mplh_batch_close.restype = C.c_int
-    lib.mplh_batch_update_cells.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.mplh_batch_update_cells.restype = C.c_int
-    lib.mplh_batch_map_uploads.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-    lib.mplh_batch_map_uploads.restype = C.c_int
-    lib.mplh_batch_set_path.argtypes = [C.c_void_p, C.c_int]
-    lib.mplh_batch_set_path.restype = C.c_int
-    lib.mplh_batch_last_path.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
-    lib.mplh_batch_last_path.restype = C.c_int
-    lib.mplh_batch_plan_detail.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                           C.c_int64]
-    lib.mplh_batch_plan_detail.restype = C.c_int
-    lib.mplh_batch_plan_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int, C.c_int,
-                                         C.c_void_p, C.c_void_p]
-    lib.mplh_batch_plan_keep.restype = C.c_int
-    lib.mplh_batch_kept.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64]
-    lib.mplh_batch_kept.restype = C.c_int
-    lib.mplh_batch_grow_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
-                                          C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
-    lib.mplh_batch_grow_stats.restype = C.c_int
-    lib.mplh_batch_set_grow_caps.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
-    lib.mplh_batch_set_grow_caps.restype = C.c_int
-    return lib, fn
+    lib = _lib()
+    return run_iterative(lib.mplh_iterative_plan, lib, args, search_radius, max_iter)
 
 
 def plan(args):
     """MPL::MapPlanner<Dim>::plan() with the GPU env (one query)."""
-    lib, fn = _host()
-    return run_plan(fn, lib, args)
+    lib = _lib()
+    return run_plan(lib.mplh_plan, lib, args)
 
 
 def plan_trace(args, cap=1 << 20):
     """plan() with the GPU env, returning also the expanded nodes in A* pop order (WAYPOINT_DTYPE array)."""
-    lib, _ = _host()
-    lib.mplh_plan_trace.argtypes = [C.POINTER(PlanArgs), C.POINTER(PlanResult), C.c_void_p, C.c_int, C.POINTER(C.c_int32)]
-    lib.mplh_plan_trace.restype = C.c_int
+    lib = _lib()
     r = PlanResult()
     trace = np.zeros(cap, dtype=WAYPOINT_DTYPE)
     n = C.c_int32(0)
-    rc = lib.mplh_plan_trace(C.byref(args), C.byref(r), trace.ctypes.data, cap, C.byref(n))
-    if rc != 0:
-        raise RuntimeError(lib.mplh_last_error().decode())
+    _check(lib, lib.mplh_plan_trace(C.byref(args), C.byref(r), trace.ctypes.data, cap, C.byref(n)))
     out = {k: getattr(r, k) for k, _ in PlanResult._fields_}
     out["trace"] = trace[: n.value].copy()
     return out
@@ -337,63 +326,63 @@ class BatchPlanner:
     _RAN = {0: "lockstep", 1: "device", 2: "device_cost_terms", 3: "device_grow"}
 
     def __init__(self, args, path="auto"):
-        self._lib, _ = _host()
+        self._lib = _lib()
         self._args = args  # keeps the arrays the struct points at alive
         self._h = self._lib.mplh_batch_open(C.byref(args))
-        if not self._h:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        _check(self._lib, 0 if self._h else 1)
         self.set_path(path)
+
+    def _call(self, name, *a):
+        _check(self._lib, getattr(self._lib, name)(self._h, *a))
 
     def set_path(self, path):
         if path not in self.PATHS:
             raise ValueError(f"path must be one of {sorted(self.PATHS)}")
-        if self._lib.mplh_batch_set_path(self._h, self.PATHS[path]) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_set_path", self.PATHS[path])
 
     def set_grow_caps(self, first_cap=0, max_cap=0):
         """Diagnostics: the growing device search's first and largest arena capacity in records (0 = automatic;
         see mplx_plan_batch_grow).  Queries that outgrow max_cap run through the lock-step loop."""
-        if self._lib.mplh_batch_set_grow_caps(self._h, int(first_cap), int(max_cap)) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_set_grow_caps", int(first_cap), int(max_cap))
 
     def _last_path(self):
         dev, slots, nbytes = C.c_int32(0), C.c_int32(0), C.c_int64(0)
-        if self._lib.mplh_batch_last_path(self._h, C.byref(dev), C.byref(slots), C.byref(nbytes)) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_last_path", C.byref(dev), C.byref(slots), C.byref(nbytes))
         d = dict(path=self._RAN[dev.value], slots=int(slots.value), arena_bytes=int(nbytes.value))
         rounds, lockstep = C.c_int32(0), C.c_int32(0)
         reruns, first_cap, last_cap = C.c_int64(0), C.c_int64(0), C.c_int64(0)
-        if self._lib.mplh_batch_grow_stats(self._h, C.byref(rounds), C.byref(reruns), C.byref(first_cap),
-                                           C.byref(last_cap), C.byref(lockstep)) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_grow_stats", C.byref(rounds), C.byref(reruns), C.byref(first_cap), C.byref(last_cap),
+                   C.byref(lockstep))
         d.update(grow_rounds=int(rounds.value), grow_reruns=int(reruns.value), grow_first_cap=int(first_cap.value),
                  grow_last_cap=int(last_cap.value), grow_lockstep=int(lockstep.value))
         return d
+
+    def _plan(self, name, starts, goals, eps, max_num, *keep):
+        """mplh_batch_plan or, with keep = (collect_closed,), mplh_batch_plan_keep: (per-query results, totals)."""
+        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
+        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
+        nq = len(starts)
+        out = (QueryResult * max(nq, 1))()
+        totals = np.zeros(7)
+        self._call(name, starts.ctypes.data, goals.ctypes.data, nq, self._args.eps if eps is None else eps,
+                   self._args.max_num if max_num is None else max_num, *keep, out, totals.ctypes.data)
+        res = np.zeros(nq, dtype=_QRES)
+        for q in range(nq):
+            res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        return res, totals
 
     def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True):
         """plan() that also returns every query's trajectory (action ids) and closed set (sorted lattice keys):
         (res, totals, actions, closed) with one array per query in actions / closed.  Any max_num, including
         max_num <= 0 (unbounded): the outputs are sized from the results."""
-        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
-        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
-        nq = len(starts)
-        mx = self._args.max_num if max_num is None else max_num
-        out = (QueryResult * max(nq, 1))()
-        totals = np.zeros(7)
-        if self._lib.mplh_batch_plan_keep(self._h, starts.ctypes.data, goals.ctypes.data, nq,
-                                          self._args.eps if eps is None else eps, mx, 1 if closed else 0, out,
-                                          totals.ctypes.data) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
-        res = np.zeros(nq, dtype=_QRES)
-        for q in range(nq):
-            res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        res, totals = self._plan("mplh_batch_plan_keep", starts, goals, eps, max_num, 1 if closed else 0)
+        nq = len(res)
         na, nc = int(res["n_actions"].sum()), int(res["n_closed"].sum()) if closed else 0
         aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
         acts = np.zeros(max(na, 1), np.int32)
         keys = np.zeros(max(nc, 1), np.uint64) if closed else None
-        if self._lib.mplh_batch_kept(self._h, aoff.ctypes.data, acts.ctypes.data, acts.size, coff.ctypes.data,
-                                     None if keys is None else keys.ctypes.data, 0 if keys is None else keys.size) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_kept", aoff.ctypes.data, acts.ctypes.data, acts.size, coff.ctypes.data,
+                   None if keys is None else keys.ctypes.data, 0 if keys is None else keys.size)
         tot = self._totals(totals)
         return (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
                 [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
@@ -405,19 +394,7 @@ class BatchPlanner:
         return t
 
     def plan(self, starts, goals, eps=None, max_num=None):
-        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
-        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
-        nq = len(starts)
-        out = (QueryResult * max(nq, 1))()
-        totals = np.zeros(7)
-        rc = self._lib.mplh_batch_plan(self._h, starts.ctypes.data, goals.ctypes.data, nq,
-                                       self._args.eps if eps is None else eps,
-                                       self._args.max_num if max_num is None else max_num, out, totals.ctypes.data)
-        if rc != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
-        res = np.zeros(nq, dtype=_QRES)
-        for q in range(nq):
-            res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        res, totals = self._plan("mplh_batch_plan", starts, goals, eps, max_num)
         return res, self._totals(totals)
 
     def update_cells(self, cells, values):
@@ -427,14 +404,12 @@ class BatchPlanner:
         values = np.ascontiguousarray(values, dtype=np.int8).reshape(-1)
         if values.size != len(cells):
             raise ValueError("one value per cell")
-        if self._lib.mplh_batch_update_cells(self._h, cells.ctypes.data, values.ctypes.data, len(cells)) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_update_cells", cells.ctypes.data, values.ctypes.data, len(cells))
 
     def map_uploads(self):
         """(full, delta): whole-grid uploads and sparse updates the session's env has made."""
         full, delta = C.c_int64(0), C.c_int64(0)
-        if self._lib.mplh_batch_map_uploads(self._h, C.byref(full), C.byref(delta)) != 0:
-            raise RuntimeError(self._lib.mplh_last_error().decode())
+        self._call("mplh_batch_map_uploads", C.byref(full), C.byref(delta))
         return full.value, delta.value
 
     def close(self) -> float:
@@ -451,25 +426,6 @@ class BatchPlanner:
             self.close()
         except Exception:
             pass
-
-
-def _traj_lib():
-    if not LIB.exists():
-        raise ImportError(f"{LIB} not built (python -c 'import __graft_entry__ as g; g.build()')")
-    lib = C.CDLL(str(LIB))
-    lib.mplh_last_error.restype = C.c_char_p
-    return lib
-
-
-def load_traj_solve_fn(path, fn):
-    """fn(dim, control, yaw_control, wps, wp_control, n_wp, dts, v, n_samples, n_seg, seg_t, coeff, samples,
-    waypoints): mplh_traj_solve's signature (host/mpl_host_capi.cpp)."""
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_int,
-                  C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    f.restype = C.c_int
-    return L, f
 
 
 def run_traj_solve(fn, lib, dim, control, pos=None, waypoints=None, wp_control=None, dts=None, v=1.0, yaw_control=0x01,
@@ -496,12 +452,9 @@ def run_traj_solve(fn, lib, dim, control, pos=None, waypoints=None, wp_control=N
     samples = np.zeros((n_samples + 1, 4 * dim + 3))
     wout = np.zeros((max(n, 1), 4 * dim + 2))
     n_seg = C.c_int32(0)
-    rc = fn(dim, control, yaw_control, wps.ctypes.data if n else None, None if ctl is None else ctl.ctypes.data, n,
-            None if d is None else d.ctypes.data, float(v), n_samples, C.byref(n_seg), seg_t.ctypes.data,
-            coeff.ctypes.data, samples.ctypes.data, wout.ctypes.data)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"trajectory solve failed rc={rc}")
+    _check(lib, fn(dim, control, yaw_control, wps.ctypes.data if n else None, None if ctl is None else ctl.ctypes.data,
+                   n, None if d is None else d.ctypes.data, float(v), n_samples, C.byref(n_seg), seg_t.ctypes.data,
+                   coeff.ctypes.data, samples.ctypes.data, wout.ctypes.data))
     s = n_seg.value
     return dict(segments=s, seg_t=seg_t[: max(n - 1, 0)].copy(), coeff=coeff[:s].copy(), samples=samples,
                 waypoints=wout[: s + 1 if s else 0].copy())
@@ -510,41 +463,22 @@ def run_traj_solve(fn, lib, dim, control, pos=None, waypoints=None, wp_control=N
 def traj_solve(dim, control, **kw):
     """MPL::TrajSolver on the host (mpl_host.hpp: the reference's dense formulation, one path).  Arguments as
     run_traj_solve."""
-    lib = _traj_lib()
-    _, fn = load_traj_solve_fn(LIB, "mplh_traj_solve")
-    return run_traj_solve(fn, lib, dim, control, **kw)
+    lib = _lib()
+    return run_traj_solve(lib.mplh_traj_solve, lib, dim, control, **kw)
 
 
 def traj_sample(dim, seg_t, coeff, control, n_samples):
     """Trajectory<dim> built on the host from segment times and Primitive1D coefficients (segments x (dim+1) x 6,
     axes then yaw), each segment with the control flag `control`: (sample(n_samples), getWaypoints()) as arrays
     of rows {pos, vel, acc, jrk, yaw, yaw_dot, t} and {pos, vel, acc, jrk, yaw, t}."""
-    lib = _traj_lib()
-    lib.mplh_traj_sample.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
-                                     C.c_void_p]
-    lib.mplh_traj_sample.restype = C.c_int
+    lib = _lib()
     seg_t = np.ascontiguousarray(seg_t, dtype=np.float64)
     coeff = np.ascontiguousarray(coeff, dtype=np.float64).reshape(len(seg_t), dim + 1, 6)
     samples = np.zeros((n_samples + 1, 4 * dim + 3))
     wout = np.zeros((len(seg_t) + 1, 4 * dim + 2))
-    rc = lib.mplh_traj_sample(dim, len(seg_t), seg_t.ctypes.data, coeff.ctypes.data, control, n_samples,
-                              samples.ctypes.data, wout.ctypes.data)
-    if rc != 0:
-        raise RuntimeError(lib.mplh_last_error().decode())
+    _check(lib, lib.mplh_traj_sample(dim, len(seg_t), seg_t.ctypes.data, coeff.ctypes.data, control, n_samples,
+                                     samples.ctypes.data, wout.ctypes.data))
     return samples, wout[: len(seg_t) + 1 if len(seg_t) else 0]
-
-
-def load_traj_scale_fn(path, fn, flags=False):
-    """fn(dim, n_seg, seg_t, coeff, control, mode, mv, ri, rf, n_samples, status, total_t, seg_T, n_lambda, lambda,
-    samples[, flags]): mplh_traj_scale's signature (host/mpl_host_capi.cpp), with the reference driver's trailing
-    per-row flags when `flags`."""
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
-                  C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_double), C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
-                  C.c_void_p] + ([C.c_void_p] if flags else [])
-    f.restype = C.c_int
-    return L, f
 
 
 def run_traj_scale(fn, lib, dim, seg_t, coeff, mode, mv=1.0, ri=1.0, rf=1.0, control=0x07, n_samples=50, flags=False):
@@ -563,10 +497,7 @@ def run_traj_scale(fn, lib, dim, seg_t, coeff, mode, mv=1.0, ri=1.0, rf=1.0, con
     fl = np.zeros(n_samples + 1, dtype=np.uint8)
     args = [dim, n, seg_t.ctypes.data, coeff.ctypes.data, control, mode, float(mv), float(ri), float(rf), n_samples,
             C.byref(st), C.byref(tot), seg_T.ctypes.data, C.byref(nl), lam.ctypes.data, samples.ctypes.data]
-    rc = fn(*(args + ([fl.ctypes.data] if flags else [])))
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"trajectory scale failed rc={rc}")
+    _check(lib, fn(*(args + ([fl.ctypes.data] if flags else []))))
     r = dict(status=st.value, total_t=tot.value, seg_T=seg_T[:n].copy(), **{"lambda": lam[: nl.value].copy()},
              samples=samples)
     if flags:
@@ -579,17 +510,8 @@ def traj_scale(dim, seg_t, coeff, mode, **kw):
 
     As in the reference, sample(N)'s last time N * (total / N) can land an ulp past the last lambda segment;
     getTau then finds no root and that row is the trajectory's start state."""
-    lib = _traj_lib()
-    _, fn = load_traj_scale_fn(LIB, "mplh_traj_scale")
-    return run_traj_scale(fn, lib, dim, seg_t, coeff, mode, **kw)
-
-
-def load_solve_fn(path, fn):
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    f.argtypes = [C.c_double] * 5 + [C.POINTER(C.c_int32), C.c_void_p]
-    f.restype = C.c_int
-    return L, f
+    lib = _lib()
+    return run_traj_scale(lib.mplh_traj_scale, lib, dim, seg_t, coeff, mode, **kw)
 
 
 def run_solve(fn, a, b, c, d, e):
@@ -602,22 +524,7 @@ def run_solve(fn, a, b, c, d, e):
 
 def solve_roots(a, b, c, d, e):
     """The host's closed-form root solver (mpl_host.hpp), as run_solve."""
-    _traj_lib()
-    _, fn = load_solve_fn(LIB, "mplh_solve")
-    return run_solve(fn, a, b, c, d, e)
-
-
-def load_traj_check_fn(path, fn):
-    """fn(dim, map, mdim, origin, res, potential, potential_weight, gradient_weight, region, v_max, a_max, j_max,
-    yaw_max, n_paths, offset, seg_t, coeff, control, total_t, n_lambda, lambda, nthreads, status, cost, seg_free,
-    seg_valid): mplh_traj_check's signature (host/mpl_host_capi.cpp)."""
-    L = C.CDLL(str(path))
-    f = getattr(L, fn)
-    vp, d = C.c_void_p, C.c_double
-    f.argtypes = [C.c_int, vp, vp, vp, d, vp, d, d, vp, d, d, d, d, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp,
-                  vp, vp, vp]
-    f.restype = C.c_int
-    return L, f
+    return run_solve(_lib().mplh_solve, a, b, c, d, e)
 
 
 def run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, potential=None, potential_weight=0.1,
@@ -648,13 +555,11 @@ def run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, potent
     def p(a):
         return None if a is None else a.ctypes.data
 
-    rc = fn(dim, grid.ctypes.data, mdim.ctypes.data, origin.ctypes.data, float(res), p(pot), float(potential_weight),
-            float(gradient_weight), p(reg), float(v_max), float(a_max), float(j_max), float(yaw_max), n_paths,
-            offset.ctypes.data, seg_t.ctypes.data, coeff.ctypes.data, ctl.ctypes.data, p(total_t), p(n_lambda), p(lam),
-            int(nthreads), status.ctypes.data, cost.ctypes.data, free.ctypes.data, valid.ctypes.data)
-    if rc != 0:
-        err = getattr(lib, "mplh_last_error", None)
-        raise RuntimeError(err().decode() if err else f"trajectory check failed rc={rc}")
+    _check(lib, fn(dim, grid.ctypes.data, mdim.ctypes.data, origin.ctypes.data, float(res), p(pot),
+                   float(potential_weight), float(gradient_weight), p(reg), float(v_max), float(a_max), float(j_max),
+                   float(yaw_max), n_paths, offset.ctypes.data, seg_t.ctypes.data, coeff.ctypes.data, ctl.ctypes.data,
+                   p(total_t), p(n_lambda), p(lam), int(nthreads), status.ctypes.data, cost.ctypes.data,
+                   free.ctypes.data, valid.ctypes.data))
     return dict(status=status[:n_paths], cost=cost[:n_paths], seg_free=free[:int(offset[-1])],
                 seg_valid=valid[:int(offset[-1])], offset=offset)
 
@@ -662,6 +567,5 @@ def run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, potent
 def traj_check(dim, grid, mdim, origin, res, paths, control, **kw):
     """env_map_host::traverse_trajectory, is_free and validate_primitive on the host (mpl_host.hpp) for a batch of
     trajectories, as mplx_traj_check computes them on the device.  Arguments as run_traj_check."""
-    lib = _traj_lib()
-    _, fn = load_traj_check_fn(LIB, "mplh_traj_check")
-    return run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, **kw)
+    lib = _lib()
+    return run_traj_check(lib.mplh_traj_check, lib, dim, grid, mdim, origin, res, paths, control, **kw)

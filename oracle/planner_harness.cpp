@@ -111,24 +111,25 @@ class env_map_oracle : public MPL::env_map_host<Dim> {
 };
 }  // namespace
 
+// the message of the last failed orcp_* call, under the host library's name so the same bindings read it
+static thread_local std::string g_err;
+extern "C" const char *mplh_last_error(void) { return g_err.c_str(); }
+
 extern "C" int orcp_lpa_run(const mplh_plan_args *a, const mplh_lpa_step *steps, int n_steps, mplh_lpa_out *outs,
                             int32_t *actions, int cap_actions) {
-  auto go = [&](auto dimtag) {
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     MPL::MapPlanner<Dim> planner(false);
     auto mu = mplh::make_map<Dim>(a);
     planner.setEnv(std::make_shared<env_map_oracle<Dim>>(mu, a), mu);
     mplh::run_lpa<Dim>(planner, mu, a, steps, n_steps, outs, actions, cap_actions);
-  };
-  if (a->dim == 2) go(std::integral_constant<int, 2>());
-  else go(std::integral_constant<int, 3>());
-  return 0;
+  });
 }
 
 extern "C" int orcp_plan(const mplh_plan_args *a, mplh_plan_result *r, uint64_t *closed_keys, int cap_closed,
                          int32_t *actions, int cap_actions) {
   *r = mplh_plan_result{};
-  auto go = [&](auto dimtag) {
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     MPL::MapPlanner<Dim> planner(false);
     auto env = std::make_shared<env_map_oracle<Dim>>(mplh::make_map<Dim>(a), a);
@@ -138,10 +139,7 @@ extern "C" int orcp_plan(const mplh_plan_args *a, mplh_plan_result *r, uint64_t 
       std::fprintf(stderr, "[orcp_plan] plan %.1f ms: get_succ (oracle) %.1f ms, host bookkeeping %.1f ms, %d expansions, %d closed + %d open states\n",
                    r->seconds * 1e3, env->seconds_in_get_succ * 1e3, (r->seconds - env->seconds_in_get_succ) * 1e3, r->expanded,
                    r->n_closed, r->n_open);
-  };
-  if (a->dim == 2) go(std::integral_constant<int, 2>());
-  else go(std::integral_constant<int, 3>());
-  return 0;
+  });
 }
 
 extern "C" int orcp_iterative_plan(const mplh_plan_args *a, const double *search_radius, int max_iter,
@@ -149,30 +147,24 @@ extern "C" int orcp_iterative_plan(const mplh_plan_args *a, const double *search
                                    int cap_closed, int32_t *actions, int cap_actions) {
   *first = mplh_plan_result{};
   *last = mplh_plan_result{};
-  auto go = [&](auto dimtag) {
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     MPL::MapPlanner<Dim> planner(false);
     auto mu = mplh::make_map<Dim>(a);
     planner.setEnv(std::make_shared<env_map_oracle<Dim>>(mu, a), mu);
     mplh::run_iterative<Dim>(planner, a, search_radius, max_iter, first, last, info, closed_keys, cap_closed, actions,
                              cap_actions);
-  };
-  if (a->dim == 2) go(std::integral_constant<int, 2>());
-  else go(std::integral_constant<int, 3>());
-  return 0;
+  });
 }
 
 extern "C" int orcp_plan_trajectory(const mplh_plan_args *a, int N, mplh_plan_result *r, double *samples, double *totals,
                                     double *waypoints, int cap_wp, int32_t *n_wp, double *mids) {
   *r = mplh_plan_result{};
-  auto go = [&](auto dimtag) {
+  return mplh::with_dim(a->dim, g_err, 2, [&](auto dimtag) {
     constexpr int Dim = decltype(dimtag)::value;
     MPL::MapPlanner<Dim> planner(false);
     auto mu = mplh::make_map<Dim>(a);
     planner.setEnv(std::make_shared<env_map_oracle<Dim>>(mu, a), mu);
     mplh::run_trajectory<Dim>(planner, a, N, r, samples, totals, waypoints, cap_wp, n_wp, mids);
-  };
-  if (a->dim == 2) go(std::integral_constant<int, 2>());
-  else go(std::integral_constant<int, 3>());
-  return 0;
+  });
 }

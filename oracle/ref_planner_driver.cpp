@@ -8,6 +8,7 @@
 #include <chrono>
 
 #include "../motion_primitive_library_b200/host/plan_capi_types.h"
+#include "../motion_primitive_library_b200/host/traj_rows.hpp"
 
 namespace {
 template <int Dim>
@@ -274,37 +275,12 @@ int trajectory(const mplh_plan_args *a, int N, mplh_plan_result *r, double *samp
   totals[2] = traj.Jyaw();
   totals[3] = (double)traj.segs.size();
   const auto cmds = traj.sample(N);
-  const int W = 4 * Dim + 3;
-  for (int i = 0; i <= N; i++) {
-    double *o = samples + (size_t)i * W;
-    for (int d = 0; d < Dim; d++) {
-      o[d] = cmds[i].pos(d);
-      o[Dim + d] = cmds[i].vel(d);
-      o[2 * Dim + d] = cmds[i].acc(d);
-      o[3 * Dim + d] = cmds[i].jrk(d);
-    }
-    o[4 * Dim] = cmds[i].yaw;
-    o[4 * Dim + 1] = cmds[i].yaw_dot;
-    o[4 * Dim + 2] = cmds[i].t;
-  }
-  const int V = 4 * Dim + 2;
+  for (int i = 0; i <= N; i++) mplh::put_command_row<Dim>(samples, i, cmds[i]);
   const auto ws = traj.getWaypoints();
   *n_wp = (int)ws.size();
-  for (int i = 0; i < (int)ws.size() + N + 1; i++) {
-    const bool wp = i < (int)ws.size();
-    if (wp && i >= cap_wp) continue;
-    const decimal_t dt = traj.getTotalTime() / N;
-    const Waypoint<Dim> w = wp ? ws[i] : traj.evaluate((i - (int)ws.size()) * dt);
-    double *o = wp ? waypoints + (size_t)i * V : mids + (size_t)(i - (int)ws.size()) * V;
-    for (int d = 0; d < Dim; d++) {
-      o[d] = w.pos(d);
-      o[Dim + d] = w.vel(d);
-      o[2 * Dim + d] = w.acc(d);
-      o[3 * Dim + d] = w.jrk(d);
-    }
-    o[4 * Dim] = w.yaw;
-    o[4 * Dim + 1] = w.t;
-  }
+  for (int i = 0; i < (int)ws.size() && i < cap_wp; i++) mplh::put_waypoint_row<Dim>(waypoints, i, ws[i]);
+  const decimal_t dt = traj.getTotalTime() / N;
+  for (int i = 0; i <= N; i++) mplh::put_waypoint_row<Dim>(mids, i, traj.evaluate(i * dt));
   return 0;
 }
 

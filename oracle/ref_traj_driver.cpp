@@ -7,6 +7,7 @@
 
 #include <stdexcept>
 
+#include "../motion_primitive_library_b200/host/traj_rows.hpp"
 #include "mplx.h"
 
 namespace {
@@ -49,21 +50,11 @@ void solve(int control, int yaw_control, const mplx_waypoint *wps, const uint8_t
       }
   if (samples) {
     const auto cmds = traj.sample(n_samples);
-    const int W = 4 * Dim + 3;
-    for (int i = 0; i <= n_samples; i++) {
-      double *o = samples + (size_t)i * W;
-      for (int d = 0; d < Dim; d++) { o[d] = cmds[i].pos(d); o[Dim + d] = cmds[i].vel(d); o[2 * Dim + d] = cmds[i].acc(d); o[3 * Dim + d] = cmds[i].jrk(d); }
-      o[4 * Dim] = cmds[i].yaw; o[4 * Dim + 1] = cmds[i].yaw_dot; o[4 * Dim + 2] = cmds[i].t;
-    }
+    for (int i = 0; i <= n_samples; i++) mplh::put_command_row<Dim>(samples, i, cmds[i]);
   }
   if (waypoints) {
-    const int V = 4 * Dim + 2;
     const auto ws = traj.getWaypoints();
-    for (size_t i = 0; i < ws.size(); i++) {
-      double *o = waypoints + i * V;
-      for (int d = 0; d < Dim; d++) { o[d] = ws[i].pos(d); o[Dim + d] = ws[i].vel(d); o[2 * Dim + d] = ws[i].acc(d); o[3 * Dim + d] = ws[i].jrk(d); }
-      o[4 * Dim] = ws[i].yaw; o[4 * Dim + 1] = ws[i].t;
-    }
+    for (size_t i = 0; i < ws.size(); i++) mplh::put_waypoint_row<Dim>(waypoints, i, ws[i]);
   }
 }
 }  // namespace

@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <string>
 
+#include "../motion_primitive_library_b200/host/traj_rows.hpp"
 #include "mplx.h"
 
 static thread_local std::string g_err;
@@ -88,12 +89,7 @@ void scale(int n_seg, const double *seg_t, const double *coeff, int control, int
     }
   if (samples) {
     const auto cmds = traj.sample(n_samples);
-    const int W = 4 * Dim + 3;
-    for (int i = 0; i <= n_samples; i++) {
-      double *o = samples + (size_t)i * W;
-      for (int d = 0; d < Dim; d++) { o[d] = cmds[i].pos(d); o[Dim + d] = cmds[i].vel(d); o[2 * Dim + d] = cmds[i].acc(d); o[3 * Dim + d] = cmds[i].jrk(d); }
-      o[4 * Dim] = cmds[i].yaw; o[4 * Dim + 1] = cmds[i].yaw_dot; o[4 * Dim + 2] = cmds[i].t;
-    }
+    for (int i = 0; i <= n_samples; i++) mplh::put_command_row<Dim>(samples, i, cmds[i]);
   }
   if (flags) {
     // 1 where Lambda::evaluate finds no segment with ti <= tau < tf for the row's tau (trajectory.h:100-110):

@@ -31,11 +31,11 @@ ref:
 	  else echo "reference sources not readable under $(REF_INC): oracle/_ref/$$1 not built"; fi; \
 	done
 
-_ref/libmplref_traj.so: ref_traj_driver.cpp ../include/mplx.h shim_traj/Eigen/Core
+_ref/libmplref_traj.so: ref_traj_driver.cpp ../include/mplx.h ../motion_primitive_library_b200/host/traj_rows.hpp shim_traj/Eigen/Core
 	mkdir -p _ref
 	$(CXX) $(REF_FLAGS) -o $@ ref_traj_driver.cpp $(REF_INC)/../src/mpl_traj_solver/poly_solver.cpp $(REF_INC)/../src/mpl_traj_solver/poly_traj.cpp
 
-_ref/libmplref_traj_scale.so: ref_traj_scale_driver.cpp ../include/mplx.h shim_traj/Eigen/Core
+_ref/libmplref_traj_scale.so: ref_traj_scale_driver.cpp ../include/mplx.h ../motion_primitive_library_b200/host/traj_rows.hpp shim_traj/Eigen/Core
 	mkdir -p _ref
 	$(CXX) $(REF_FLAGS) -o $@ ref_traj_scale_driver.cpp
 

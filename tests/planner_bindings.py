@@ -3,13 +3,13 @@ TEST-ONLY harness oracle/liboracle_planner.so (same host A*, CPU-oracle env)."""
 import subprocess
 from pathlib import Path
 
-from motion_primitive_library_b200.planner import (PlanArgs, PlanResult, QueryResult, Waypoint, load_fn,  # noqa: F401
-                                                   iterative_plan, load_iter_fn, load_lpa_fn, load_traj_fn, lpa_session,
-                                                   make_args, plan, plan_batch, plan_trajectory, run_iterative, run_lpa,
-                                                   run_plan, run_trajectory)
+from motion_primitive_library_b200.planner import (PlanArgs, PlanResult, QueryResult, Waypoint, bind,  # noqa: F401
+                                                   iterative_plan, lpa_session, make_args, plan, plan_batch,
+                                                   plan_trajectory, run_iterative, run_lpa, run_plan, run_trajectory)
 from reference_record import reference
 
 ROOT = Path(__file__).resolve().parent.parent
+ORACLE_PLANNER = ROOT / "oracle" / "liboracle_planner.so"
 
 
 def plan_gpu(args):
@@ -17,10 +17,9 @@ def plan_gpu(args):
 
 
 def plan_oracle(args):
-    p = ROOT / "oracle" / "liboracle_planner.so"
-    if not p.exists():
+    if not ORACLE_PLANNER.exists():
         subprocess.check_call(["make", "-C", str(ROOT / "oracle"), "liboracle_planner.so"], stdout=subprocess.DEVNULL)
-    lib, fn = load_fn(p, "orcp_plan")
+    lib, fn = bind(ORACLE_PLANNER, "orcp_plan", "mplh_plan")
     return run_plan(fn, lib, args)
 
 
@@ -29,8 +28,7 @@ REF_PLANNER = ROOT / "oracle" / "_ref" / "libmplref_planner.so"
 
 def lpa_oracle(args, script):
     """The product's host LPA* driven by the CPU-oracle env (TEST-ONLY harness)."""
-    p = ROOT / "oracle" / "liboracle_planner.so"
-    lib, fn = load_lpa_fn(p, "orcp_lpa_run")
+    lib, fn = bind(ORACLE_PLANNER, "orcp_lpa_run", "mplh_lpa_run")
     return run_lpa(fn, lib, args, script)
 
 
@@ -38,7 +36,7 @@ def lpa_reference(args, script):
     """The REFERENCE's LPA* (setLPAstar / plan / getLinkedNodes / updateBlockedNodes / updateClearedNodes /
     getSubStateSpace, unmodified sources + Eigen/Boost stand-ins) on the same script."""
     def live():
-        lib, fn = load_lpa_fn(REF_PLANNER, "refp_lpa_run")
+        lib, fn = bind(REF_PLANNER, "refp_lpa_run", "mplh_lpa_run")
         return run_lpa(fn, lib, args, script)
 
     return reference(REF_PLANNER, live)
@@ -46,28 +44,28 @@ def lpa_reference(args, script):
 
 def iterative_oracle(args, search_radius, max_iter=3):
     """The product's host plan() + iterativePlan() driven by the CPU-oracle env (TEST-ONLY harness)."""
-    lib, fn = load_iter_fn(ROOT / "oracle" / "liboracle_planner.so", "orcp_iterative_plan")
+    lib, fn = bind(ORACLE_PLANNER, "orcp_iterative_plan", "mplh_iterative_plan")
     return run_iterative(fn, lib, args, search_radius, max_iter)
 
 
 def iterative_reference(args, search_radius, max_iter=3):
     """The REFERENCE's plan() + MapPlanner::iterativePlan(start, goal, getTraj(), max_iter)."""
     def live():
-        lib, fn = load_iter_fn(REF_PLANNER, "refp_iterative_plan")
+        lib, fn = bind(REF_PLANNER, "refp_iterative_plan", "mplh_iterative_plan")
         return run_iterative(fn, lib, args, search_radius, max_iter)
 
     return reference(REF_PLANNER, live)
 
 
 def trajectory_oracle(args, n_samples=50):
-    lib, fn = load_traj_fn(ROOT / "oracle" / "liboracle_planner.so", "orcp_plan_trajectory")
+    lib, fn = bind(ORACLE_PLANNER, "orcp_plan_trajectory", "mplh_plan_trajectory")
     return run_trajectory(fn, lib, args, n_samples)
 
 
 def trajectory_reference(args, n_samples=50):
     """The REFERENCE's plan() + its own Trajectory::sample / getWaypoints / evaluate / J."""
     def live():
-        lib, fn = load_traj_fn(REF_PLANNER, "refp_plan_trajectory")
+        lib, fn = bind(REF_PLANNER, "refp_plan_trajectory", "mplh_plan_trajectory")
         return run_trajectory(fn, lib, args, n_samples)
 
     return reference(REF_PLANNER, live)
@@ -80,7 +78,7 @@ def ref_planner_available():
 def plan_reference(args):
     """The REFERENCE's MapPlanner<Dim>::plan() (unmodified sources + Eigen/Boost stand-ins)."""
     def live():
-        lib, fn = load_fn(REF_PLANNER, "refp_plan")
+        lib, fn = bind(REF_PLANNER, "refp_plan", "mplh_plan")
         return run_plan(fn, lib, args)
 
     return reference(REF_PLANNER, live)
@@ -136,9 +134,6 @@ def ref_b200_available():
 def plan_reference_b200(args):
     """The REFERENCE's MapPlanner<Dim>::plan() with integration/env_map_b200.h (libmplx behind the
     reference's virtual get_succ) installed through the virtual setMapUtil — the drop-in of INTEGRATION.md."""
-    import ctypes as C
-
-    lib, fn = load_fn(REF_B200, "refb_plan")
-    lib.refb_last_error.restype = C.c_char_p
+    lib, fn = bind(REF_B200, "refb_plan", "mplh_plan")
     lib.mplh_last_error = lib.refb_last_error
     return run_plan(fn, lib, args)

@@ -24,7 +24,7 @@ def plan_reference(args):
     A plan without a trajectory is recorded with cost +inf and no closed keys or actions: the reference leaves
     getTrajCost() unset then, and the driver exports the closed set only for a trajectory."""
     def live():
-        lib, fn = pb.load_iter_fn(pb.REF_PLANNER, "refp_iterative_plan")
+        lib, fn = pb.bind(pb.REF_PLANNER, "refp_iterative_plan", "mplh_iterative_plan")
         _, r = pb.run_iterative(fn, lib, args, (0.5,) * args.dim, max_iter=0)
         out = {k: r[k] for k in ("valid", "cost", "expanded", "n_closed", "closed", "actions")}
         if not out["valid"]:

@@ -17,7 +17,7 @@ def plan_reference(args):
     """pb.plan_reference, with the cost of a plan that found no trajectory recorded as +inf: the reference
     leaves getTrajCost() unset when the start is not free, so that value differs from run to run."""
     def live():
-        lib, fn = pb.load_fn(pb.REF_PLANNER, "refp_plan")
+        lib, fn = pb.bind(pb.REF_PLANNER, "refp_plan", "mplh_plan")
         r = pb.run_plan(fn, lib, args)
         if not r["valid"]:
             r["cost"] = float("inf")

@@ -4,7 +4,7 @@ built by oracle/traj.mk), with the same signature (mplh_traj_check in host/mpl_h
 import numpy as np
 
 from motion_primitive_library_b200 import planner as P
-from motion_primitive_library_b200.planner import load_traj_check_fn, run_traj_check, traj_check  # noqa: F401
+from motion_primitive_library_b200.planner import bind, run_traj_check, traj_check  # noqa: F401
 from reference_record import reference
 from traj_bindings import ROOT
 
@@ -15,7 +15,7 @@ VEL, ACC, JRK, YAW = 0x01, 0x03, 0x07, 0x10
 def check_reference(dim, grid, mdim, origin, res, paths, control, **kw):
     """The reference's checks on a batch of trajectories (arguments as planner.run_traj_check)."""
     def live():
-        lib, fn = load_traj_check_fn(REF_CHECK, "reft_traj_check")
+        lib, fn = bind(REF_CHECK, "reft_traj_check", "mplh_traj_check")
         r = run_traj_check(fn, lib, dim, grid, mdim, origin, res, paths, control, **kw)
         r.pop("offset")
         return r

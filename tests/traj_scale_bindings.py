@@ -4,8 +4,7 @@ planner.solve_roots) and the REFERENCE's own Trajectory::scale, scale_down steps
 mplh_solve in host/mpl_host_capi.cpp)."""
 import numpy as np
 
-from motion_primitive_library_b200.planner import (load_solve_fn, load_traj_scale_fn, run_solve, run_traj_scale,  # noqa: F401
-                                                   solve_roots, traj_scale)
+from motion_primitive_library_b200.planner import bind, run_solve, run_traj_scale, solve_roots, traj_scale  # noqa: F401
 from reference_record import reference
 from traj_bindings import ROOT
 
@@ -17,7 +16,7 @@ def scale_reference(dim, seg_t, coeff, mode, n_samples=50, max_bytes=256, **kw):
     On flagged rows the reference's lambda is indeterminate, so their vel, acc and jrk are recorded as 0.  Recorded
     arrays above max_bytes are kept as digests (None: keep them all)."""
     def live():
-        lib, fn = load_traj_scale_fn(REF_TRAJ, "reft_traj_scale", flags=True)
+        lib, fn = bind(REF_TRAJ, "reft_traj_scale")
         r = run_traj_scale(fn, lib, dim, seg_t, coeff, mode, n_samples=n_samples, flags=True, **kw)
         r["samples"][r["flags"] == 1, dim:4 * dim] = 0.0
         return r
@@ -28,7 +27,7 @@ def scale_reference(dim, seg_t, coeff, mode, n_samples=50, max_bytes=256, **kw):
 def solve_reference(a, b, c, d, e):
     """math.h's solve(a, b, c, d, e) in the reference."""
     def live():
-        _, fn = load_solve_fn(REF_TRAJ, "reft_solve")
+        _, fn = bind(REF_TRAJ, "reft_solve", "mplh_solve")
         return run_solve(fn, a, b, c, d, e)
 
     return reference(REF_TRAJ, live, max_bytes=None)
