@@ -362,6 +362,49 @@ int mplx_plan_batch_grow(mplx_ctx *ctx, int cost_terms, const mplx_waypoint *sta
 int mplx_plan_batch_grow_results(mplx_ctx *ctx, int64_t *action_offset, int32_t *actions, int64_t action_capacity,
                                  int64_t *closed_offset, uint64_t *closed_keys, int64_t closed_capacity);
 
+/* ---- the planned trajectories of the batched searches ------------------------------------------ */
+
+/* Record the trajectories of the following mplx_plan_batch / _cost_terms / _grow calls on this ctx (on = 1;
+ * 0 = off, the default).  pool_bytes > 0 sizes the trajectory room (a diagnostic); 0 = automatic, an eighth of
+ * the call's search budget.  With recording on, a finished query with a trajectory of n actions also copies the
+ * stored coordinates of its path's n + 1 states (recoverTraj's best_child_) into the room, which stays on the
+ * device; a query that finds the room full is searched again in a later round whose room holds all such queries
+ * (the kept buffer grows past the share only by what the trajectories themselves take), so
+ * mplx_plan_batch and mplx_plan_batch_cost_terms may then take more than one kernel launch.  The room comes off
+ * the budget, so fewer arenas may fit; no query's results depend on the room's size.  With recording off, every
+ * search call makes the launches it made without this call.  MPLX_ERR_ARG for on not 0 or 1 or pool_bytes < 0. */
+int mplx_set_batch_trajectories(mplx_ctx *ctx, int on, int64_t pool_bytes);
+
+/* Results of mplx_plan_batch_trajectories (HOST arrays), slots as mplx_traj_out's. */
+typedef struct {
+  int64_t *offset;       /* [n_q+1] query q owns waypoint slots [offset[q], offset[q+1]): n_actions+1 when its
+                            trajectory has at least one segment, else 0 (no trajectory, start already a goal,
+                            not searched)                                                                      */
+  mplx_waypoint *nodes;  /* [capacity] the stored coordinates of the path's states, start to goal (best_child_) */
+  double *seg_t;         /* [capacity] dt per segment (the ctx's T); the path's last slot 0                    */
+  double *coeff;         /* [capacity*(dim+1)*6] forward_action(nodes[j], U[action j], T) Primitive
+                            coefficients, mplx_traj_out's layout (highest order first, axes, then yaw; the
+                            yaw axis is 0 without a yaw control); the path's last slot 0                       */
+  double *samples;       /* NULL or [n_q*(n_samples+1)*(4*dim+3)] Trajectory::sample(n_samples) rows as
+                            mplx_traj_out's; zeros for a query without trajectory                              */
+  int64_t capacity;      /* in: waypoint slots the arrays hold                                                  */
+  int64_t total;         /* out: slots needed                                                                   */
+  double seconds;        /* out: device time of the kernels (CUDA events)                                       */
+} mplx_batch_traj_out;
+
+/* The trajectories of the last search call (mplx_plan_batch, mplx_plan_batch_cost_terms or mplx_plan_batch_grow)
+ * on this ctx, which must have run with recording on (mplx_set_batch_trajectories), for its n_q queries in query
+ * order.  Segment j of query q is Primitive(nodes[offset[q] + j], U[actions[j]], T) (env_base::forward_action)
+ * built from the coordinates the search stored for the path's states, as recoverTraj builds it; a replay of the
+ * action ids from the start can differ where a state's best predecessor is not the one that first created it.
+ * The coefficients are bit for bit the host's Primitive and the samples the host's Trajectory::sample.  The
+ * output feeds mplx_traj_check and mplx_traj_scale as it stands.  Capacity: when capacity < total the call fills
+ * offset and total and fails with MPLX_ERR_ARG.  Refusals, each with MPLX_ERR_ARG, the outputs untouched and no
+ * launch: no completed search call yet, the last one ran without recording, n_samples < 0, samples given with
+ * n_samples == 0, and a NULL out, offset, nodes, seg_t or coeff.  The kept coordinates stay until the next search
+ * call replaces them.  A constant number of launches per call.  Synchronous. */
+int mplx_plan_batch_trajectories(mplx_ctx *ctx, int n_samples, mplx_batch_traj_out *out);
+
 /* ---- trajectories through waypoints (TrajSolver) ----------------------------------------------- */
 
 /* Results of mplx_traj_solve (HOST arrays).  Path p owns the waypoint slots [offset[p], offset[p+1]); segment j

@@ -52,6 +52,8 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_cost_terms_fits",
     "mplx_plan_batch_grow",
     "mplx_plan_batch_grow_results",
+    "mplx_set_batch_trajectories",
+    "mplx_plan_batch_trajectories",
     "mplx_traj_solve",
     "mplx_traj_scale",
     "mplx_traj_check",
@@ -135,6 +137,21 @@ class GrowOut(C.Structure):
         ("last_cap", C.c_int64),
         ("arena_bytes", C.c_int64),
         ("reruns", C.c_int64),
+        ("seconds", C.c_double),
+    ]
+
+
+class BatchTrajOut(C.Structure):
+    """mplx_batch_traj_out"""
+
+    _fields_ = [
+        ("offset", C.c_void_p),
+        ("nodes", C.c_void_p),
+        ("seg_t", C.c_void_p),
+        ("coeff", C.c_void_p),
+        ("samples", C.c_void_p),
+        ("capacity", C.c_int64),
+        ("total", C.c_int64),
         ("seconds", C.c_double),
     ]
 
@@ -248,6 +265,10 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch_grow.restype = i32
     lib.mplx_plan_batch_grow_results.argtypes = [vp, vp, vp, i64, vp, vp, i64]
     lib.mplx_plan_batch_grow_results.restype = i32
+    lib.mplx_set_batch_trajectories.argtypes = [vp, i32, i64]
+    lib.mplx_set_batch_trajectories.restype = i32
+    lib.mplx_plan_batch_trajectories.argtypes = [vp, i32, C.POINTER(BatchTrajOut)]
+    lib.mplx_plan_batch_trajectories.restype = i32
     lib.mplx_traj_solve.argtypes = [vp, i32, vp, vp, vp, vp, f64, i32, i32, i32, C.POINTER(TrajOut)]
     lib.mplx_traj_solve.restype = i32
     lib.mplx_traj_scale.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(TrajScaleOut)]

@@ -194,9 +194,10 @@ struct UpdateBufs {
   }
 };
 
-// inputs, outputs and per-waypoint scratch of mplx_traj_solve, mplx_traj_scale and mplx_traj_check (mplx_traj.cu),
-// sized by the largest batch so far; the second line of members is mplx_traj_scale's and mplx_traj_check's, the
-// third mplx_traj_check's alone
+// inputs, outputs and per-waypoint scratch of mplx_traj_solve, mplx_traj_scale, mplx_traj_check and
+// mplx_plan_batch_trajectories (mplx_traj.cu), sized by the largest batch so far; the second line of members is
+// mplx_traj_scale's and mplx_traj_check's, the third mplx_traj_check's alone, the last
+// mplx_plan_batch_trajectories'
 struct TrajBufs {
   DevBuf<long long> offset;
   DevBuf<mplx_waypoint> wps;
@@ -208,7 +209,10 @@ struct TrajBufs {
   DevBuf<int32_t> n_pts;
   DevBuf<uint8_t> form, seg_free, seg_valid;
   DevBuf<double> cost;
+  DevBuf<long long> slot_src;  // mplx_plan_batch_trajectories' per-slot inputs
+  DevBuf<int32_t> slot_action;
   void release() {
+    slot_src.release(); slot_action.release();
     offset.release(); wps.release(); ctl.release(); mono.release(); status.release(); dts.release(); seg_t.release();
     taus.release(); coeff.release(); samples.release(); fac.release(); dpos.release(); dyaw.release();
     n_cand.release(); n_knot.release(); par.release(); total.release(); seg_T.release(); cand.release();
@@ -224,6 +228,7 @@ constexpr size_t kSearchArenaBudget = (size_t)8 << 30;
 // the device search (mplx_search.cu): per-slot arenas kept across calls; per-slot successor scratch
 // (succ, cost, key, action, count), the per-query arrays (queries, free_, ires, dres, offs) and the
 // result pool (closed), reused by every call and round
+enum TrajState : int { kTrajNone = 0, kTrajOff = 1, kTrajOn = 2 };
 struct SearchBufs {
   DevBuf<unsigned char> arena;
   int64_t layout_bytes = 0;  // bytes per slot of the layout the arena was cleared for
@@ -240,9 +245,27 @@ struct SearchBufs {
   std::vector<int64_t> grow_aoff, grow_coff;
   std::vector<int32_t> grow_actions;
   std::vector<uint64_t> grow_closed;
+  // trajectory recording (mplx_set_batch_trajectories): on, and the room asked for in bytes (0 = automatic)
+  bool traj_on = false;
+  int64_t traj_room_bytes = 0;
+  // the recorded coordinates of the last search call: the rooms of its rounds one after the other, the first
+  // traj_kept slots in use; toffs holds each query's place in the round's room, then the room's fill counter
+  DevBuf<mplx_waypoint> traj;
+  int64_t traj_kept = 0;
+  DevBuf<unsigned long long> toffs;
+  // what mplx_plan_batch_trajectories reads: kTrajNone before any search call (or after one that failed),
+  // kTrajOff after one without recording, kTrajOn after one with.  Query q owns the waypoint slots
+  // [traj_off[q], traj_off[q+1]); slot s holds the state traj[slot_src[s]] and the action id slot_action[s] of
+  // the segment that starts there (-1 on a path's last slot)
+  int traj_state = 0;
+  std::vector<int64_t> traj_off, slot_src;
+  std::vector<int32_t> slot_action;
   void release() {
     arena.release(); succ.release(); queries.release(); cost.release(); dres.release(); key.release();
     closed.release(); action.release(); count.release(); ires.release(); free_.release(); offs.release();
+    traj.release(); toffs.release();
+    traj_kept = 0;
+    traj_state = 0;
     layout_bytes = 0;
     cleared = 0;
     next_epoch = 1;

@@ -7,7 +7,10 @@
 //                successors in control order with their keys, and each thread runs the sample loop of
 //                its primitive (traverse_groups) for the edge cost;
 //   thread 0     relaxes the successors, tests the goal and the limits (mplx_search.cuh).
-// So there is no launch, no PCIe transfer and no host work per iteration.
+// So there is no launch, no PCIe transfer and no host work per iteration.  After the search, thread 0 traces
+// the trajectory back and, with trajectory recording on, copies the stored coordinates of the states on it
+// (SState::coord, which the slot's next query overwrites) to a device room kept for
+// mplx_plan_batch_trajectories.
 //
 // The occupancy search (no potential map, no yaw control) runs search_kernel<DIM, ORD, false, false>: the
 // sample loop never evaluates velocities.  The cost-term search serves every plan, including
@@ -23,7 +26,10 @@
 // worst-case arenas runs the kernel without the capacity check (CHECK false), which gives the same results
 // and spills less.
 // mplx_plan_batch_grow sizes arenas for the batch and searches overflowed queries again in larger arenas
-// (include/mplx.h states its round schedule).
+// (include/mplx.h states its round schedule).  With trajectory recording on, a finished query also reserves room
+// for its path's coordinates in the trajectory room, a share of the budget rather than the worst case; one that
+// finds it full is searched again in a later round whose room holds it, so mplx_plan_batch and
+// mplx_plan_batch_cost_terms may then take more than one round.
 #include <cuda_runtime.h>
 #include <string.h>
 
@@ -67,6 +73,13 @@ struct Job {
   uint64_t *pool;
   unsigned long long *pool_used, *offs;
   unsigned long long pool_cap;  // in uint64 units
+  // trajectory recording (mplx_set_batch_trajectories), traj == nullptr when off: a done query with n_actions > 0
+  // also reserves n_actions + 1 waypoint slots of traj with one atomicAdd on *traj_used and writes there the
+  // stored coordinates of the states its trace-back walked, start to goal; toffs[q] receives its first slot or,
+  // when the room is full (the query is then kPoolFull), the slots it needed
+  mplx_waypoint *traj;
+  unsigned long long *traj_used, *toffs;
+  unsigned long long traj_cap;  // in waypoint slots
 };
 enum GrowState : int32_t { kDone = 1, kOverflowed = 2, kPoolFull = 3 };
 
@@ -99,7 +112,9 @@ __device__ __forceinline__ uint64_t node_hash(const mplx_waypoint *w) {
 // kernel is the occupancy search, whose code does not carry the velocity coefficients.
 // CHECK: the arena's capacity is checked (consume<true>).  A launch whose arenas hold every query's worst
 // case (layout_for) runs without it, exactly as with it, and spills less in the sample loop.
-template <int DIM, int ORD, bool YAW, bool COST, bool CHECK>
+// REC: trajectory recording (J.traj); its own instantiation, so that a kernel without it compiles exactly as it
+// did before recording existed (a branch in the tail alone moves the sample loop's register allocation).
+template <int DIM, int ORD, bool YAW, bool COST, bool CHECK, bool REC>
 __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant__ EnvParams P, const __grid_constant__ Job J) {
   static_assert(COST || !YAW, "a yaw control always sums cost terms");
   __shared__ mplx_waypoint s_node;
@@ -186,18 +201,26 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
         J.state[q] = kOverflowed;
       } else {
         // the trace-back reads only states and predecessor records, so the dead heap (4*cap int32, more than
-        // the at most n_states + 1 actions) holds the trajectory until the pool has room for it
+        // the at most n_states + 1 <= cap + 1 actions) holds the trajectory until the pool has room for it; with
+        // recording, its first half the actions and its second half the chain of cap + 1 states
         int32_t *traj = reinterpret_cast<int32_t *>(A.hp);
+        int32_t *chain = REC ? traj + 2 * A.cap : nullptr;
         int na = 0;
-        const double c = finish(A, S, traj, 4 * A.cap, &na);
+        const double c = finish(A, S, traj, REC ? 2 * A.cap - 1 : 4 * A.cap, &na, chain);
         int nc = 0;
         if (S.status != kIdle && S.status != kTrivial)
           for (int s = 0; s < A.n_states; s++) nc += (A.st[s].flags & kClosed) ? 1 : 0;
         const unsigned long long nk = J.closed ? (unsigned long long)nc : 0ull;
         const unsigned long long units = nk + (unsigned long long)(na + 1) / 2;
         const unsigned long long off = atomicAdd(J.pool_used, units);
-        if (off + units > J.pool_cap) {
+        unsigned long long tunits = 0, toff = 0;
+        if constexpr (REC) {
+          tunits = na > 0 ? (unsigned long long)na + 1 : 0ull;
+          if (tunits) toff = atomicAdd(J.traj_used, tunits);
+        }
+        if (off + units > J.pool_cap || (REC && toff + tunits > J.traj_cap)) {
           J.offs[q] = units;  // the room its rerun's pool must have
+          if constexpr (REC) J.toffs[q] = tunits;
           J.state[q] = kPoolFull;
         } else {
           uint64_t *keys = J.pool + off;
@@ -208,6 +231,12 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
           }
           int32_t *acts = reinterpret_cast<int32_t *>(keys + nk);
           for (int i = 0; i < na; i++) acts[i] = traj[i];
+          if constexpr (REC) {
+            // thread 0 alone: a block-wide copy after a barrier measured slower at cfg5 (it raised the recording
+            // kernel's spills in the sample loop)
+            for (unsigned long long i = 0; i < tunits; i++) J.traj[toff + i] = A.st[chain[i]].coord;
+            J.toffs[q] = toff;
+          }
           J.cost[q] = c;
           J.valid[q] = isinf(c) ? 0 : 1;
           J.expanded[q] = S.expanded;
@@ -223,22 +252,26 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
 }
 
 // The instantiation a plan runs: <DIM, ORD, false, false> for the occupancy search, <DIM, ORD, yaw bit,
-// true> for the cost-term search, each with the capacity check or without.  f receives the kernel's address.
+// true> for the cost-term search, each with the capacity check or without and with trajectory recording or
+// without.  f receives the kernel's address.
 template <class F>
-cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, bool check, F &&f) {
-  return with_bool(check, [&](auto CHECK) {
-    return with_dim(P.dim, [&](auto DIM) {
-      return with_order(P.control, [&](auto ORD) {
-        if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, CHECK>);
-        return with_bool(P.control & 16, [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, CHECK>); });
+cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, bool check, bool rec, F &&f) {
+  return with_bool(rec, [&](auto REC) {
+    return with_bool(check, [&](auto CHECK) {
+      return with_dim(P.dim, [&](auto DIM) {
+        return with_order(P.control, [&](auto ORD) {
+          if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, CHECK, REC>);
+          return with_bool(P.control & 16,
+                           [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, CHECK, REC>); });
+        });
       });
     });
   });
 }
 
-int resident_ctas(const EnvParams &P, bool cost_terms, bool check, int block) {
+int resident_ctas(const EnvParams &P, bool cost_terms, bool check, bool rec, int block) {
   int per_sm = 0;
-  const cudaError_t e = with_search_kernel(P, cost_terms, check, [&](auto kernel) {
+  const cudaError_t e = with_search_kernel(P, cost_terms, check, rec, [&](auto kernel) {
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
   });
   if (e != cudaSuccess) {
@@ -266,9 +299,17 @@ constexpr size_t kQueryBytes =
 int search_budget(const SearchBufs &B, size_t &budget) {
   size_t free_b = 0, total_b = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
-  const size_t held = B.arena.cap + B.closed.cap * sizeof(uint64_t);
+  const size_t held = B.arena.cap + B.closed.cap * sizeof(uint64_t) + B.traj.cap * sizeof(mplx_waypoint);
   budget = std::min(kSearchArenaBudget, (free_b + held) / 4);
   return MPLX_OK;
+}
+
+// The trajectory room (waypoint slots) of a call with recording on, out of its budget: the size
+// mplx_set_batch_trajectories asked for, else an eighth of the budget; 0 with recording off.
+int64_t traj_room(const SearchBufs &B, size_t budget) {
+  if (!B.traj_on) return 0;
+  const size_t bytes = B.traj_room_bytes > 0 ? (size_t)B.traj_room_bytes : budget / 8;
+  return std::max<int64_t>(1, (int64_t)(bytes / sizeof(mplx_waypoint)));
 }
 
 // The result pool (uint64 units) of a call whose every query may take its worst case: max_expand closed keys
@@ -277,20 +318,22 @@ int64_t worst_pool_units(int n_q, int max_expand, bool with_closed) {
   return (int64_t)n_q * ((with_closed ? max_expand : 0) + (max_expand + 1) / 2);
 }
 
-// mplx_plan_batch*'s device memory: the per-query arrays, a result pool for every query's worst case and as
-// many worst-case arenas as fit next to them in the budget (search_budget).  MPLX_ERR_ALLOC, with nothing
-// changed, when not even one arena fits.
+// mplx_plan_batch*'s device memory: the per-query arrays, a result pool for every query's worst case, the
+// trajectory room with recording on (troom slots) and as many worst-case arenas as fit next to them in the budget
+// (search_budget).  MPLX_ERR_ALLOC, with nothing changed, when not even one arena fits.
 int size_batch(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, bool with_closed, Layout &L,
-               int64_t &slots) {
+               int64_t &slots, int64_t &troom) {
   const int nU = c->P.nU;
   L = layout_for(max_expand, nU);
   const int block = ((nU + 31) / 32) * 32;
   size_t budget = 0;
   const int rc = search_budget(c->sb, budget);
   if (rc) return rc;
-  const size_t results =
-      (size_t)n_q * kQueryBytes + (size_t)worst_pool_units(n_q, max_expand, with_closed) * sizeof(uint64_t);
-  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, block));
+  troom = traj_room(c->sb, budget);
+  const size_t results = (size_t)n_q * kQueryBytes +
+                         (size_t)worst_pool_units(n_q, max_expand, with_closed) * sizeof(uint64_t) +
+                         (size_t)troom * sizeof(mplx_waypoint);
+  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, c->sb.traj_on, block));
   const size_t left = results < budget ? budget - results : 0;
   slots = std::min<int64_t>(slots, (int64_t)(left / (size_t)L.bytes));
   if (slots < 1)
@@ -351,6 +394,7 @@ int upload(mplx_ctx *c, const mplx_waypoint *starts, const mplx_waypoint *goals,
   CU(B.ires.reserve(6 * (size_t)n_q));
   CU(B.dres.reserve((size_t)n_q));
   CU(B.offs.reserve((size_t)n_q + 1));
+  if (B.traj_on) CU(B.toffs.reserve((size_t)n_q + 1));
   CU(cudaMemcpyAsync(B.queries.p, starts, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
   CU(cudaMemcpyAsync(B.queries.p + n_q, goals, sizeof(mplx_waypoint) * n_q, cudaMemcpyHostToDevice, c->stream));
   if (start_free) CU(cudaMemcpyAsync(B.free_.p, start_free, n_q, cudaMemcpyHostToDevice, c->stream));
@@ -364,14 +408,44 @@ struct Round {
   std::vector<double> cost;
   std::vector<unsigned long long> offs;  // kDone: the query's place in pool; kPoolFull: the units it needed
   std::vector<uint64_t> pool;            // the result pool, drained
+  std::vector<unsigned long long> toffs;  // with recording: kDone: the query's place in the room (from tbase);
+                                          // kPoolFull: the slots it needed
+  int64_t tbase = 0;                      // with recording: the room's first slot in SearchBufs::traj
   double seconds = 0;  // device time of the round's launch
   int32_t at(RoundField f, int q) const { return ires[(size_t)f * cost.size() + q]; }
 };
 
+// The trajectory room of a call's next round: what is left of the call's share (troom slots) after the slots the
+// earlier rounds kept or, when the queries that found the room full (again_t slots between them) need more, exactly
+// that, so the kept buffer never holds more than the share or what the call's trajectories themselves take.
+int64_t next_room(const SearchBufs &B, int64_t troom, int64_t again_t) {
+  return std::max<int64_t>(1, std::max(troom - B.traj_kept, again_t));
+}
+
+// Makes room for troom more recorded waypoints after the traj_kept ones the call has recorded so far.
+int reserve_traj(mplx_ctx *c, int64_t troom) {
+  SearchBufs &B = c->sb;
+  const size_t need = (size_t)(B.traj_kept + troom);
+  if (B.traj.cap >= need) return MPLX_OK;
+  DevBuf<mplx_waypoint> nb;
+  CU(nb.reserve(need));
+  if (B.traj_kept > 0) {
+    const cudaError_t e = cudaMemcpyAsync(nb.p, B.traj.p, sizeof(mplx_waypoint) * (size_t)B.traj_kept,
+                                          cudaMemcpyDeviceToDevice, c->stream);
+    if (e != cudaSuccess) nb.release();
+    CU(e);
+  }
+  B.traj.release();  // cudaFree waits for the copy
+  B.traj = nb;
+  return MPLX_OK;
+}
+
 // One launch over the queries `qlist` in `slots` arenas of layout L with a result pool of pool_units
-// uint64: reserves the per-slot scratch and the pool, launches, and copies the results and the pool back.
+// uint64 and, troom > 0, a trajectory room of troom waypoint slots after the ones the call has kept: reserves the
+// per-slot scratch, the pool and the room, launches, and copies the results and the pool back.  The room's
+// contents stay on the device (SearchBufs::traj).
 int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, const Layout &L, int64_t slots,
-              int64_t pool_units, Round &R) {
+              int64_t pool_units, int64_t troom, Round &R) {
   SearchBufs &B = c->sb;
   const int nU = c->P.nU;
   const int n_q = b.n_q;
@@ -388,6 +462,11 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   CU(cudaMemcpyAsync(ql, qlist.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
   CU(cudaMemsetAsync(B.count.p + slots, 0, sizeof(int32_t), c->stream));
   CU(cudaMemsetAsync(B.offs.p + n_q, 0, sizeof(unsigned long long), c->stream));
+  if (troom > 0) {
+    rc = reserve_traj(c, troom);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(B.toffs.p + n_q, 0, sizeof(unsigned long long), c->stream));
+  }
 
   Job J{};
   J.starts = B.queries.p;
@@ -421,6 +500,10 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   J.pool_used = B.offs.p + n_q;
   J.offs = B.offs.p;
   J.pool_cap = (unsigned long long)pool_units;
+  J.traj = troom > 0 ? B.traj.p + B.traj_kept : nullptr;
+  J.traj_used = troom > 0 ? B.toffs.p + n_q : nullptr;
+  J.toffs = troom > 0 ? B.toffs.p : nullptr;
+  J.traj_cap = troom > 0 ? (unsigned long long)troom : 0ull;
   B.next_epoch += (uint32_t)n;
 
   EnvParams P = c->P;
@@ -430,7 +513,7 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   const bool check = b.max_expand <= 0 || L.cap < 1 + (int64_t)b.max_expand * nU;
   TimedRun timed;
   const cudaError_t le = timed.run(c->stream, c->launches, [&](int *launches) {
-    return with_search_kernel(P, b.cost_terms, check, [&](auto kernel) {
+    return with_search_kernel(P, b.cost_terms, check, troom > 0, [&](auto kernel) {
       kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
       const cudaError_t e = cudaGetLastError();
       if (e == cudaSuccess) *launches += 1;
@@ -444,18 +527,64 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   R.ires.resize(5 * (size_t)n_q);
   R.cost.resize(n_q);
   R.offs.resize(n_q);
-  unsigned long long used = 0;
+  unsigned long long used = 0, tused = 0;
+  if (troom > 0) {
+    R.toffs.resize(n_q);
+    CU(cudaMemcpyAsync(R.toffs.data(), B.toffs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost,
+                       c->stream));
+    CU(cudaMemcpyAsync(&tused, B.toffs.p + n_q, sizeof tused, cudaMemcpyDeviceToHost, c->stream));
+  }
   CU(cudaMemcpyAsync(R.ires.data(), B.ires.p, sizeof(int32_t) * R.ires.size(), cudaMemcpyDeviceToHost, c->stream));
   CU(cudaMemcpyAsync(R.cost.data(), B.dres.p, sizeof(double) * n_q, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaMemcpyAsync(R.offs.data(), B.offs.p, sizeof(unsigned long long) * n_q, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaMemcpyAsync(&used, B.offs.p + n_q, sizeof used, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   CU(timed.seconds(&R.seconds));
+  // the room's used part stays; the next round's room follows it
+  R.tbase = B.traj_kept;
+  if (troom > 0) B.traj_kept += (int64_t)std::min<unsigned long long>(tused, (unsigned long long)troom);
   // the pool is drained before the next round reuses it
   R.pool.resize((size_t)std::min<unsigned long long>(used, (unsigned long long)pool_units));
   if (!R.pool.empty())
     CU(cudaMemcpy(R.pool.data(), B.closed.p, sizeof(uint64_t) * R.pool.size(), cudaMemcpyDeviceToHost));
   return MPLX_OK;
+}
+
+// A search call that passed its refusals starts: what an earlier call recorded is dropped, and with recording
+// off so is the room.
+void traj_begin(SearchBufs &B) {
+  B.traj_state = kTrajNone;
+  B.traj_kept = 0;
+  B.traj_off.clear();
+  B.slot_src.clear();
+  B.slot_action.clear();
+  if (!B.traj_on) {
+    B.traj.release();
+    B.toffs.release();
+  }
+}
+
+// The call's recorded trajectories for mplx_plan_batch_trajectories: query q has n_actions(q) action ids at
+// actions(q) and, when it has at least one, the states of its path at traj[src[q] ...].
+template <class NA, class ACT>
+void traj_publish(SearchBufs &B, int n_q, const std::vector<int64_t> &src, NA n_actions, ACT actions) {
+  if (!B.traj_on) {
+    B.traj_state = kTrajOff;
+    return;
+  }
+  B.traj_off.assign((size_t)n_q + 1, 0);
+  for (int q = 0; q < n_q; q++) {
+    const int na = n_actions(q);
+    if (na > 0) {
+      const int32_t *a = actions(q);
+      for (int j = 0; j <= na; j++) {
+        B.slot_src.push_back(src[q] + j);
+        B.slot_action.push_back(j < na ? a[j] : -1);
+      }
+    }
+    B.traj_off[q + 1] = (int64_t)B.slot_src.size();
+  }
+  B.traj_state = kTrajOn;
 }
 
 int plan_batch_fits(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, int with_closed,
@@ -466,8 +595,8 @@ int plan_batch_fits(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int m
   rc = mplx_bind(c);
   if (rc) return rc;
   Layout L;
-  int64_t s = 0;
-  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed != 0, L, s);
+  int64_t s = 0, troom = 0;
+  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed != 0, L, s, troom);
   if (rc) return rc;
   if (slots) *slots = (int32_t)s;
   if (arena_bytes) *arena_bytes = L.bytes;
@@ -491,29 +620,59 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
   if (rc) return rc;
   const bool with_closed = out->closed_keys != nullptr;
   Layout L;
-  int64_t slots = 0;
-  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed, L, slots);
+  int64_t slots = 0, troom = 0;
+  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed, L, slots, troom);
   if (rc) return rc;
+  SearchBufs &B = c->sb;
+  traj_begin(B);
   out->slots = 0;
   out->arena_bytes = 0;
   out->seconds = 0;
   out->action_offset[0] = 0;
   if (out->closed_offset) out->closed_offset[0] = 0;
-  if (n_q == 0) return MPLX_OK;
+  std::vector<int64_t> tsrc(n_q, 0);
+  if (n_q == 0) {
+    traj_publish(B, 0, tsrc, [](int) { return 0; }, [](int) { return (const int32_t *)nullptr; });
+    return MPLX_OK;
+  }
 
   rc = upload(c, starts, goals, start_free, n_q);
   if (rc) return rc;
   const Batch b{n_q, max_expand, cost_terms, with_closed, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
-  std::vector<int32_t> all(n_q);
-  std::iota(all.begin(), all.end(), 0);
-  Round R;
-  rc = run_round(c, b, all, L, slots, worst_pool_units(n_q, max_expand, with_closed), R);
-  if (rc) return rc;
+  std::vector<int32_t> cur(n_q);
+  std::iota(cur.begin(), cur.end(), 0);
+  // worst-case arenas and pool: no query can overflow or find the pool full, so one round serves every query
+  // unless the trajectory room is full; those queries run again, in a room that holds them all
+  std::vector<Round> rounds(1);
+  std::vector<int32_t> round_of(n_q, 0);
+  int64_t again_t = 0;
+  double seconds = 0;
+  for (;;) {
+    Round &R = rounds.back();
+    rc = run_round(c, b, cur, L, slots, worst_pool_units(n_q, max_expand, with_closed), troom > 0 ? next_room(B, troom, again_t) : 0, R);
+    if (rc) return rc;
+    seconds += R.seconds;
+    std::vector<int32_t> again;
+    again_t = 0;
+    for (const int32_t q : cur) {
+      const int32_t st = R.at(kState, q);
+      if (st == kDone) {
+        round_of[q] = (int32_t)rounds.size() - 1;
+        if (troom > 0) tsrc[q] = R.tbase + (int64_t)R.toffs[q];
+      } else if (troom > 0 && st == kPoolFull) {
+        again.push_back(q);
+        again_t += (int64_t)R.toffs[q];
+      } else {
+        return fail(MPLX_ERR_CUDA, "%s: query %d did not fit its worst-case arena and result pool", fn, q);
+      }
+    }
+    if (again.empty()) break;
+    cur.swap(again);
+    rounds.emplace_back();
+  }
   int64_t ao = 0, co = 0;
   for (int q = 0; q < n_q; q++) {
-    // worst-case arenas and pool: no query can overflow or find the pool full
-    if (R.at(kState, q) != kDone)
-      return fail(MPLX_ERR_CUDA, "%s: query %d did not fit its worst-case arena and result pool", fn, q);
+    const Round &R = rounds[round_of[q]];
     out->valid[q] = R.at(kValid, q);
     out->cost[q] = R.cost[q];
     out->expanded[q] = R.at(kExpanded, q);
@@ -536,9 +695,11 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
       out->closed_offset[q + 1] = co;
     }
   }
+  traj_publish(B, n_q, tsrc, [&](int q) { return rounds[round_of[q]].at(kNActions, q); },
+               [&](int q) { return out->actions + out->action_offset[q]; });
   out->slots = (int32_t)slots;
   out->arena_bytes = L.bytes;
-  out->seconds = R.seconds;
+  out->seconds = seconds;
   return MPLX_OK;
 }
 
@@ -578,15 +739,16 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
   const int block = ((nU + 31) / 32) * 32;
   const bool ct = cost_terms != 0;
 
-  // the per-query arrays and the pool's automatic size come off the budget first
+  // the per-query arrays, the trajectory room and the pool's automatic size come off the budget first
   size_t budget = 0;
   rc = search_budget(c->sb, budget);
   if (rc) return rc;
   SearchBufs &B = c->sb;
-  const size_t results = (size_t)n_q * kQueryBytes;
+  const int64_t troom = traj_room(B, budget);
+  const size_t results = (size_t)n_q * kQueryBytes + (size_t)troom * sizeof(mplx_waypoint);
   const size_t pool_auto = budget / 8;
   const size_t avail = results + pool_auto < budget ? budget - results - pool_auto : 0;
-  const int64_t resident = resident_ctas(c->P, ct, true, block);
+  const int64_t resident = resident_ctas(c->P, ct, true, B.traj_on, block);
   int64_t cap_max = cap_fitting(1, avail);
   if (cap_max < 1)
     return fail(MPLX_ERR_ALLOC, "%s: one search arena and the results (%lld bytes) exceed the budget of %lld bytes",
@@ -598,6 +760,7 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
   const int64_t pool_units =
       std::max<int64_t>(1, pool_bytes > 0 ? pool_bytes / (int64_t)sizeof(uint64_t) : (int64_t)(pool_auto / 8));
 
+  traj_begin(B);
   memset(out->valid, 0, sizeof(int32_t) * n_q);
   memset(out->expanded, 0, sizeof(int32_t) * n_q);
   memset(out->n_closed, 0, sizeof(int32_t) * n_q);
@@ -613,7 +776,9 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
   out->seconds = 0;
   std::vector<std::vector<int32_t>> acts(n_q);
   std::vector<std::vector<uint64_t>> keys(n_q);
+  std::vector<int64_t> tsrc(n_q, 0);
   auto publish = [&]() {
+    traj_publish(B, n_q, tsrc, [&](int q) { return (int)acts[q].size(); }, [&](int q) { return acts[q].data(); });
     B.grow_aoff.assign((size_t)n_q + 1, 0);
     B.grow_coff.assign((size_t)n_q + 1, 0);
     B.grow_actions.clear();
@@ -641,13 +806,14 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
   int32_t rounds = 0;
   int64_t reruns = 0;
   int64_t again_units = 0;  // the most pool units a query of this round's list found no room for
+  int64_t again_t = 0;      // the trajectory slots the queries of this round's list found no room for
   for (;;) {
     const Layout L = layout_cap(cap);
     const int64_t n = (int64_t)cur.size();
     const int64_t slots = std::max<int64_t>(1, std::min({n, resident, (int64_t)(avail / (size_t)L.bytes)}));
     // a pool that holds the largest query that found it full: the first of them to reserve fits, so every
     // round completes at least one query
-    rc = run_round(c, b, cur, L, slots, std::max(pool_units, again_units), R);
+    rc = run_round(c, b, cur, L, slots, std::max(pool_units, again_units), troom > 0 ? next_room(B, troom, again_t) : 0, R);
     if (rc) return rc;
     seconds += R.seconds;
     if (rounds == 0) {
@@ -659,6 +825,7 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
 
     std::vector<int32_t> again;  // the result pool was full: the same capacity again
     again_units = 0;
+    again_t = 0;
     for (const int32_t q : cur) {
       const int32_t st = R.at(kState, q);
       if (st == kDone) {
@@ -673,9 +840,11 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
         keys[q].assign(k, k + nk);
         const int32_t *a = reinterpret_cast<const int32_t *>(k + nk);
         acts[q].assign(a, a + out->n_actions[q]);
+        if (troom > 0) tsrc[q] = R.tbase + (int64_t)R.toffs[q];
       } else if (st == kPoolFull) {
         again.push_back(q);
         again_units = std::max(again_units, (int64_t)R.offs[q]);
+        if (troom > 0) again_t += (int64_t)R.toffs[q];
       } else if (cap < cap_max) {
         next.push_back(q);
       }  // overflowed at the largest capacity: searched stays 0
@@ -754,5 +923,15 @@ extern "C" int mplx_plan_batch_grow_results(mplx_ctx *c, int64_t *action_offset,
     memcpy(closed_offset, B.grow_coff.data(), sizeof(int64_t) * B.grow_coff.size());
     if (!B.grow_closed.empty()) memcpy(closed_keys, B.grow_closed.data(), sizeof(uint64_t) * B.grow_closed.size());
   }
+  return MPLX_OK;
+}
+
+extern "C" int mplx_set_batch_trajectories(mplx_ctx *c, int on, int64_t pool_bytes) {
+  const char *fn = "mplx_set_batch_trajectories";
+  if (!c) return fail(MPLX_ERR_ARG, "%s: null ctx", fn);
+  if (on != 0 && on != 1) return fail(MPLX_ERR_ARG, "%s: on must be 0 or 1", fn);
+  if (pool_bytes < 0) return fail(MPLX_ERR_ARG, "%s: pool_bytes must be >= 0", fn);
+  c->sb.traj_on = on != 0;
+  c->sb.traj_room_bytes = pool_bytes;
   return MPLX_OK;
 }

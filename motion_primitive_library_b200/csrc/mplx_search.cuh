@@ -5,7 +5,7 @@
 // (host/mpl_host.hpp) step by step, so a query gives what AstarStepper gives:
 //   PriorityQueue      mpl_host.hpp:1050-1102  (the same swaps and heap_idx updates)
 //   AstarStepper       mpl_host.hpp:1449-1518  (start / pop / consume / finish)
-//   recoverTraj        mpl_host.hpp:1392-1433
+//   recoverTraj        mpl_host.hpp:1392-1433 (with its best_child_ chain)
 //   env_map_host       mpl_host.hpp:572-587    (is_goal with the walkRay test, is_free)
 //   env_base           mpl_host.hpp:460-474    (get_heur / cal_heur)
 // Plain IEEE operations only (the library builds with -fmad=false; the CPU test with
@@ -371,14 +371,18 @@ MPLX_HD void consume(Arena &A, Query &S, const Grid &G, const Goal &Q, int n, Ke
 
 // AstarStepper::finish + recoverTraj (mpl_host.hpp:1392-1433, 1511-1518).  Writes the action ids
 // from start to goal into actions[0, *n_actions) (at most cap; more sets *n_actions = -1) and
-// returns the cost (+inf when no trajectory).
-MPLX_HD double finish(const Arena &A, const Query &S, int32_t *actions, int cap, int *n_actions) {
+// returns the cost (+inf when no trajectory).  chain, when given, has room for cap + 1 state indices and
+// receives the states the trace-back walked, recoverTraj's best_child_ from start to goal: *n_actions + 1
+// of them when a trajectory is found (its contents are undefined otherwise).
+MPLX_HD double finish(const Arena &A, const Query &S, int32_t *actions, int cap, int *n_actions,
+                      int32_t *chain = nullptr) {
   *n_actions = 0;
   if (S.status == kTrivial) return 0;
   if (S.status != kGoal) return INFINITY;
   int curr = S.cur;
   int n = 0;
   bool found = false;
+  if (chain) chain[0] = curr;
   for (int guard = 0; guard <= A.n_states && A.st[curr].pred_head >= 0; guard++) {
     int min_id = -1, min_node = -1;
     double min_rhs = INFINITY, min_g = INFINITY;
@@ -402,6 +406,7 @@ MPLX_HD double finish(const Arena &A, const Query &S, int32_t *actions, int cap,
     if (n < cap) actions[n] = A.pr[min_id].action;
     n++;
     curr = min_node;
+    if (chain && n <= cap) chain[n] = curr;
     if (A.st[curr].key == S.start_key) {
       found = true;
       break;
@@ -417,6 +422,12 @@ MPLX_HD double finish(const Arena &A, const Query &S, int32_t *actions, int cap,
     actions[i] = actions[j];
     actions[j] = t;
   }
+  if (chain)
+    for (int i = 0, j = n; i < j; i++, j--) {
+      const int32_t t = chain[i];
+      chain[i] = chain[j];
+      chain[j] = t;
+    }
   *n_actions = n;
   return A.st[S.cur].g;
 }

@@ -11,6 +11,8 @@
 //   traj_coeff_kernel   one thread per segment: Primitive1D coefficients from the end-point derivatives
 //   traj_sample_kernel  one thread per sample: Trajectory::sample(N) of those coefficients, in the host's
 //                       operand order (include/mpl_basis/trajectory.h:100-137, primitive.h:128-145)
+#include <string.h>
+
 #include <algorithm>
 
 #include "mplx_dispatch.h"
@@ -609,6 +611,143 @@ extern "C" int mplx_traj_solve(mplx_ctx *c, int n_paths, const int64_t *offset, 
     CU(cudaMemcpyAsync(out->coeff, B.coeff.p, sizeof(double) * n_wp * (dim + 1) * 6, cudaMemcpyDeviceToHost, st));
   }
   if (out->samples) CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(timed.seconds(&out->seconds));
+  return MPLX_OK;
+}
+
+// ---- the planned trajectories of the batched searches (mplx_plan_batch_trajectories, include/mplx.h) ---------
+//   ptraj_seg_kernel    one thread per waypoint slot: the state the search stored, and the coefficients of
+//                       Primitive(state, U[action], T) (primitive.h:220-256), arithmetic-free copies
+//   ptraj_path_kernel   one thread per query: the running sum of segment times, as traj_sweep_kernel adds them
+//   traj_sample_kernel  as for mplx_traj_solve
+namespace mplx {
+namespace {
+
+struct PtrajArgs {
+  long long n_slots;
+  const mplx_waypoint *kept;  // the search's recorded states (SearchBufs::traj)
+  const long long *src;       // per slot: its state in kept
+  const int32_t *action;      // per slot: the action of the segment starting there, -1 on a path's last slot
+  const double *U;
+  int udim, control;
+  double T;
+  mplx_waypoint *nodes;
+  double *seg_t, *coeff;
+};
+
+template <int DIM>
+__global__ void __launch_bounds__(128) ptraj_seg_kernel(PtrajArgs A) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < A.n_slots;
+       s += (long long)gridDim.x * blockDim.x) {
+    const mplx_waypoint w = A.kept[A.src[s]];
+    A.nodes[s] = w;
+    double c[(DIM + 1) * 6];
+#pragma unroll
+    for (int k = 0; k < (DIM + 1) * 6; k++) c[k] = 0.0;
+    const int a = A.action[s];
+    if (a >= 0) {
+      const double *u = A.U + (size_t)a * A.udim;
+      const int o = A.control & 15;
+#pragma unroll
+      for (int i = 0; i < DIM; i++) {
+        double *ci = c + i * 6;
+        if (o == MPLX_SNP) { ci[1] = u[i]; ci[2] = w.jrk[i]; ci[3] = w.acc[i]; ci[4] = w.vel[i]; ci[5] = w.pos[i]; }
+        else if (o == MPLX_JRK) { ci[2] = u[i]; ci[3] = w.acc[i]; ci[4] = w.vel[i]; ci[5] = w.pos[i]; }
+        else if (o == MPLX_ACC) { ci[3] = u[i]; ci[4] = w.vel[i]; ci[5] = w.pos[i]; }
+        else if (o == MPLX_VEL) { ci[4] = u[i]; ci[5] = w.pos[i]; }
+      }
+      if (A.control & 16) {
+        c[DIM * 6 + 4] = u[DIM];
+        c[DIM * 6 + 5] = w.yaw;
+      }
+    }
+    A.seg_t[s] = a >= 0 ? A.T : 0.0;
+    double *o = A.coeff + s * (DIM + 1) * 6;
+#pragma unroll
+    for (int k = 0; k < (DIM + 1) * 6; k++) o[k] = c[k];
+  }
+}
+
+__global__ void __launch_bounds__(128) ptraj_path_kernel(TrajArgs A) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n_paths) return;
+  const long long b = A.offset[p];
+  const int W = (int)(A.offset[p + 1] - b);
+  bool mono = true;
+  if (W > 0) A.taus[b] = 0.0;
+  for (int j = 0; j + 1 < W; j++) {
+    A.taus[b + j + 1] = A.seg_t[b + j] + A.taus[b + j];
+    mono = mono && A.taus[b + j + 1] >= A.taus[b + j];
+  }
+  A.status[p] = W >= 2 ? 1 : 0;
+  A.mono[p] = mono ? 1 : 0;
+}
+
+}  // namespace
+}  // namespace mplx
+
+extern "C" int mplx_plan_batch_trajectories(mplx_ctx *c, int n_samples, mplx_batch_traj_out *out) {
+  const char *fn = "mplx_plan_batch_trajectories";
+  if (!c) return fail(MPLX_ERR_ARG, "%s: null ctx", fn);
+  const SearchBufs &S = c->sb;
+  if (S.traj_state == kTrajNone) return fail(MPLX_ERR_ARG, "%s: no completed search call on this ctx", fn);
+  if (S.traj_state == kTrajOff)
+    return fail(MPLX_ERR_ARG, "%s: the last search call ran without recording (mplx_set_batch_trajectories)", fn);
+  if (n_samples < 0) return fail(MPLX_ERR_ARG, "%s: n_samples < 0", fn);
+  if (!out || !out->offset || !out->nodes || !out->seg_t || !out->coeff)
+    return fail(MPLX_ERR_ARG, "%s: missing array", fn);
+  if (out->samples && n_samples == 0) return fail(MPLX_ERR_ARG, "%s: samples with n_samples == 0", fn);
+  const int n_q = (int)S.traj_off.size() - 1;
+  const long long total = S.traj_off.back();
+  if (out->samples && (long long)n_q * (n_samples + 1) >= ((long long)1 << 40))
+    return fail(MPLX_ERR_ARG, "%s: too many samples", fn);
+  if (out->capacity < total) {
+    memcpy(out->offset, S.traj_off.data(), sizeof(int64_t) * S.traj_off.size());
+    out->total = total;
+    return fail(MPLX_ERR_ARG, "%s: capacity %lld below the %lld waypoint slots needed", fn, (long long)out->capacity,
+                total);
+  }
+  if (int r = mplx_bind(c)) return r;
+  memcpy(out->offset, S.traj_off.data(), sizeof(int64_t) * S.traj_off.size());
+  out->total = total;
+  out->seconds = 0.0;
+  if (n_q == 0) return MPLX_OK;
+  const int dim = c->dim;
+  TrajBufs &B = c->tb;
+  const size_t nw = (size_t)std::max<long long>(total, 1);
+  CU(B.offset.reserve(n_q + 1)); CU(B.status.reserve(n_q)); CU(B.mono.reserve(n_q));
+  CU(B.wps.reserve(nw)); CU(B.seg_t.reserve(nw)); CU(B.taus.reserve(nw)); CU(B.coeff.reserve(nw * (dim + 1) * 6));
+  CU(B.slot_src.reserve(nw)); CU(B.slot_action.reserve(nw));
+  const size_t n_rows = out->samples ? (size_t)n_q * (n_samples + 1) : 0;
+  if (out->samples) CU(B.samples.reserve(n_rows * (4 * dim + 3)));
+  cudaStream_t st = c->stream;
+  CU(cudaMemcpyAsync(B.offset.p, S.traj_off.data(), sizeof(int64_t) * (n_q + 1), cudaMemcpyHostToDevice, st));
+  if (total > 0) {
+    CU(cudaMemcpyAsync(B.slot_src.p, S.slot_src.data(), sizeof(int64_t) * total, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.slot_action.p, S.slot_action.data(), sizeof(int32_t) * total, cudaMemcpyHostToDevice, st));
+  }
+  const mplx::PtrajArgs PA{total, S.traj.p, B.slot_src.p, B.slot_action.p, c->U.p, c->P.udim, c->P.control, c->P.T,
+                           B.wps.p, B.seg_t.p, B.coeff.p};
+  mplx::TrajArgs A{n_q, B.offset.p, B.wps.p, nullptr, nullptr, 0.0, c->P.control, 0, n_samples, B.status.p, B.mono.p,
+                   B.seg_t.p, B.taus.p, B.coeff.p, out->samples ? B.samples.p : nullptr, nullptr, nullptr, nullptr};
+  TimedRun timed;
+  // a constant launch count: the slot kernel and the path kernel, then the sample kernel when asked
+  CU(timed.run(st, c->launches, [&](int *launches) {
+    return mplx::with_dim(dim, [&](auto DIM) {
+      if (cudaError_t e = mplx::launch(mplx::ptraj_seg_kernel<DIM>, total, true, st, launches, PA)) return e;
+      if (cudaError_t e = mplx::launch(mplx::ptraj_path_kernel, n_q, false, st, launches, A)) return e;
+      if (!A.samples) return cudaSuccess;
+      return mplx::launch(mplx::traj_sample_kernel<DIM>, (long long)n_q * (n_samples + 1), true, st, launches, A);
+    });
+  }));
+  if (total > 0) {
+    CU(cudaMemcpyAsync(out->nodes, B.wps.p, sizeof(mplx_waypoint) * total, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->seg_t, B.seg_t.p, sizeof(double) * total, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out->coeff, B.coeff.p, sizeof(double) * total * (dim + 1) * 6, cudaMemcpyDeviceToHost, st));
+  }
+  if (out->samples)
+    CU(cudaMemcpyAsync(out->samples, B.samples.p, sizeof(double) * n_rows * (4 * dim + 3), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(timed.seconds(&out->seconds));
   return MPLX_OK;

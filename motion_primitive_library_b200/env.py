@@ -93,6 +93,7 @@ class env_map:
         self.potential_weight_, self.gradient_weight_ = 0.1, 0.0
         self._potential = None
         self._dirty = True
+        self._last_nq = 0  # queries of the last plan_batch* call (batch_trajectories' offset length)
         self.upload_map()
 
     # -- lifecycle ------------------------------------------------------------------------
@@ -421,33 +422,41 @@ class env_map:
         abi.check(rc)
 
     def plan_batch(self, starts, goals, eps=1.0, max_expand=1000, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
-                   tol_yaw=-1.0, start_free=None, closed=True):
+                   tol_yaw=-1.0, start_free=None, closed=True, trajectories=False, n_samples=0, traj_room_bytes=0):
         """mplx_plan_batch: the A* searches of n (start, goal) queries on the device (occupancy planning;
         plan_batch_cost_terms serves potential-field and yaw planning).  Returns a dict: valid, cost, expanded,
         n_closed (arrays), actions / closed (one array per query), slots, arena_bytes, seconds.  Raises
-        MplxError (code MPLX_ERR_ARG) for the plans it refuses."""
+        MplxError (code MPLX_ERR_ARG) for the plans it refuses.
+
+        trajectories=True records the searches' trajectories (mplx_set_batch_trajectories; traj_room_bytes > 0
+        sizes the device room, a diagnostic) and adds `trajectories`, one dict per query (see _trajectories), and
+        `traj_seconds`, the device time of mplx_plan_batch_trajectories."""
         return self._plan_batch(self._lib.mplx_plan_batch, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc,
-                                tol_yaw, start_free, closed)
+                                tol_yaw, start_free, closed, trajectories, n_samples, traj_room_bytes)
 
     def plan_batch_cost_terms(self, starts, goals, eps=1.0, max_expand=1000, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
-                              tol_yaw=-1.0, start_free=None, closed=True):
+                              tol_yaw=-1.0, start_free=None, closed=True, trajectories=False, n_samples=0,
+                              traj_room_bytes=0):
         """mplx_plan_batch_cost_terms: plan_batch for every plan, including a potential map (with or without a
         gradient weight), a yaw control and a search region; the sample loop sums the potential, gradient and
         yaw-alignment terms.  tol_yaw >= 0 adds |yaw - goal yaw| <= tol_yaw to the goal test.  Same results dict;
         raises MplxError for max_expand <= 0, more than 256 primitives, a missing map or parameters
-        (MPLX_ERR_ARG) and search memory beyond the budget (MPLX_ERR_ALLOC)."""
+        (MPLX_ERR_ARG) and search memory beyond the budget (MPLX_ERR_ALLOC).  trajectories, n_samples and
+        traj_room_bytes as plan_batch."""
         return self._plan_batch(self._lib.mplx_plan_batch_cost_terms, starts, goals, eps, max_expand, tol_pos, tol_vel,
-                                tol_acc, tol_yaw, start_free, closed)
+                                tol_acc, tol_yaw, start_free, closed, trajectories, n_samples, traj_room_bytes)
 
     def plan_batch_grow(self, starts, goals, eps=1.0, max_expand=-1, tol_pos=0.5, tol_vel=-1.0, tol_acc=-1.0,
                         tol_yaw=-1.0, start_free=None, closed=True, cost_terms=False, first_cap=0, max_cap=0,
-                        pool_bytes=0):
+                        pool_bytes=0, trajectories=False, n_samples=0, traj_room_bytes=0):
         """mplx_plan_batch_grow: plan_batch (cost_terms=False) or plan_batch_cost_terms (cost_terms=True) with
         arenas sized for the batch and grown for the queries that outgrow them, so max_expand <= 0 (unbounded)
         is served too.  first_cap / max_cap / pool_bytes: 0 = automatic (include/mplx.h has the round schedule).
         Returns plan_batch's dict plus searched (0: the query needed more than the largest arena; its fields are
-        0 / +inf and its lists empty), rounds, reruns, first_cap and last_cap."""
+        0 / +inf and its lists empty), rounds, reruns, first_cap and last_cap.  trajectories, n_samples and
+        traj_room_bytes as plan_batch (a query with searched 0 has no trajectory)."""
         self._sync_params()
+        self._record(trajectories, traj_room_bytes)
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)
         goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE).reshape(-1)
         n = starts.size
@@ -460,21 +469,66 @@ class env_map:
             self._h, 1 if cost_terms else 0, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps),
             int(max_expand), float(tol_pos), float(tol_vel), float(tol_acc), float(tol_yaw), 1 if closed else 0,
             int(first_cap), int(max_cap), int(pool_bytes), C.byref(out)))
+        self._last_nq = n
         na, nc = int(n_actions.sum()), int(n_closed.sum()) if closed else 0
         aoff, coff = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
         acts, keys = np.zeros(max(na, 1), np.int32), np.zeros(max(nc, 1), np.uint64)
         abi.check(self._lib.mplx_plan_batch_grow_results(self._h, aoff.ctypes.data, acts.ctypes.data, acts.size,
                                                          coff.ctypes.data, keys.ctypes.data if closed else None,
                                                          keys.size))
-        return dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
-                    actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
-                    closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
-                    searched=searched, slots=int(out.slots), arena_bytes=int(out.arena_bytes),
-                    seconds=float(out.seconds), rounds=int(out.rounds), reruns=int(out.reruns),
-                    first_cap=int(out.first_cap), last_cap=int(out.last_cap))
+        res = dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
+                   actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
+                   closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
+                   searched=searched, slots=int(out.slots), arena_bytes=int(out.arena_bytes),
+                   seconds=float(out.seconds), rounds=int(out.rounds), reruns=int(out.reruns),
+                   first_cap=int(out.first_cap), last_cap=int(out.last_cap))
+        if trajectories:
+            res["trajectories"], res["traj_seconds"] = self.batch_trajectories(
+                n_samples, sum(len(a) + 1 for a in res["actions"] if len(a)))
+        return res
 
-    def _plan_batch(self, fn, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc, tol_yaw, start_free, closed):
+    def _record(self, trajectories, traj_room_bytes):
+        abi.check(self._lib.mplx_set_batch_trajectories(self._h, 1 if trajectories else 0, int(traj_room_bytes)))
+
+    def batch_trajectories(self, n_samples=0, capacity=1):
+        """mplx_plan_batch_trajectories: the trajectories of the last plan_batch* call, which ran with
+        trajectories=True.  Returns (one dict per query, device seconds).  A dict holds `nodes` (WAYPOINT_DTYPE,
+        the stored coordinates of the path's states from start to goal; their positions are a path for
+        TrajSolverBatch.solve), `seg_t` (one T per segment), `coeff` (segments x (Dim+1) x 6: Primitive
+        coefficients, axes then yaw) and, with n_samples > 0, `samples` (Trajectory::sample(n_samples) rows
+        {pos, vel, acc, jrk, yaw, yaw_dot, t}).  A query without a trajectory has no nodes and no segments.  The
+        dicts go as they are into traverse_trajectories and TrajSolverBatch.scale.  capacity: the waypoint slots
+        to try first (a query with n > 0 actions takes n + 1)."""
+        dim = self.Dim
+        n_q = self._last_nq
+        offset = np.zeros(n_q + 1, np.int64)
+        samples = np.zeros((n_q, n_samples + 1, 4 * dim + 3)) if n_samples > 0 else None
+        cap = max(int(capacity), 1)
+        for _ in range(2):  # the first call reports the slots needed when cap is too small
+            nodes = np.zeros(cap, dtype=WAYPOINT_DTYPE)
+            seg_t = np.zeros(cap)
+            coeff = np.zeros((cap, dim + 1, 6))
+            out = abi.BatchTrajOut(offset.ctypes.data, nodes.ctypes.data, seg_t.ctypes.data, coeff.ctypes.data,
+                                   abi.ptr(samples), cap, 0, 0.0)
+            rc = self._lib.mplx_plan_batch_trajectories(self._h, int(n_samples), C.byref(out))
+            if rc == 0 or out.total <= cap:
+                break
+            cap = int(out.total)
+        abi.check(rc)
+        res = []
+        for q in range(n_q):
+            o, o1 = int(offset[q]), int(offset[q + 1])
+            s = max(o1 - o - 1, 0)
+            r = dict(nodes=nodes[o:o1].copy(), seg_t=seg_t[o:o + s].copy(), coeff=coeff[o:o + s].copy())
+            if samples is not None:
+                r["samples"] = samples[q].copy()
+            res.append(r)
+        return res, float(out.seconds)
+
+    def _plan_batch(self, fn, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc, tol_yaw, start_free, closed,
+                    trajectories=False, n_samples=0, traj_room_bytes=0):
         self._sync_params()
+        self._record(trajectories, traj_room_bytes)
         starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE).reshape(-1)
         goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE).reshape(-1)
         n = starts.size
@@ -490,10 +544,15 @@ class env_map:
                            0, 0, 0.0)
         abi.check(fn(self._h, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps), int(max_expand),
                      float(tol_pos), float(tol_vel), float(tol_acc), float(tol_yaw), C.byref(out)))
-        return dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
-                    actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
-                    closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
-                    slots=int(out.slots), arena_bytes=int(out.arena_bytes), seconds=float(out.seconds))
+        self._last_nq = n
+        res = dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
+                   actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
+                   closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
+                   slots=int(out.slots), arena_bytes=int(out.arena_bytes), seconds=float(out.seconds))
+        if trajectories:
+            res["trajectories"], res["traj_seconds"] = self.batch_trajectories(
+                n_samples, sum(len(a) + 1 for a in res["actions"] if len(a)))
+        return res
 
     def set_kernel(self, which: int):
         """0 = auto, 1 = literal sequential loop, 2 = register kernel, 3 = flat kernel, 4 = dealing kernel."""

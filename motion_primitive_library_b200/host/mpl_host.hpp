@@ -1555,6 +1555,8 @@ class env_map_gpu : public env_map_host<Dim> {
   mutable std::vector<decimal_t> action_cost_;
   mutable unsigned long action_cost_version_ = ~0ul;
   static mplx_waypoint pod(const Waypoint<Dim> &w) { return to_pod(w); }
+  /// the waypoint of a device state, with the env's control flag
+  Waypoint<Dim> unpod(const mplx_waypoint &p) const { return from_pod(p, control_); }
   int control() const { return control_; }
 
   /// bring the device copy of the map (sparse edits as sparse updates), the parameters, the potential
@@ -2796,6 +2798,11 @@ class MultiQueryPlanner {
     std::size_t n_closed = 0;
     std::vector<int> actions;
     std::vector<uint64_t> closed_keys;  // sorted; only with setCollectClosed(true)
+    /// only with setCollectTrajectories(true): recoverTraj's edges (segment k = forward_action(traj[k].from,
+    /// traj[k].action_id), `from` the stored coordinates of the path's k-th state) and the stored coordinates of
+    /// the goal state the last one leads to; empty without a trajectory of at least one segment
+    std::vector<Edge<Dim>> traj;
+    Waypoint<Dim> traj_end;
   };
   /// Which loop plan() runs.  AUTO picks, for max_expand > 0 and |U| <= 256 when the batch's worst-case
   /// search memory fits the device-memory budget:
@@ -2847,6 +2854,20 @@ class MultiQueryPlanner {
   }
   /// also return each query's closed set (sorted lattice keys) in Result::closed_keys
   void setCollectClosed(bool on) { collect_closed_ = on; }
+  /// also return each query's trajectory in Result::traj / traj_end, on every path: the lock-step loop takes
+  /// recoverTraj's edges, the device searches record the stored coordinates of the path's states
+  /// (mplx_set_batch_trajectories, mplx_plan_batch_trajectories)
+  void setCollectTrajectories(bool on) { collect_traj_ = on; }
+  /// a query's trajectory as PlannerBase::getTrajectory builds it: forward_action per edge
+  Trajectory<Dim> trajectory(const Result &r) const {
+    vec_E<Primitive<Dim>> prs;
+    for (const auto &e : r.traj) {
+      Primitive<Dim> pr;
+      gpu_->forward_action(e.from, e.action_id, pr);
+      prs.push_back(pr);
+    }
+    return Trajectory<Dim>(prs);
+  }
   /// the path the last plan() ran: true = a device search
   bool lastPlanOnDevice() const { return last_device_ != 0; }
   /// the path the last plan() ran: 0 = lock-step, 1 = mplx_plan_batch, 2 = mplx_plan_batch_cost_terms,
@@ -2967,6 +2988,10 @@ class MultiQueryPlanner {
       res[q].valid = !std::isinf(res[q].cost);
       res[q].expanded = st[q]->expanded();
       for (const auto &e : traj) res[q].actions.push_back(e.action_id);
+      if (collect_traj_ && !traj.empty()) {
+        res[q].traj = traj;
+        res[q].traj_end = ss[q]->best_child_.back()->coord;
+      }
       for (const auto *stt : ss[q]->order_)
         if (stt->iterationclosed) {
           res[q].n_closed++;
@@ -3014,6 +3039,35 @@ class MultiQueryPlanner {
     nodes_ += d.expd[q];
   }
 
+  /// Trajectory recording for the next device search on the ctx: on with setCollectTrajectories(true).
+  void record_trajectories() const {
+    if (mplx_set_batch_trajectories(gpu_->ctx(), collect_traj_ ? 1 : 0, 0) != MPLX_OK)
+      throw std::runtime_error(mplx_last_error());
+  }
+
+  /// Result::traj / traj_end of the queries the last device search gave a trajectory (res[q].actions set), from
+  /// the stored coordinates it recorded (mplx_plan_batch_trajectories).
+  void take_device_trajectories(std::vector<Result> &res) const {
+    const std::size_t Q = res.size();
+    int64_t cap = 0;
+    for (const Result &r : res)
+      if (!r.actions.empty()) cap += (int64_t)r.actions.size() + 1;
+    cap = std::max<int64_t>(cap, 1);
+    std::vector<int64_t> off(Q + 1);
+    std::vector<mplx_waypoint> nodes((std::size_t)cap);
+    std::vector<double> seg((std::size_t)cap), coeff((std::size_t)cap * (Dim + 1) * 6);
+    mplx_batch_traj_out out{off.data(), nodes.data(), seg.data(), coeff.data(), nullptr, cap, 0, 0.0};
+    if (mplx_plan_batch_trajectories(gpu_->ctx(), 0, &out) != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    for (std::size_t q = 0; q < Q; q++) {
+      const int64_t n = off[q + 1] - off[q];
+      if (n == 0) continue;
+      if (n != (int64_t)res[q].actions.size() + 1) throw std::runtime_error("device trajectory length mismatch");
+      for (int64_t j = 0; j + 1 < n; j++)
+        res[q].traj.push_back(Edge<Dim>{gpu_->unpod(nodes[(std::size_t)(off[q] + j)]), res[q].actions[(std::size_t)j]});
+      res[q].traj_end = gpu_->unpod(nodes[(std::size_t)(off[q] + n - 1)]);
+    }
+  }
+
   /// plan() on the device: every query's whole A* in one mplx_plan_batch call (cost_terms:
   /// mplx_plan_batch_cost_terms).  The start-is-free test runs here on the host map, as in the lock-step
   /// loop.  Returns false, with nothing planned, when the worst-case search memory does not fit the
@@ -3042,6 +3096,7 @@ class MultiQueryPlanner {
     mplx_batch_out out{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), d.aoff.data(), d.acts.data(),
                        (int64_t)d.acts.size(), collect_closed_ ? d.coff.data() : nullptr,
                        collect_closed_ ? d.keys.data() : nullptr, (int64_t)d.keys.size(), 0, 0, 0.0};
+    record_trajectories();
     const auto t0 = std::chrono::steady_clock::now();
     const int rc = (cost_terms ? mplx_plan_batch_cost_terms : mplx_plan_batch)(
         gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_,
@@ -3056,6 +3111,7 @@ class MultiQueryPlanner {
     slots_ = out.slots;
     arena_bytes_ = out.arena_bytes;
     for (std::size_t q = 0; q < Q; q++) take_device_result(d, q, res[q]);
+    if (collect_traj_) take_device_trajectories(res);
     return true;
   }
 
@@ -3077,6 +3133,7 @@ class MultiQueryPlanner {
     std::vector<int32_t> nact(Q), searched(Q);
     mplx_grow_out out{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), nact.data(), searched.data(), 0, 0, 0,
                       0, 0, 0, 0.0};
+    record_trajectories();
     const auto t0 = std::chrono::steady_clock::now();
     const int rc = mplx_plan_batch_grow(gpu_->ctx(), gpu_->keys_only_possible() ? 0 : 1, S.data(), G.data(), fr.data(),
                                         (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_, gpu_->tol_acc_,
@@ -3106,6 +3163,8 @@ class MultiQueryPlanner {
       }
       take_device_result(d, q, res[q]);
     }
+    // the device's trajectories before the lock-step loop takes the rest (unsearched queries have none)
+    if (collect_traj_) take_device_trajectories(res);
     if (!rest.empty()) {
       const int path = path_;
       path_ = LOCKSTEP;
@@ -3165,6 +3224,7 @@ class MultiQueryPlanner {
   bool keys_only_ = true;
   int path_ = AUTO;
   bool collect_closed_ = false;
+  bool collect_traj_ = false;
   int last_device_ = 0;  // lastDevicePath()
   int slots_ = 0;
   long long arena_bytes_ = 0;

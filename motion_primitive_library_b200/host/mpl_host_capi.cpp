@@ -124,6 +124,12 @@ struct BatchSession {
   std::vector<int64_t> aoff, coff;
   std::vector<int32_t> actions;
   std::vector<uint64_t> closed;
+  // mplh_batch_set_trajectories; and the trajectories of the last plan made with it on, in mplx_traj_out's slot
+  // layout (query q's nodes at [toff[q], toff[q+1]), one segment time and (dim+1)*6 coefficients per slot)
+  bool traj = false, has_traj = false;
+  std::vector<int64_t> toff;
+  std::vector<mplx_waypoint> tnodes;
+  std::vector<double> tseg, tcoeff;
 };
 /// the Dim of a MultiQueryPlanner<Dim>, for the bodies with_session runs
 template <class Q>
@@ -200,6 +206,30 @@ int batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *
       s.closed.insert(s.closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
       s.aoff[q + 1] = (int64_t)s.actions.size();
       s.coff[q + 1] = (int64_t)s.closed.size();
+    }
+    s.has_traj = s.traj;
+    if (s.traj) {
+      using Env = std::decay_t<decltype(mq.env())>;
+      s.toff.assign((size_t)n_q + 1, 0);
+      s.tnodes.clear();
+      s.tseg.clear();
+      s.tcoeff.clear();
+      for (int q = 0; q < n_q; q++) {
+        for (const auto &e : res[q].traj) {
+          Primitive<Dim> pr;
+          mq.env().forward_action(e.from, e.action_id, pr);
+          s.tnodes.push_back(Env::pod(e.from));
+          s.tseg.push_back(pr.t());
+          for (int a = 0; a <= Dim; a++)
+            for (int k = 0; k < 6; k++) s.tcoeff.push_back(a < Dim ? pr.pr(a).c[k] : pr.pr_yaw().c[k]);
+        }
+        if (!res[q].traj.empty()) {  // the goal state: no segment
+          s.tnodes.push_back(Env::pod(res[q].traj_end));
+          s.tseg.push_back(0.0);
+          s.tcoeff.insert(s.tcoeff.end(), (size_t)(Dim + 1) * 6, 0.0);
+        }
+        s.toff[q + 1] = (int64_t)s.tnodes.size();
+      }
     }
     if (totals) {
       totals[0] = (double)mq.iterations(); totals[1] = (double)mq.nodes_expanded(); totals[2] = secs;
@@ -408,6 +438,56 @@ int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coef
     const Trajectory<Dim> traj = make_trajectory<Dim>(n_seg, seg_t, coeff, control);
     if (samples) put_samples<Dim>(traj, n_samples, samples);
     if (waypoints) put_waypoints<Dim>(traj, waypoints);
+  });
+}
+
+/* The session's plans also collect every query's trajectory (on = 1; 0 = off, the default), whichever path runs
+ * them (MultiQueryPlanner::setCollectTrajectories), for mplh_batch_trajectories. */
+int mplh_batch_set_trajectories(void *session, int on) {
+  return with_session(session, [&](auto &mq, BatchSession &s) {
+    mq.setCollectTrajectories(on != 0);
+    s.traj = on != 0;
+  }, on == 0 || on == 1, "null session or on not 0 or 1");
+}
+
+/* The trajectories of the session's last plan, which ran with mplh_batch_set_trajectories(session, 1), in
+ * mplx_batch_traj_out's layout: query q owns the slots [offset[q], offset[q+1]) (n_actions + 1 with a trajectory
+ * of at least one segment, else 0): nodes (the stored coordinates of the path's states, start to goal), seg_t (dt
+ * per segment, 0 on the last slot) and coeff ((dim+1)*6 per slot: forward_action's Primitive, highest order first,
+ * axes then yaw; 0 on the last slot); samples NULL or [n_q*(n_samples+1)*(4*dim+3)] Trajectory::sample(n_samples)
+ * rows (zeros for a query without trajectory).  When capacity < the slots needed, offset and *total are written
+ * and the call fails.  Fails with nothing written without such a plan, for n_samples < 0, samples with
+ * n_samples == 0, or a missing array. */
+int mplh_batch_trajectories(void *session, int n_samples, int64_t *offset, mplx_waypoint *nodes, double *seg_t,
+                            double *coeff, double *samples, int64_t capacity, int64_t *total) {
+  return with_session(session, [&](auto &, BatchSession &s) {
+    constexpr int NC = 6;
+    if (!s.has_traj) throw std::runtime_error("the session's last plan did not collect trajectories");
+    if (n_samples < 0 || (samples && n_samples == 0)) throw std::runtime_error("bad n_samples");
+    if (!offset || !nodes || !seg_t || !coeff || !total) throw std::runtime_error("missing output array");
+    const int64_t need = (int64_t)s.tnodes.size();
+    std::copy(s.toff.begin(), s.toff.end(), offset);
+    *total = need;
+    if (capacity < need) throw std::runtime_error("capacity below the waypoint slots needed");
+    std::copy(s.tnodes.begin(), s.tnodes.end(), nodes);
+    std::copy(s.tseg.begin(), s.tseg.end(), seg_t);
+    std::copy(s.tcoeff.begin(), s.tcoeff.end(), coeff);
+    if (!samples) return;
+    mplh::with_dim(s.dim, g_err, 2, [&](auto dimtag) {
+      constexpr int Dim = decltype(dimtag)::value;
+      const std::size_t rows = (std::size_t)n_samples + 1, w = 4 * Dim + 3;
+      for (std::size_t q = 0; q + 1 < s.toff.size(); q++) {
+        double *o = samples + q * rows * w;
+        const int64_t b = s.toff[q], n = s.toff[q + 1] - b;
+        if (n == 0) {
+          std::fill(o, o + rows * w, 0.0);
+          continue;
+        }
+        put_samples<Dim>(make_trajectory<Dim>((int)n - 1, s.tseg.data() + b, s.tcoeff.data() + b * (Dim + 1) * NC,
+                                              s.control),
+                         n_samples, o);
+      }
+    });
   });
 }
 }

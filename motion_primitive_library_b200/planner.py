@@ -76,6 +76,8 @@ SIGNATURES = {
     "mplh_batch_grow_stats": ([_vp, _i32p, _i64p, _i64p, _i64p, _i32p], _i),
     "mplh_batch_last_path": ([_vp, _i32p, _i32p, _i64p], _i),
     "mplh_batch_close": ([_vp, C.POINTER(_d)], _i),
+    "mplh_batch_set_trajectories": ([_vp, _i], _i),
+    "mplh_batch_trajectories": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64p], _i),
     "mplh_traj_solve": ([_i, _i, _i, _vp, _vp, _i, _vp, _d, _i, _i32p, _vp, _vp, _vp, _vp], _i),
     "mplh_traj_sample": ([_i, _i, _vp, _vp, _i, _i, _vp, _vp], _i),
     "mplh_traj_scale": ([_i, _i, _vp, _vp, _i, _i, _d, _d, _d, _i, _i32p, C.POINTER(_d), _vp, _i32p, _vp, _vp], _i),
@@ -371,11 +373,21 @@ class BatchPlanner:
             res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
         return res, totals
 
-    def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True):
+    def plan_detail(self, starts, goals, eps=None, max_num=None, closed=True, trajectories=False, n_samples=0):
         """plan() that also returns every query's trajectory (action ids) and closed set (sorted lattice keys):
         (res, totals, actions, closed) with one array per query in actions / closed.  Any max_num, including
-        max_num <= 0 (unbounded): the outputs are sized from the results."""
-        res, totals = self._plan("mplh_batch_plan_keep", starts, goals, eps, max_num, 1 if closed else 0)
+        max_num <= 0 (unbounded): the outputs are sized from the results.
+
+        trajectories=True collects every query's planned trajectory on whichever path runs
+        (MultiQueryPlanner::setCollectTrajectories) and returns (res, totals, actions, closed, trajectories):
+        one dict per query as env_map.batch_trajectories gives them (nodes, seg_t, coeff and, with n_samples > 0,
+        samples)."""
+        self._call("mplh_batch_set_trajectories", 1 if trajectories else 0)
+        try:
+            res, totals = self._plan("mplh_batch_plan_keep", starts, goals, eps, max_num, 1 if closed else 0)
+        finally:
+            if trajectories:
+                self._call("mplh_batch_set_trajectories", 0)
         nq = len(res)
         na, nc = int(res["n_actions"].sum()), int(res["n_closed"].sum()) if closed else 0
         aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
@@ -384,8 +396,31 @@ class BatchPlanner:
         self._call("mplh_batch_kept", aoff.ctypes.data, acts.ctypes.data, acts.size, coff.ctypes.data,
                    None if keys is None else keys.ctypes.data, 0 if keys is None else keys.size)
         tot = self._totals(totals)
-        return (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
-                [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
+        out = (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
+               [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
+        if not trajectories:
+            return out
+        return out + (self._trajectories(nq, int(sum(n + 1 for n in res["n_actions"] if n)), n_samples),)
+
+    def _trajectories(self, nq, cap, n_samples):
+        """mplh_batch_trajectories: the last plan's trajectories, one dict per query."""
+        dim = self._args.dim
+        cap = max(cap, 1)
+        offset, total = np.zeros(nq + 1, np.int64), C.c_int64(0)
+        nodes = np.zeros(cap, dtype=WAYPOINT_DTYPE)
+        seg_t, coeff = np.zeros(cap), np.zeros((cap, dim + 1, 6))
+        samples = np.zeros((nq, n_samples + 1, 4 * dim + 3)) if n_samples > 0 else None
+        self._call("mplh_batch_trajectories", int(n_samples), offset.ctypes.data, nodes.ctypes.data, seg_t.ctypes.data,
+                   coeff.ctypes.data, None if samples is None else samples.ctypes.data, cap, C.byref(total))
+        res = []
+        for q in range(nq):
+            o, o1 = int(offset[q]), int(offset[q + 1])
+            s = max(o1 - o - 1, 0)
+            r = dict(nodes=nodes[o:o1].copy(), seg_t=seg_t[o:o + s].copy(), coeff=coeff[o:o + s].copy())
+            if samples is not None:
+                r["samples"] = samples[q].copy()
+            res.append(r)
+        return res
 
     def _totals(self, totals):
         t = dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),
