@@ -405,6 +405,32 @@ typedef struct {
  * call replaces them.  A constant number of launches per call.  Synchronous. */
 int mplx_plan_batch_trajectories(mplx_ctx *ctx, int n_samples, mplx_batch_traj_out *out);
 
+/* ---- one tunnel per query of the batched searches ---------------------------------------------- */
+
+/* MapPlanner<Dim>::setSearchRegion(path, dense) once per query for the following mplx_plan_batch / _cost_terms /
+ * _grow calls: query q's tunnel is built from the points pts[pt_offset[q] .. pt_offset[q+1]) (ctx-dim doubles
+ * each) with the one radius (ctx-dim doubles) and dense flag of the batch, and is exactly the region
+ * mplx_set_search_region_path builds from those points.  Those calls must then have exactly n_q queries (else
+ * MPLX_ERR_ARG, doing nothing); query q searches in tunnel q, which replaces the ctx-wide region for it, as
+ * setSearchRegion replaces search_region_.  The expansion, edge and trajectory-check calls keep the ctx-wide region.
+ * n_q = 0 clears the tunnels.  mplx_set_map drops them; mplx_update_cells keeps them.
+ *
+ * A tunnel is stored as the 8x8x8 bricks (8x8 tiles in 2-D) it touches, with one bit per cell, so its memory grows
+ * with the tunnel, not the map (mplx_batch_regions_info reports it).  The store comes off the search calls' budget
+ * (mplx_plan_batch_fits); MPLX_ERR_ALLOC, with the tunnels unchanged, when it alone exceeds that budget.  A constant
+ * number of launches whatever n_q.  Refusals, each with MPLX_ERR_ARG, nothing changed and no launch: no map,
+ * n_q < 0, a NULL array (n_q > 0), pt_offset[0] != 0, and a query with no points (pt_offset must increase).
+ * Synchronous. */
+int mplx_set_batch_regions(mplx_ctx *ctx, int n_q, const int64_t *pt_offset, const double *pts, const double *radius,
+                           int dense);
+
+/* The tunnels set on the ctx: their query count (0 = none), bricks and device bytes.  Any pointer may be NULL. */
+int mplx_batch_regions_info(mplx_ctx *ctx, int32_t *n_q, int64_t *n_bricks, int64_t *bytes);
+
+/* Diagnostics: query q's tunnel as one byte per voxel (1 = inside), the layout mplx_set_search_region_path's
+ * out_region has.  MPLX_ERR_ARG when no tunnels are set, q is out of range or out is NULL.  Synchronous. */
+int mplx_read_batch_region(mplx_ctx *ctx, int q, uint8_t *out);
+
 /* ---- trajectories through waypoints (TrajSolver) ----------------------------------------------- */
 
 /* Results of mplx_traj_solve (HOST arrays).  Path p owns the waypoint slots [offset[p], offset[p+1]); segment j

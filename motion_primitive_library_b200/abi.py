@@ -54,6 +54,9 @@ EXPORTED_SYMBOLS = (
     "mplx_plan_batch_grow_results",
     "mplx_set_batch_trajectories",
     "mplx_plan_batch_trajectories",
+    "mplx_set_batch_regions",
+    "mplx_batch_regions_info",
+    "mplx_read_batch_region",
     "mplx_traj_solve",
     "mplx_traj_scale",
     "mplx_traj_check",
@@ -269,6 +272,12 @@ def load() -> C.CDLL:
     lib.mplx_set_batch_trajectories.restype = i32
     lib.mplx_plan_batch_trajectories.argtypes = [vp, i32, C.POINTER(BatchTrajOut)]
     lib.mplx_plan_batch_trajectories.restype = i32
+    lib.mplx_set_batch_regions.argtypes = [vp, i32, vp, vp, vp, i32]
+    lib.mplx_set_batch_regions.restype = i32
+    lib.mplx_batch_regions_info.argtypes = [vp, C.POINTER(C.c_int32), C.POINTER(i64), C.POINTER(i64)]
+    lib.mplx_batch_regions_info.restype = i32
+    lib.mplx_read_batch_region.argtypes = [vp, i32, vp]
+    lib.mplx_read_batch_region.restype = i32
     lib.mplx_traj_solve.argtypes = [vp, i32, vp, vp, vp, vp, f64, i32, i32, i32, C.POINTER(TrajOut)]
     lib.mplx_traj_solve.restype = i32
     lib.mplx_traj_scale.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, i32, C.POINTER(TrajScaleOut)]

@@ -117,7 +117,7 @@ int mplx_destroy(mplx_ctx *c) {
   c->occ.release(); c->occ2.release(); c->ttab.release(); c->tcount.release(); c->tdt.release();
   for (int b = 0; b < kPackBufs; b++) c->cb[b].release();
   if (c->d2h_stream) cudaStreamDestroy(c->d2h_stream);
-  c->eb.release(); c->fxq.release(); c->ub.release(); c->sb.release(); c->tb.release();
+  c->eb.release(); c->fxq.release(); c->ub.release(); c->sb.release(); c->tun.release(); c->tb.release();
   c->d_nodes.release(); c->d_succ.release(); c->d_count.release(); c->d_action.release();
   c->d_lattice.release(); c->d_cost.release(); c->d_key.release();
   c->h_nodes.release(); c->h_succ.release(); c->h_count.release(); c->h_action.release();
@@ -180,6 +180,7 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
   c->has_map = true;
   c->has_pot = false;
   c->has_region = false;
+  c->tun.release();  // the per-query tunnels go with the ctx-wide region
   refresh_params(c);
   return MPLX_OK;
 }

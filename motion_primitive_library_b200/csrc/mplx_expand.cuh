@@ -10,6 +10,7 @@
 #include "mplx_device.cuh"
 #include "mplx_kernels.h"
 #include "mplx_prim.cuh"
+#include "mplx_tunnel.cuh"
 
 namespace mplx {
 
@@ -29,6 +30,17 @@ constexpr VoxelRaw kVoxelNone = 0x100u;  // in-region, free
 __device__ __forceinline__ VoxelRaw voxel_fetch(const EnvParams &P, int idx) {
   unsigned r = 0x100u;
   if (P.region_bits != nullptr) r = ((__ldg(P.region_bits + (idx >> 5)) >> (idx & 31)) & 1u) << 8;
+  if (P.pot != nullptr)
+    r |= (unsigned)(unsigned char)__ldg(P.pot + idx);
+  else
+    r |= (__ldg(P.occ_bits + (idx >> 5)) >> (idx & 31)) & 1u;
+  return r;
+}
+// voxel_fetch with the tunnel bit read from one query's tunnel (mplx_set_batch_regions) in place of
+// P.region_bits, which a tunnelled query ignores
+__device__ __forceinline__ VoxelRaw voxel_fetch_tunnel(const EnvParams &P, const TunnelView &tv, int idx) {
+  const int x = idx % P.mdim[0], yz = idx / P.mdim[0];
+  unsigned r = (unsigned)tunnel_has(tv, P.dim, P.mdim, x, yz % P.mdim[1], yz / P.mdim[1]) << 8;
   if (P.pot != nullptr)
     r |= (unsigned)(unsigned char)__ldg(P.pot + idx);
   else
@@ -413,13 +425,14 @@ __device__ __forceinline__ int sample_loop_count(const EnvParams &P, int n, doub
 // otherwise the terms of the group were added to c in sample order -> 0, call again with left - UNR.
 // n_samples counts what the reference's loop visits (up to and including the first blocking
 // sample) and is only maintained when the stats counters are on.
-template <int DIM, int ORD, bool YAW, int UNR>
+// TUN: the tunnel bit comes from the query's tunnel *tv (voxel_fetch_tunnel) rather than P.region_bits.
+template <int DIM, int ORD, bool YAW, int UNR, bool TUN = false>
 __device__ __forceinline__ int sample_group(const EnvParams &P, const double (&cf)[CoefLayout<DIM, ORD, YAW>::NCMAX],
                                             bool need_vel, double dt, int left, double &t, double &c,
-                                            unsigned &n_samples, YawRot &yr) {
+                                            unsigned &n_samples, YawRot &yr, const TunnelView *tv = nullptr) {
   using CL = CoefLayout<DIM, ORD, YAW>;
   const int NC = CL::ncoef(need_vel);
-  const bool plain = P.pot == nullptr && P.region_bits == nullptr && !YAW;
+  const bool plain = !TUN && P.pot == nullptr && P.region_bits == nullptr && !YAW;
   double ts[UNR];
   int idx[UNR];
   bool in[UNR];
@@ -464,7 +477,7 @@ __device__ __forceinline__ int sample_group(const EnvParams &P, const double (&c
 #pragma unroll
   for (int j = 0; j < UNR; j++) {
     raw[j] = kVoxelNone;
-    if (j < left && in[j]) raw[j] = voxel_fetch(P, idx[j]);
+    if (j < left && in[j]) raw[j] = TUN ? voxel_fetch_tunnel(P, *tv, idx[j]) : voxel_fetch(P, idx[j]);
   }
   bool blocked[UNR];
   double term[UNR];
@@ -506,16 +519,17 @@ __device__ __forceinline__ int sample_group(const EnvParams &P, const double (&c
 // Phase C of the register kernel (mplx_kernels.cu) and the edge cost of the device search
 // (mplx_search.cu): the reference's loop `for (t = 0; t < T; t += dt)` (env_map.h:99) in groups of UNR
 // samples with group-level control flow only (sample_group).  count = iterations of that loop
-// (sample_loop_count).
-template <int DIM, int ORD, bool YAW, int UNR>
+// (sample_loop_count).  TUN and tv: as sample_group.
+template <int DIM, int ORD, bool YAW, int UNR, bool TUN = false>
 __device__ __forceinline__ double traverse_groups(const EnvParams &P, const double (&cf)[CoefLayout<DIM, ORD, YAW>::NCMAX],
-                                                 bool need_vel, double dt, int count, unsigned &n_samples) {
+                                                 bool need_vel, double dt, int count, unsigned &n_samples,
+                                                 const TunnelView *tv = nullptr) {
   double c = 0;
   double t = 0;
   YawRot yr;
   if (YAW) yr.init(cf[CoefLayout<DIM, ORD, YAW>::ncoef(need_vel) - 2], cf[CoefLayout<DIM, ORD, YAW>::ncoef(need_vel) - 1], dt);
   for (int left = count;; left -= UNR) {
-    const int st = sample_group<DIM, ORD, YAW, UNR>(P, cf, need_vel, dt, left, t, c, n_samples, yr);
+    const int st = sample_group<DIM, ORD, YAW, UNR, TUN>(P, cf, need_vel, dt, left, t, c, n_samples, yr, tv);
     if (st == 2) return INFINITY;
     if (st == 1) return c;
   }

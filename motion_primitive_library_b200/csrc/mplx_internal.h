@@ -272,6 +272,22 @@ struct SearchBufs {
   }
 };
 
+// The per-query tunnels of the batched searches (mplx_set_batch_regions, mplx_tunnel.cuh): query q owns the bricks
+// [off[q], off[q+1]) of key and their tunnel_words(dim) mask words each in bits; n_q = 0 when none are set
+struct TunnelStore {
+  int n_q = 0;
+  int64_t n_bricks = 0;
+  DevBuf<uint64_t> key;
+  DevBuf<uint32_t> bits;
+  DevBuf<int64_t> off;
+  size_t bytes() const { return key.cap * sizeof(uint64_t) + bits.cap * sizeof(uint32_t) + off.cap * sizeof(int64_t); }
+  void release() {
+    key.release(); bits.release(); off.release();
+    n_q = 0;
+    n_bricks = 0;
+  }
+};
+
 struct mplx_ctx {
   int dim = 0, device = 0;
   cudaStream_t stream = nullptr;
@@ -305,10 +321,20 @@ struct mplx_ctx {
   EdgeBufs eb;
   UpdateBufs ub;
   SearchBufs sb;
+  TunnelStore tun;
   TrajBufs tb;
   int64_t launches = 0;
   unsigned long long last_stats[2] = {0, 0};
 };
+
+namespace mplx {
+// mplx_maps.cu: the cells and the half-widths of MapPlanner::setSearchRegion, shared by mplx_set_search_region_path
+// and mplx_set_batch_regions
+void region_path_cells(const mplx_ctx *c, const double *path, int n_pts, int dense, std::vector<int> &cells);
+void region_radius_cells(const mplx_ctx *c, const double *radius, int *rn);
+// mplx_search.cu: the device memory one search call may take
+int search_budget(const mplx_ctx *c, size_t &budget);
+}  // namespace mplx
 
 extern "C" {
 int mplx_bind(mplx_ctx *ctx);

@@ -80,6 +80,11 @@ struct Job {
   mplx_waypoint *traj;
   unsigned long long *traj_used, *toffs;
   unsigned long long traj_cap;  // in waypoint slots
+  // per-query tunnels (mplx_set_batch_regions), read by the TUN kernels only: query q's bricks are
+  // [tun_off[q], tun_off[q+1]) of tun_key / tun_bits
+  const uint64_t *tun_key;
+  const uint32_t *tun_bits;
+  const int64_t *tun_off;
 };
 enum GrowState : int32_t { kDone = 1, kOverflowed = 2, kPoolFull = 3 };
 
@@ -114,9 +119,11 @@ __device__ __forceinline__ uint64_t node_hash(const mplx_waypoint *w) {
 // case (layout_for) runs without it, exactly as with it, and spills less in the sample loop.
 // REC: trajectory recording (J.traj); its own instantiation, so that a kernel without it compiles exactly as it
 // did before recording existed (a branch in the tail alone moves the sample loop's register allocation).
-template <int DIM, int ORD, bool YAW, bool COST, bool CHECK, bool REC>
+// TUN: each query searches in its own tunnel (J.tun_*) in place of the ctx-wide region; instantiated with CHECK only.
+template <int DIM, int ORD, bool YAW, bool COST, bool CHECK, bool REC, bool TUN = false>
 __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant__ EnvParams P, const __grid_constant__ Job J) {
   static_assert(COST || !YAW, "a yaw control always sums cost terms");
+  static_assert(CHECK || !TUN, "the tunnel kernels are instantiated with the capacity check only");
   __shared__ mplx_waypoint s_node;
   __shared__ uint32_t vbits[9];
   __shared__ int s_q, s_status;
@@ -161,6 +168,14 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
     }
     __syncthreads();
     if (s_q >= J.n_q) return;
+    TunnelView tv{};
+    if constexpr (TUN) {
+      tv.q = J.qlist[s_q];
+      const int64_t b0 = J.tun_off[tv.q];
+      tv.key = J.tun_key + b0;
+      tv.bits = J.tun_bits + b0 * tunnel_words(DIM);
+      tv.n = (int)(J.tun_off[tv.q + 1] - b0);
+    }
     while (s_status == kRunning) {
       PrimState<DIM, ORD, YAW> pr;
       bool emit, same;
@@ -179,8 +194,9 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
           double dt;
           const int n = sample_count_n(P, max_v, dt);
           unsigned n_samples = 0;
-          cost = traverse_groups<DIM, ORD, YAW, COST ? kCostUnr : 4>(P, cf, vel, dt, sample_loop_count(P, n, dt),
-                                                                     n_samples);
+          cost = traverse_groups<DIM, ORD, YAW, COST ? kCostUnr : 4, TUN>(P, cf, vel, dt,
+                                                                          sample_loop_count(P, n, dt), n_samples,
+                                                                          TUN ? &tv : nullptr);
         }
         if (!isinf(cost)) cost += intrinsic;
         s_cost[sl] = cost;
@@ -253,25 +269,32 @@ __global__ void __launch_bounds__(kThreads) search_kernel(const __grid_constant_
 
 // The instantiation a plan runs: <DIM, ORD, false, false> for the occupancy search, <DIM, ORD, yaw bit,
 // true> for the cost-term search, each with the capacity check or without and with trajectory recording or
-// without.  f receives the kernel's address.
+// without; with per-query tunnels (tun) the TUN kernel, which always checks the capacity (in worst-case arenas the
+// check changes nothing, and it halves the tunnel kernels).  f receives the kernel's address.
 template <class F>
-cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, bool check, bool rec, F &&f) {
+cudaError_t with_search_kernel(const EnvParams &P, bool cost_terms, bool check, bool rec, bool tun, F &&f) {
   return with_bool(rec, [&](auto REC) {
-    return with_bool(check, [&](auto CHECK) {
-      return with_dim(P.dim, [&](auto DIM) {
-        return with_order(P.control, [&](auto ORD) {
-          if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, CHECK, REC>);
-          return with_bool(P.control & 16,
-                           [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, CHECK, REC>); });
-        });
+    return with_bool(check || tun, [&](auto CHECK) {
+      return with_bool(tun, [&](auto TUN) {
+        if constexpr (TUN && !CHECK) {
+          return cudaErrorInvalidValue;
+        } else {
+          return with_dim(P.dim, [&](auto DIM) {
+            return with_order(P.control, [&](auto ORD) {
+              if (!cost_terms) return f(search_kernel<DIM, ORD, false, false, CHECK, REC, TUN>);
+              return with_bool(P.control & 16,
+                               [&](auto YAW) { return f(search_kernel<DIM, ORD, YAW, true, CHECK, REC, TUN>); });
+            });
+          });
+        }
       });
     });
   });
 }
 
-int resident_ctas(const EnvParams &P, bool cost_terms, bool check, bool rec, int block) {
+int resident_ctas(const EnvParams &P, bool cost_terms, bool check, bool rec, bool tun, int block) {
   int per_sm = 0;
-  const cudaError_t e = with_search_kernel(P, cost_terms, check, rec, [&](auto kernel) {
+  const cudaError_t e = with_search_kernel(P, cost_terms, check, rec, tun, [&](auto kernel) {
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0);
   });
   if (e != cudaSuccess) {
@@ -293,14 +316,26 @@ namespace {
 constexpr size_t kQueryBytes =
     2 * sizeof(mplx_waypoint) + 1 + 6 * sizeof(int32_t) + sizeof(double) + sizeof(unsigned long long);
 
+}  // namespace
+
 // The device memory one search call may take: a quarter of the device memory free at the call, counting the
-// arenas and the result pool the ctx already holds as free (they are reused or replaced), at most
-// kSearchArenaBudget.
-int search_budget(const SearchBufs &B, size_t &budget) {
+// arenas, the result pool and the per-query tunnels the ctx already holds as free (the search buffers are reused
+// or replaced; a search call takes the tunnels it reads off its budget again), at most kSearchArenaBudget.
+int mplx::search_budget(const mplx_ctx *c, size_t &budget) {
+  const SearchBufs &B = c->sb;
   size_t free_b = 0, total_b = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
-  const size_t held = B.arena.cap + B.closed.cap * sizeof(uint64_t) + B.traj.cap * sizeof(mplx_waypoint);
+  const size_t held =
+      B.arena.cap + B.closed.cap * sizeof(uint64_t) + B.traj.cap * sizeof(mplx_waypoint) + c->tun.bytes();
   budget = std::min(kSearchArenaBudget, (free_b + held) / 4);
+  return MPLX_OK;
+}
+
+namespace {
+// With per-query tunnels set, a search call must have exactly as many queries (query q searches in tunnel q).
+int check_tunnels(const mplx_ctx *c, const char *fn, int n_q) {
+  if (c->tun.n_q > 0 && n_q != c->tun.n_q)
+    return fail(MPLX_ERR_ARG, "%s: %d queries, but mplx_set_batch_regions set %d tunnels", fn, n_q, c->tun.n_q);
   return MPLX_OK;
 }
 
@@ -327,13 +362,14 @@ int size_batch(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_ex
   L = layout_for(max_expand, nU);
   const int block = ((nU + 31) / 32) * 32;
   size_t budget = 0;
-  const int rc = search_budget(c->sb, budget);
+  const int rc = search_budget(c, budget);
   if (rc) return rc;
   troom = traj_room(c->sb, budget);
   const size_t results = (size_t)n_q * kQueryBytes +
                          (size_t)worst_pool_units(n_q, max_expand, with_closed) * sizeof(uint64_t) +
-                         (size_t)troom * sizeof(mplx_waypoint);
-  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, c->sb.traj_on, block));
+                         (size_t)troom * sizeof(mplx_waypoint) + c->tun.bytes();
+  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, c->sb.traj_on,
+                                                                     c->tun.n_q > 0, block));
   const size_t left = results < budget ? budget - results : 0;
   slots = std::min<int64_t>(slots, (int64_t)(left / (size_t)L.bytes));
   if (slots < 1)
@@ -504,6 +540,10 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   J.traj_used = troom > 0 ? B.toffs.p + n_q : nullptr;
   J.toffs = troom > 0 ? B.toffs.p : nullptr;
   J.traj_cap = troom > 0 ? (unsigned long long)troom : 0ull;
+  const bool tun = c->tun.n_q > 0;
+  J.tun_key = c->tun.key.p;
+  J.tun_bits = c->tun.bits.p;
+  J.tun_off = c->tun.off.p;
   B.next_epoch += (uint32_t)n;
 
   EnvParams P = c->P;
@@ -513,7 +553,7 @@ int run_round(mplx_ctx *c, const Batch &b, const std::vector<int32_t> &qlist, co
   const bool check = b.max_expand <= 0 || L.cap < 1 + (int64_t)b.max_expand * nU;
   TimedRun timed;
   const cudaError_t le = timed.run(c->stream, c->launches, [&](int *launches) {
-    return with_search_kernel(P, b.cost_terms, check, troom > 0, [&](auto kernel) {
+    return with_search_kernel(P, b.cost_terms, check, troom > 0, tun, [&](auto kernel) {
       kernel<<<(int)slots, block, 0, c->stream>>>(P, J);
       const cudaError_t e = cudaGetLastError();
       if (e == cudaSuccess) *launches += 1;
@@ -592,6 +632,8 @@ int plan_batch_fits(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int m
   int rc = check_plan(c, fn, cost_terms, max_expand);
   if (rc) return rc;
   if (n_q < 0) return fail(MPLX_ERR_ARG, "%s: n_q < 0", fn);
+  rc = check_tunnels(c, fn, n_q);
+  if (rc) return rc;
   rc = mplx_bind(c);
   if (rc) return rc;
   Layout L;
@@ -616,6 +658,8 @@ int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint
   if (out->action_capacity < (int64_t)n_q * max_expand ||
       (out->closed_keys && out->closed_capacity < (int64_t)n_q * max_expand))
     return fail(MPLX_ERR_ARG, "%s: capacities below n_q*max_expand", fn);
+  rc = check_tunnels(c, fn, n_q);
+  if (rc) return rc;
   rc = mplx_bind(c);
   if (rc) return rc;
   const bool with_closed = out->closed_keys != nullptr;
@@ -733,6 +777,8 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
     return fail(MPLX_ERR_ARG, "%s: missing output array", fn);
   if (first_cap < 0 || max_cap < 0 || pool_bytes < 0)
     return fail(MPLX_ERR_ARG, "%s: first_cap, max_cap and pool_bytes must be >= 0", fn);
+  rc = check_tunnels(c, fn, n_q);
+  if (rc) return rc;
   rc = mplx_bind(c);
   if (rc) return rc;
   const int nU = c->P.nU;
@@ -741,14 +787,14 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
 
   // the per-query arrays, the trajectory room and the pool's automatic size come off the budget first
   size_t budget = 0;
-  rc = search_budget(c->sb, budget);
+  rc = search_budget(c, budget);
   if (rc) return rc;
   SearchBufs &B = c->sb;
   const int64_t troom = traj_room(B, budget);
-  const size_t results = (size_t)n_q * kQueryBytes + (size_t)troom * sizeof(mplx_waypoint);
+  const size_t results = (size_t)n_q * kQueryBytes + (size_t)troom * sizeof(mplx_waypoint) + c->tun.bytes();
   const size_t pool_auto = budget / 8;
   const size_t avail = results + pool_auto < budget ? budget - results - pool_auto : 0;
-  const int64_t resident = resident_ctas(c->P, ct, true, B.traj_on, block);
+  const int64_t resident = resident_ctas(c->P, ct, true, B.traj_on, c->tun.n_q > 0, block);
   int64_t cap_max = cap_fitting(1, avail);
   if (cap_max < 1)
     return fail(MPLX_ERR_ALLOC, "%s: one search arena and the results (%lld bytes) exceed the budget of %lld bytes",

@@ -252,6 +252,34 @@ class env_map:
                                                         1 if dense else 0, out.ctypes.data))
         return out
 
+    def set_batch_regions(self, paths, radius, dense=False):
+        """One tunnel per query of the following plan_batch* calls (mplx_set_batch_regions): query q searches inside
+        set_search_region_path(paths[q], radius, dense)'s region, in place of the env-wide one, and those calls must
+        then have len(paths) queries.  Each path is points x Dim; an empty list clears the tunnels.  upload_map()
+        drops them, update_cells() keeps them."""
+        if len(paths) == 0:
+            abi.check(self._lib.mplx_set_batch_regions(self._h, 0, None, None, None, 0))
+            return
+        pts = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1, self.Dim) for p in paths]
+        off = np.zeros(len(pts) + 1, np.int64)
+        off[1:] = np.cumsum([len(p) for p in pts])
+        flat = np.ascontiguousarray(np.concatenate(pts) if off[-1] else np.zeros((1, self.Dim)))
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        abi.check(self._lib.mplx_set_batch_regions(self._h, len(pts), off.ctypes.data, flat.ctypes.data,
+                                                   rad.ctypes.data, 1 if dense else 0))
+
+    def batch_regions_info(self):
+        """The tunnels set_batch_regions installed: dict(n_q, n_bricks, bytes) (n_q = 0: none)."""
+        n, b, by = C.c_int32(), C.c_int64(), C.c_int64()
+        abi.check(self._lib.mplx_batch_regions_info(self._h, C.byref(n), C.byref(b), C.byref(by)))
+        return dict(n_q=n.value, n_bricks=b.value, bytes=by.value)
+
+    def read_batch_region(self, q):
+        """Query q's tunnel as one byte per voxel, set_search_region_path's layout (mplx_read_batch_region)."""
+        out = np.empty(self.map_util_.map.size, dtype=np.uint8)
+        abi.check(self._lib.mplx_read_batch_region(self._h, int(q), out.ctypes.data))
+        return out
+
     def _sync_params(self):
         if not self._dirty:
             return

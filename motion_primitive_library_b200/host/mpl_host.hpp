@@ -2858,6 +2858,17 @@ class MultiQueryPlanner {
   /// recoverTraj's edges, the device searches record the stored coordinates of the path's states
   /// (mplx_set_batch_trajectories, mplx_plan_batch_trajectories)
   void setCollectTrajectories(bool on) { collect_traj_ = on; }
+  /// One tunnel per query of the following plans (MapPlanner::setSearchRegion(paths[q], dense) with
+  /// setSearchRadius(radius) for query q alone, in place of the env's own region); an empty list clears them, and
+  /// a plan must then have paths.size() queries.  The device searches build them all at once
+  /// (mplx_set_batch_regions).  The lock-step loop (small batches, LOCKSTEP and the growing search's fallback) runs
+  /// tunnelled queries one at a time, each with its tunnel installed env-wide (set_search_region_path), and then
+  /// restores the env's region: correct, and as slow as planning the queries one by one.
+  void setSearchRegions(const std::vector<vec_E<Vecf<Dim>>> &paths, const Vecf<Dim> &radius, bool dense) {
+    region_paths_ = paths;
+    region_radius_ = radius;
+    region_dense_ = dense;
+  }
   /// a query's trajectory as PlannerBase::getTrajectory builds it: forward_action per edge
   Trajectory<Dim> trajectory(const Result &r) const {
     vec_E<Primitive<Dim>> prs;
@@ -2900,6 +2911,8 @@ class MultiQueryPlanner {
     arena_bytes_ = 0;
     grow_rounds_ = grow_lockstep_ = 0;
     grow_reruns_ = grow_first_cap_ = grow_last_cap_ = 0;
+    if (!region_paths_.empty() && region_paths_.size() != starts.size())
+      throw std::runtime_error("setSearchRegions: one path per query");
     const bool unbounded_auto =
         path_ == AUTO && max_expand <= 0 &&
         starts.size() >= (gpu_->keys_only_possible() ? kDeviceSearchMinQueries : kDeviceCostTermsMinQueries);
@@ -2917,6 +2930,7 @@ class MultiQueryPlanner {
       if (plan_device(starts, goals, eps, max_expand, true, res)) return res;
     }
     last_device_ = 0;
+    if (!region_paths_.empty()) return plan_tunnels_lockstep(starts, goals, eps, max_expand);
     // the search states of the previous plan() are recycled, not freed: a planner that answers batch
     // after batch allocates (and page-faults) its state memory once
     if (ss_.size() != starts.size()) release();
@@ -3002,6 +3016,62 @@ class MultiQueryPlanner {
     return res;
   }
 
+  /// The lock-step loop for tunnelled queries: one query at a time with its tunnel as the env's region, which is
+  /// restored afterwards.
+  std::vector<Result> plan_tunnels_lockstep(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
+                                            decimal_t eps, int max_expand) {
+    const std::size_t Q = starts.size();
+    std::vector<vec_E<Vecf<Dim>>> paths;
+    paths.swap(region_paths_);
+    const std::vector<bool> region = gpu_->search_region_;
+    const int path = path_;
+    path_ = LOCKSTEP;
+    std::vector<Result> res(Q);
+    long its = 0, nodes = 0;
+    double tp = 0, td = 0, tr = 0;
+    auto restore = [&]() {
+      path_ = path;
+      region_paths_.swap(paths);
+      gpu_->set_search_region(region);
+    };
+    try {
+      for (std::size_t q = 0; q < Q; q++) {
+        gpu_->set_search_region_path(paths[q], region_radius_, region_dense_);
+        std::vector<Result> one = plan(vec_E<Waypoint<Dim>>{starts[q]}, vec_E<Waypoint<Dim>>{goals[q]}, eps, max_expand);
+        res[q] = std::move(one[0]);
+        its += iterations_;
+        nodes += nodes_;
+        tp += t_pop_;
+        td += t_dev_;
+        tr += t_relax_;
+      }
+    } catch (...) {
+      restore();
+      throw;
+    }
+    restore();
+    iterations_ = its;
+    nodes_ = nodes;
+    t_pop_ = tp;
+    t_dev_ = td;
+    t_relax_ = tr;
+    return res;
+  }
+
+  /// The tunnels of setSearchRegions on the ctx for the next device search (cleared without them).
+  void install_tunnels() const {
+    std::vector<int64_t> off(region_paths_.size() + 1, 0);
+    std::vector<double> pts;
+    for (std::size_t q = 0; q < region_paths_.size(); q++) {
+      for (const auto &p : region_paths_[q])
+        for (int k = 0; k < Dim; k++) pts.push_back(p(k));
+      off[q + 1] = (int64_t)(pts.size() / Dim);
+    }
+    if (mplx_set_batch_regions(gpu_->ctx(), (int)region_paths_.size(), off.data(), pts.data(), region_radius_.d,
+                               region_dense_ ? 1 : 0) != MPLX_OK)
+      throw std::runtime_error(mplx_last_error());
+  }
+
   /// The queries in the device's form, with the start-is-free test run on the host map as the lock-step
   /// loop runs it (env_map.h:48-51).
   void device_queries(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
@@ -3080,6 +3150,7 @@ class MultiQueryPlanner {
     iterations_ = nodes_ = 0;
     t_pop_ = t_dev_ = t_relax_ = 0;
     gpu_->prepare_device();
+    install_tunnels();
     // sized before any result buffer exists: the host arrays below are as large as the device's
     const int fit = (cost_terms ? mplx_plan_batch_cost_terms_fits : mplx_plan_batch_fits)(
         gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
@@ -3126,6 +3197,7 @@ class MultiQueryPlanner {
     iterations_ = nodes_ = 0;
     t_pop_ = t_dev_ = t_relax_ = 0;
     gpu_->prepare_device();
+    install_tunnels();
     std::vector<mplx_waypoint> S, G;
     std::vector<uint8_t> fr;
     device_queries(starts, goals, S, G, fr);
@@ -3154,11 +3226,13 @@ class MultiQueryPlanner {
     t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     vec_E<Waypoint<Dim>> restS, restG;
     std::vector<std::size_t> rest;
+    std::vector<vec_E<Vecf<Dim>>> restP;  // their tunnels, with setSearchRegions
     for (std::size_t q = 0; q < Q; q++) {
       if (!searched[q]) {
         rest.push_back(q);
         restS.push_back(starts[q]);
         restG.push_back(goals[q]);
+        if (!region_paths_.empty()) restP.push_back(region_paths_[q]);
         continue;
       }
       take_device_result(d, q, res[q]);
@@ -3168,14 +3242,17 @@ class MultiQueryPlanner {
     if (!rest.empty()) {
       const int path = path_;
       path_ = LOCKSTEP;
+      region_paths_.swap(restP);
       std::vector<Result> sub;
       try {
         sub = plan(restS, restG, eps, max_expand);
       } catch (...) {
         path_ = path;
+        region_paths_.swap(restP);
         throw;
       }
       path_ = path;
+      region_paths_.swap(restP);
       for (std::size_t i = 0; i < rest.size(); i++) res[rest[i]] = std::move(sub[i]);
       iterations_ = nodes_ = 0;
       for (const Result &r : res) {
@@ -3225,6 +3302,9 @@ class MultiQueryPlanner {
   int path_ = AUTO;
   bool collect_closed_ = false;
   bool collect_traj_ = false;
+  std::vector<vec_E<Vecf<Dim>>> region_paths_;  // setSearchRegions
+  Vecf<Dim> region_radius_;
+  bool region_dense_ = false;
   int last_device_ = 0;  // lastDevicePath()
   int slots_ = 0;
   long long arena_bytes_ = 0;

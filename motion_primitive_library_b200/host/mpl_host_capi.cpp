@@ -441,6 +441,29 @@ int mplh_traj_sample(int dim, int n_seg, const double *seg_t, const double *coef
   });
 }
 
+/* One tunnel per query of the session's next plans (MultiQueryPlanner::setSearchRegions): query q's path is the
+ * points pts[pt_offset[q] .. pt_offset[q+1]) (dim doubles each), with one radius (dim doubles) and dense flag for
+ * all; those plans must have n_q queries.  n_q = 0 clears them.  Fails for a null session, n_q < 0, a missing array
+ * (n_q > 0), pt_offset[0] != 0 or a query with no points. */
+int mplh_batch_set_regions(void *session, int n_q, const int64_t *pt_offset, const double *pts, const double *radius,
+                           int dense) {
+  bool ok = n_q == 0 || (n_q > 0 && pt_offset && pts && radius && pt_offset[0] == 0);
+  for (int q = 0; ok && q < n_q; q++) ok = pt_offset[q + 1] > pt_offset[q];
+  return with_session(session, [&](auto &mq, BatchSession &) {
+    constexpr int Dim = mq_dim<std::decay_t<decltype(mq)>>::value;
+    std::vector<vec_E<Vecf<Dim>>> paths((std::size_t)n_q);
+    for (int q = 0; q < n_q; q++)
+      for (int64_t i = pt_offset[q]; i < pt_offset[q + 1]; i++) {
+        Vecf<Dim> p;
+        for (int k = 0; k < Dim; k++) p(k) = pts[i * Dim + k];
+        paths[(std::size_t)q].push_back(p);
+      }
+    Vecf<Dim> r;
+    for (int k = 0; k < Dim; k++) r(k) = n_q > 0 ? radius[k] : 0.0;
+    mq.setSearchRegions(paths, r, dense != 0);
+  }, ok, "null session, n_q < 0, a missing array, pt_offset[0] != 0 or a query with no points");
+}
+
 /* The session's plans also collect every query's trajectory (on = 1; 0 = off, the default), whichever path runs
  * them (MultiQueryPlanner::setCollectTrajectories), for mplh_batch_trajectories. */
 int mplh_batch_set_trajectories(void *session, int on) {

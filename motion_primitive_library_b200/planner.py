@@ -77,6 +77,7 @@ SIGNATURES = {
     "mplh_batch_last_path": ([_vp, _i32p, _i32p, _i64p], _i),
     "mplh_batch_close": ([_vp, C.POINTER(_d)], _i),
     "mplh_batch_set_trajectories": ([_vp, _i], _i),
+    "mplh_batch_set_regions": ([_vp, _i, _vp, _vp, _vp, _i], _i),
     "mplh_batch_trajectories": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64p], _i),
     "mplh_traj_solve": ([_i, _i, _i, _vp, _vp, _i, _vp, _d, _i, _i32p, _vp, _vp, _vp, _vp], _i),
     "mplh_traj_sample": ([_i, _i, _vp, _vp, _i, _i, _vp, _vp], _i),
@@ -346,6 +347,24 @@ class BatchPlanner:
         """Diagnostics: the growing device search's first and largest arena capacity in records (0 = automatic;
         see mplx_plan_batch_grow).  Queries that outgrow max_cap run through the lock-step loop."""
         self._call("mplh_batch_set_grow_caps", int(first_cap), int(max_cap))
+
+    def set_search_regions(self, paths, radius, dense=False):
+        """One tunnel per query of the following plans (MultiQueryPlanner::setSearchRegions): query q searches inside
+        MapPlanner::setSearchRegion(paths[q], dense) with the search radius `radius` (Dim metres), in place of any
+        env-wide region, and those plans must have len(paths) queries.  Each path is points x Dim; an empty list
+        clears them.  The device searches build every tunnel at once; the lock-step loop plans tunnelled queries one
+        at a time (correct, and slow)."""
+        dim = self._args.dim
+        if len(paths) == 0:
+            self._call("mplh_batch_set_regions", 0, None, None, None, 0)
+            return
+        pts = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1, dim) for p in paths]
+        off = np.zeros(len(pts) + 1, np.int64)
+        off[1:] = np.cumsum([len(p) for p in pts])
+        flat = np.ascontiguousarray(np.concatenate(pts) if off[-1] else np.zeros((1, dim)))
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        self._call("mplh_batch_set_regions", len(pts), off.ctypes.data, flat.ctypes.data, rad.ctypes.data,
+                   1 if dense else 0)
 
     def _last_path(self):
         dev, slots, nbytes = C.c_int32(0), C.c_int32(0), C.c_int64(0)
