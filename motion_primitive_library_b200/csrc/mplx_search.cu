@@ -18,10 +18,12 @@
 // the potential, gradient and yaw-alignment terms per sample in loop order (sample_group), as the register
 // and dealing kernels do, so the edge costs equal theirs bit for bit.
 //
-// Every entry point searches in rounds of one launch each (run_round).  A round searches a list of queries
-// in arenas of one capacity; a query that outgrows its arena ends in kOverflow (consume<true>), and one that
-// finishes reserves room for its closed keys and actions in a device result pool, drained after the round.
-// mplx_plan_batch and mplx_plan_batch_cost_terms run one round with worst-case arenas and a pool that holds
+// Every entry point runs through one host driver: its refusals (open_call), its device memory (size_call),
+// then search(), which runs the rounds of a Schedule (run_rounds) and hands the kept rounds to the entry point's
+// own result collection.  A round is one launch (run_round) that searches a list of queries in arenas of one
+// capacity; a query that outgrows its arena ends in kOverflow (consume<true>), and one that finishes reserves
+// room for its closed keys and actions in a device result pool, drained after the round.
+// mplx_plan_batch and mplx_plan_batch_cost_terms schedule one capacity, worst-case arenas and a pool that holds
 // every query's worst case, so none of their queries can overflow or find the pool full.  A round in
 // worst-case arenas runs the kernel without the capacity check (CHECK false), which gives the same results
 // and spills less.
@@ -30,6 +32,8 @@
 // for its path's coordinates in the trajectory room, a share of the budget rather than the worst case; one that
 // finds it full is searched again in a later round whose room holds it, so mplx_plan_batch and
 // mplx_plan_batch_cost_terms may then take more than one round.
+// Follow-up: mplx_plan_batch_grow sizes its slots by the checked kernel also in worst-case rounds, which launch
+// the unchecked one; sizing them by that kernel, as the bounded calls do, changes their slots and speed.
 #include <cuda_runtime.h>
 #include <string.h>
 
@@ -332,13 +336,6 @@ int mplx::search_budget(const mplx_ctx *c, size_t &budget) {
 }
 
 namespace {
-// With per-query tunnels set, a search call must have exactly as many queries (query q searches in tunnel q).
-int check_tunnels(const mplx_ctx *c, const char *fn, int n_q) {
-  if (c->tun.n_q > 0 && n_q != c->tun.n_q)
-    return fail(MPLX_ERR_ARG, "%s: %d queries, but mplx_set_batch_regions set %d tunnels", fn, n_q, c->tun.n_q);
-  return MPLX_OK;
-}
-
 // The trajectory room (waypoint slots) of a call with recording on, out of its budget: the size
 // mplx_set_batch_trajectories asked for, else an eighth of the budget; 0 with recording off.
 int64_t traj_room(const SearchBufs &B, size_t budget) {
@@ -353,35 +350,60 @@ int64_t worst_pool_units(int n_q, int max_expand, bool with_closed) {
   return (int64_t)n_q * ((with_closed ? max_expand : 0) + (max_expand + 1) / 2);
 }
 
-// mplx_plan_batch*'s device memory: the per-query arrays, a result pool for every query's worst case, the
-// trajectory room with recording on (troom slots) and as many worst-case arenas as fit next to them in the budget
-// (search_budget).  MPLX_ERR_ALLOC, with nothing changed, when not even one arena fits.
-int size_batch(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, bool with_closed, Layout &L,
-               int64_t &slots, int64_t &troom) {
-  const int nU = c->P.nU;
-  L = layout_for(max_expand, nU);
-  const int block = ((nU + 31) / 32) * 32;
-  size_t budget = 0;
+// the capacity of a query's next arena after it outgrew one (include/mplx.h, the round schedule)
+constexpr int64_t kGrowFactor = 4;
+
+// The rounds a call runs.  Every query starts in arenas of capacity first_cap; the ones that overflow run again with
+// kGrowFactor times the capacity, up to max_cap, and one that overflows at max_cap ends unsearched (unsearched_ok)
+// or fails the call.  A round takes min(its queries, resident, avail / arena bytes) arenas, at least one, a result
+// pool of pool_units and, with recording, the trajectory room next_room gives out of troom slots.
+struct Schedule {
+  int64_t first_cap = 0, max_cap = 0, pool_units = 0, resident = 0, troom = 0;
+  size_t avail = 0;
+  bool unsearched_ok = false;
+};
+
+// A search call's device memory: its budget (search_budget), the trajectory room with recording on (s.troom), the
+// bytes it holds next to its arenas besides the result pool (the per-query arrays, the room and the per-query
+// tunnels), and how many CTAs of the kernel it sizes by (with the capacity check or without) are resident at once.
+// s.avail: what is left for arenas next to a result pool of pool_bytes(budget).
+template <class F>
+int size_call(mplx_ctx *c, bool cost_terms, bool check, int n_q, F &&pool_bytes, Schedule &s, size_t &budget,
+              size_t &held) {
   const int rc = search_budget(c, budget);
   if (rc) return rc;
-  troom = traj_room(c->sb, budget);
-  const size_t results = (size_t)n_q * kQueryBytes +
-                         (size_t)worst_pool_units(n_q, max_expand, with_closed) * sizeof(uint64_t) +
-                         (size_t)troom * sizeof(mplx_waypoint) + c->tun.bytes();
-  slots = std::min<int64_t>(std::max(n_q, 1), (int64_t)resident_ctas(c->P, cost_terms, false, c->sb.traj_on,
-                                                                     c->tun.n_q > 0, block));
-  const size_t left = results < budget ? budget - results : 0;
-  slots = std::min<int64_t>(slots, (int64_t)(left / (size_t)L.bytes));
+  s.troom = traj_room(c->sb, budget);
+  held = (size_t)n_q * kQueryBytes + (size_t)s.troom * sizeof(mplx_waypoint) + c->tun.bytes();
+  const size_t pool = pool_bytes(budget);
+  s.avail = held + pool < budget ? budget - held - pool : 0;
+  const int block = ((c->P.nU + 31) / 32) * 32;
+  s.resident = resident_ctas(c->P, cost_terms, check, c->sb.traj_on, c->tun.n_q > 0, block);
+  return MPLX_OK;
+}
+
+// mplx_plan_batch*'s schedule: one capacity, worst-case arenas (layout L) and a result pool for every query's worst
+// case, sized by the kernel they launch; `slots` worst-case arenas fit next to the pool, at most one per query.
+// MPLX_ERR_ALLOC, with nothing changed, when not even one arena fits.
+int size_batch(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, bool with_closed, Layout &L,
+               int64_t &slots, Schedule &s) {
+  L = layout_for(max_expand, c->P.nU);
+  s.first_cap = s.max_cap = L.cap;
+  s.pool_units = worst_pool_units(n_q, max_expand, with_closed);
+  const size_t pool = (size_t)s.pool_units * sizeof(uint64_t);
+  size_t budget = 0, held = 0;
+  const int rc = size_call(c, cost_terms, false, n_q, [&](size_t) { return pool; }, s, budget, held);
+  if (rc) return rc;
+  slots = std::min<int64_t>({std::max(n_q, 1), s.resident, (int64_t)(s.avail / (size_t)L.bytes)});
   if (slots < 1)
     return fail(MPLX_ERR_ALLOC,
                 "%s: one search arena (%lld bytes) and the results (%lld bytes) exceed the budget of %lld bytes", fn,
-                (long long)L.bytes, (long long)results, (long long)budget);
+                (long long)L.bytes, (long long)(held + pool), (long long)budget);
   return MPLX_OK;
 }
 
 // The refusals of the entry points; the occupancy search (cost_terms false) also refuses the plans with
 // per-sample cost terms, and all but mplx_plan_batch_grow (unbounded_ok) an unbounded search.
-int check_plan(mplx_ctx *c, const char *fn, bool cost_terms, int max_expand, bool unbounded_ok = false) {
+int check_plan(mplx_ctx *c, const char *fn, bool cost_terms, int max_expand, bool unbounded_ok) {
   if (!c) return fail(MPLX_ERR_ARG, "%s: null ctx", fn);
   if (!c->has_map || !c->has_params) return fail(MPLX_ERR_ARG, "%s: map or params not set", fn);
   if (!cost_terms) {
@@ -391,6 +413,28 @@ int check_plan(mplx_ctx *c, const char *fn, bool cost_terms, int max_expand, boo
   }
   if (max_expand <= 0 && !unbounded_ok) return fail(MPLX_ERR_ARG, "%s: max_expand must be > 0", fn);
   if (c->P.nU > kThreads) return fail(MPLX_ERR_ARG, "%s: nU > %d", fn, kThreads);
+  return MPLX_OK;
+}
+
+// The refusals every search call makes, in the order it reports them: the plan (check_plan), the call's own
+// arguments (check_args: its out struct and its queries), the per-query tunnels (with them set, a call must have
+// exactly as many queries: query q searches in tunnel q); then the ctx binds its device.
+template <class F>
+int open_call(mplx_ctx *c, const char *fn, bool cost_terms, int max_expand, bool unbounded_ok, int n_q,
+              F &&check_args) {
+  int rc = check_plan(c, fn, cost_terms, max_expand, unbounded_ok);
+  if (rc) return rc;
+  rc = check_args();
+  if (rc) return rc;
+  if (c->tun.n_q > 0 && n_q != c->tun.n_q)
+    return fail(MPLX_ERR_ARG, "%s: %d queries, but mplx_set_batch_regions set %d tunnels", fn, n_q, c->tun.n_q);
+  return mplx_bind(c);
+}
+
+// The first refusals of a call that takes an out struct and query arrays.
+int check_queries(const char *fn, const void *out, int n_q, const mplx_waypoint *starts, const mplx_waypoint *goals) {
+  if (!out) return fail(MPLX_ERR_ARG, "%s: null out", fn);
+  if (n_q < 0 || (n_q > 0 && (!starts || !goals))) return fail(MPLX_ERR_ARG, "%s: bad query arrays", fn);
   return MPLX_OK;
 }
 
@@ -449,6 +493,11 @@ struct Round {
   int64_t tbase = 0;                      // with recording: the room's first slot in SearchBufs::traj
   double seconds = 0;  // device time of the round's launch
   int32_t at(RoundField f, int q) const { return ires[(size_t)f * cost.size() + q]; }
+  // a kDone query's closed keys (with closed keys) and then its actions, in the drained pool
+  const uint64_t *keys(int q) const { return pool.data() + offs[q]; }
+  const int32_t *actions(int q, bool with_closed) const {
+    return reinterpret_cast<const int32_t *>(keys(q) + (with_closed ? at(kNClosed, q) : 0));
+  }
 };
 
 // The trajectory room of a call's next round: what is left of the call's share (troom slots) after the slots the
@@ -604,21 +653,91 @@ void traj_begin(SearchBufs &B) {
   }
 }
 
-// The call's recorded trajectories for mplx_plan_batch_trajectories: query q has n_actions(q) action ids at
-// actions(q) and, when it has at least one, the states of its path at traj[src[q] ...].
-template <class NA, class ACT>
-void traj_publish(SearchBufs &B, int n_q, const std::vector<int64_t> &src, NA n_actions, ACT actions) {
+// What a call's rounds gave: a searched query's results are in kept[round_of[q]] (round_of -1: not searched).
+struct Searched {
+  std::vector<Round> kept;
+  std::vector<int32_t> round_of;
+  int32_t rounds = 0, slots = 0;  // launches; the first round's arena slots
+  int64_t arena_bytes = 0, last_cap = 0, reruns = 0;
+  double seconds = 0;
+};
+
+int run_rounds(mplx_ctx *c, const char *fn, const Batch &b, const Schedule &s, Searched &S) {
+  SearchBufs &B = c->sb;
+  S.round_of.assign((size_t)b.n_q, -1);
+  std::vector<int32_t> cur(b.n_q), next;
+  std::iota(cur.begin(), cur.end(), 0);
+  int64_t cap = s.first_cap;
+  int64_t again_units = 0;  // the most pool units a query of this round's list found no room for
+  int64_t again_t = 0;      // the trajectory slots the queries of this round's list found no room for
+  while (!cur.empty()) {
+    const Layout L = layout_cap(cap);
+    const int64_t slots =
+        std::max<int64_t>(1, std::min({(int64_t)cur.size(), s.resident, (int64_t)(s.avail / (size_t)L.bytes)}));
+    // a pool that holds the largest query that found it full: the first of them to reserve fits, so every
+    // round completes at least one query
+    Round R;
+    const int rc = run_round(c, b, cur, L, slots, std::max(s.pool_units, again_units),
+                             s.troom > 0 ? next_room(B, s.troom, again_t) : 0, R);
+    if (rc) return rc;
+    S.seconds += R.seconds;
+    if (S.rounds == 0) {
+      S.slots = (int32_t)slots;
+      S.arena_bytes = L.bytes;
+    }
+    S.rounds++;
+    S.last_cap = cap;
+
+    std::vector<int32_t> again;  // the result pool or the trajectory room was full: the same capacity again
+    again_units = 0;
+    again_t = 0;
+    bool keep = false;
+    for (const int32_t q : cur) {
+      const int32_t st = R.at(kState, q);
+      if (st == kDone) {
+        S.round_of[q] = (int32_t)S.kept.size();
+        keep = true;
+      } else if (st == kPoolFull) {
+        again.push_back(q);
+        again_units = std::max(again_units, (int64_t)R.offs[q]);
+        if (s.troom > 0) again_t += (int64_t)R.toffs[q];
+      } else if (cap < s.max_cap) {
+        next.push_back(q);
+      } else if (!s.unsearched_ok) {
+        return fail(MPLX_ERR_CUDA, "%s: query %d did not fit its worst-case arena and result pool", fn, q);
+      }
+    }
+    if (keep) S.kept.push_back(std::move(R));
+    S.reruns += (int64_t)again.size();
+    if (!again.empty()) {
+      cur.swap(again);
+    } else {
+      S.reruns += (int64_t)next.size();
+      cur.swap(next);
+      next.clear();
+      cap = std::min(cap * kGrowFactor, s.max_cap);
+    }
+  }
+  return MPLX_OK;
+}
+
+// The call's recorded trajectories for mplx_plan_batch_trajectories: a searched query with at least one action has
+// the states of its path in its round's room.
+void traj_publish(SearchBufs &B, const Searched &S, bool with_closed) {
   if (!B.traj_on) {
     B.traj_state = kTrajOff;
     return;
   }
+  const int n_q = (int)S.round_of.size();
   B.traj_off.assign((size_t)n_q + 1, 0);
   for (int q = 0; q < n_q; q++) {
-    const int na = n_actions(q);
+    const Round *R = S.round_of[q] < 0 ? nullptr : &S.kept[S.round_of[q]];
+    const int na = R ? R->at(kNActions, q) : 0;
     if (na > 0) {
-      const int32_t *a = actions(q);
+      const int64_t src = R->tbase + (int64_t)R->toffs[q];
+      const int32_t *a = R->actions(q, with_closed);
       for (int j = 0; j <= na; j++) {
-        B.slot_src.push_back(src[q] + j);
+        B.slot_src.push_back(src + j);
         B.slot_action.push_back(j < na ? a[j] : -1);
       }
     }
@@ -627,130 +746,101 @@ void traj_publish(SearchBufs &B, int n_q, const std::vector<int64_t> &src, NA n_
   B.traj_state = kTrajOn;
 }
 
+// The one driver of the search calls, after their refusals and sizing: uploads the queries, runs the schedule's
+// rounds, hands them to the call's `collect` and publishes the recorded trajectories.
+template <class F>
+int search(mplx_ctx *c, const char *fn, const Batch &b, const mplx_waypoint *starts, const mplx_waypoint *goals,
+           const uint8_t *start_free, const Schedule &s, F &&collect) {
+  SearchBufs &B = c->sb;
+  traj_begin(B);
+  Searched S;
+  if (b.n_q > 0) {
+    int rc = upload(c, starts, goals, start_free, b.n_q);
+    if (rc) return rc;
+    rc = run_rounds(c, fn, b, s, S);
+    if (rc) return rc;
+  }
+  const int rc = collect(S);
+  if (rc) return rc;
+  traj_publish(B, S, b.with_closed);
+  return MPLX_OK;
+}
+
 int plan_batch_fits(mplx_ctx *c, const char *fn, bool cost_terms, int n_q, int max_expand, int with_closed,
                     int32_t *slots, int64_t *arena_bytes) {
-  int rc = check_plan(c, fn, cost_terms, max_expand);
-  if (rc) return rc;
-  if (n_q < 0) return fail(MPLX_ERR_ARG, "%s: n_q < 0", fn);
-  rc = check_tunnels(c, fn, n_q);
-  if (rc) return rc;
-  rc = mplx_bind(c);
+  int rc = open_call(c, fn, cost_terms, max_expand, false, n_q,
+                     [&] { return n_q < 0 ? fail(MPLX_ERR_ARG, "%s: n_q < 0", fn) : MPLX_OK; });
   if (rc) return rc;
   Layout L;
-  int64_t s = 0, troom = 0;
-  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed != 0, L, s, troom);
+  int64_t n = 0;
+  Schedule s;
+  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed != 0, L, n, s);
   if (rc) return rc;
-  if (slots) *slots = (int32_t)s;
+  if (slots) *slots = (int32_t)n;
   if (arena_bytes) *arena_bytes = L.bytes;
   return MPLX_OK;
 }
 
+// mplx_plan_batch and mplx_plan_batch_cost_terms: one capacity, worst-case arenas and a worst-case pool, so no query
+// can overflow or find the pool full; only the queries that find the trajectory room full run again.
 int plan_batch(mplx_ctx *c, const char *fn, bool cost_terms, const mplx_waypoint *starts, const mplx_waypoint *goals,
                const uint8_t *start_free, int n_q, double eps, int max_expand, double tol_pos, double tol_vel,
                double tol_acc, double tol_yaw, mplx_batch_out *out) {
-  int rc = check_plan(c, fn, cost_terms, max_expand);
-  if (rc) return rc;
-  if (!out) return fail(MPLX_ERR_ARG, "%s: null out", fn);
-  if (n_q < 0 || (n_q > 0 && (!starts || !goals))) return fail(MPLX_ERR_ARG, "%s: bad query arrays", fn);
-  if (!out->valid || !out->cost || !out->expanded || !out->n_closed || !out->action_offset || !out->actions)
-    return fail(MPLX_ERR_ARG, "%s: missing output array", fn);
-  if (out->closed_keys && !out->closed_offset) return fail(MPLX_ERR_ARG, "%s: closed_offset missing", fn);
-  if (out->action_capacity < (int64_t)n_q * max_expand ||
-      (out->closed_keys && out->closed_capacity < (int64_t)n_q * max_expand))
-    return fail(MPLX_ERR_ARG, "%s: capacities below n_q*max_expand", fn);
-  rc = check_tunnels(c, fn, n_q);
-  if (rc) return rc;
-  rc = mplx_bind(c);
+  int rc = open_call(c, fn, cost_terms, max_expand, false, n_q, [&] {
+    if (const int rq = check_queries(fn, out, n_q, starts, goals)) return rq;
+    if (!out->valid || !out->cost || !out->expanded || !out->n_closed || !out->action_offset || !out->actions)
+      return fail(MPLX_ERR_ARG, "%s: missing output array", fn);
+    if (out->closed_keys && !out->closed_offset) return fail(MPLX_ERR_ARG, "%s: closed_offset missing", fn);
+    if (out->action_capacity < (int64_t)n_q * max_expand ||
+        (out->closed_keys && out->closed_capacity < (int64_t)n_q * max_expand))
+      return fail(MPLX_ERR_ARG, "%s: capacities below n_q*max_expand", fn);
+    return MPLX_OK;
+  });
   if (rc) return rc;
   const bool with_closed = out->closed_keys != nullptr;
   Layout L;
-  int64_t slots = 0, troom = 0;
-  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed, L, slots, troom);
+  int64_t slots = 0;
+  Schedule s;
+  rc = size_batch(c, fn, cost_terms, n_q, max_expand, with_closed, L, slots, s);
   if (rc) return rc;
-  SearchBufs &B = c->sb;
-  traj_begin(B);
   out->slots = 0;
   out->arena_bytes = 0;
   out->seconds = 0;
   out->action_offset[0] = 0;
   if (out->closed_offset) out->closed_offset[0] = 0;
-  std::vector<int64_t> tsrc(n_q, 0);
-  if (n_q == 0) {
-    traj_publish(B, 0, tsrc, [](int) { return 0; }, [](int) { return (const int32_t *)nullptr; });
-    return MPLX_OK;
-  }
-
-  rc = upload(c, starts, goals, start_free, n_q);
-  if (rc) return rc;
   const Batch b{n_q, max_expand, cost_terms, with_closed, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
-  std::vector<int32_t> cur(n_q);
-  std::iota(cur.begin(), cur.end(), 0);
-  // worst-case arenas and pool: no query can overflow or find the pool full, so one round serves every query
-  // unless the trajectory room is full; those queries run again, in a room that holds them all
-  std::vector<Round> rounds(1);
-  std::vector<int32_t> round_of(n_q, 0);
-  int64_t again_t = 0;
-  double seconds = 0;
-  for (;;) {
-    Round &R = rounds.back();
-    rc = run_round(c, b, cur, L, slots, worst_pool_units(n_q, max_expand, with_closed), troom > 0 ? next_room(B, troom, again_t) : 0, R);
-    if (rc) return rc;
-    seconds += R.seconds;
-    std::vector<int32_t> again;
-    again_t = 0;
-    for (const int32_t q : cur) {
-      const int32_t st = R.at(kState, q);
-      if (st == kDone) {
-        round_of[q] = (int32_t)rounds.size() - 1;
-        if (troom > 0) tsrc[q] = R.tbase + (int64_t)R.toffs[q];
-      } else if (troom > 0 && st == kPoolFull) {
-        again.push_back(q);
-        again_t += (int64_t)R.toffs[q];
-      } else {
-        return fail(MPLX_ERR_CUDA, "%s: query %d did not fit its worst-case arena and result pool", fn, q);
+  return search(c, fn, b, starts, goals, start_free, s, [&](const Searched &S) {
+    int64_t ao = 0, co = 0;
+    for (int q = 0; q < n_q; q++) {
+      const Round &R = S.kept[S.round_of[q]];
+      out->valid[q] = R.at(kValid, q);
+      out->cost[q] = R.cost[q];
+      out->expanded[q] = R.at(kExpanded, q);
+      const int nc = R.at(kNClosed, q);
+      out->n_closed[q] = nc;
+      const int na = R.at(kNActions, q);
+      if (na > max_expand) return fail(MPLX_ERR_ARG, "%s: query %d: trajectory longer than max_expand", fn, q);
+      // nc = expanded <= max_expand and na <= max_expand, so the compacted outputs stay within n_q*max_expand
+      const int32_t *a = R.actions(q, with_closed);
+      std::copy(a, a + na, out->actions + ao);
+      ao += na;
+      out->action_offset[q + 1] = ao;
+      if (with_closed) {
+        // the closed set's keys sorted ascending, as mplh_plan returns them (plan_capi.hpp export_result)
+        std::copy(R.keys(q), R.keys(q) + nc, out->closed_keys + co);
+        std::sort(out->closed_keys + co, out->closed_keys + co + nc);
+        co += nc;
+        out->closed_offset[q + 1] = co;
       }
     }
-    if (again.empty()) break;
-    cur.swap(again);
-    rounds.emplace_back();
-  }
-  int64_t ao = 0, co = 0;
-  for (int q = 0; q < n_q; q++) {
-    const Round &R = rounds[round_of[q]];
-    out->valid[q] = R.at(kValid, q);
-    out->cost[q] = R.cost[q];
-    out->expanded[q] = R.at(kExpanded, q);
-    const int nc = R.at(kNClosed, q);
-    out->n_closed[q] = nc;
-    const int na = R.at(kNActions, q);
-    if (na > max_expand) return fail(MPLX_ERR_ARG, "%s: query %d: trajectory longer than max_expand", fn, q);
-    // nc = expanded <= max_expand and na <= max_expand, so the compacted outputs stay within n_q*max_expand
-    const uint64_t *keys = R.pool.data() + R.offs[q];
-    const int nk = with_closed ? nc : 0;
-    const int32_t *a = reinterpret_cast<const int32_t *>(keys + nk);
-    std::copy(a, a + na, out->actions + ao);
-    ao += na;
-    out->action_offset[q + 1] = ao;
-    if (with_closed) {
-      // the closed set's keys sorted ascending, as mplh_plan returns them (plan_capi.hpp export_result)
-      std::copy(keys, keys + nk, out->closed_keys + co);
-      std::sort(out->closed_keys + co, out->closed_keys + co + nk);
-      co += nk;
-      out->closed_offset[q + 1] = co;
-    }
-  }
-  traj_publish(B, n_q, tsrc, [&](int q) { return rounds[round_of[q]].at(kNActions, q); },
-               [&](int q) { return out->actions + out->action_offset[q]; });
-  out->slots = (int32_t)slots;
-  out->arena_bytes = L.bytes;
-  out->seconds = seconds;
-  return MPLX_OK;
+    out->slots = S.slots;
+    out->arena_bytes = S.arena_bytes;
+    out->seconds = S.seconds;
+    return MPLX_OK;
+  });
 }
 
 // ---- mplx_plan_batch_grow ------------------------------------------------------------------------------
-
-// the capacity of a query's next arena after it outgrew one (include/mplx.h, the round schedule)
-constexpr int64_t kGrowFactor = 4;
 
 // The largest capacity at which `slots` arenas fit `avail` bytes (0 when not even capacity 1 does).
 int64_t cap_fitting(int64_t slots, size_t avail) {
@@ -769,149 +859,81 @@ int plan_batch_grow(mplx_ctx *c, int cost_terms, const mplx_waypoint *starts, co
                     int64_t pool_bytes, mplx_grow_out *out) {
   const char *fn = "mplx_plan_batch_grow";
   if (cost_terms != 0 && cost_terms != 1) return fail(MPLX_ERR_ARG, "%s: cost_terms must be 0 or 1", fn);
-  int rc = check_plan(c, fn, cost_terms != 0, max_expand, true);
-  if (rc) return rc;
-  if (!out) return fail(MPLX_ERR_ARG, "%s: null out", fn);
-  if (n_q < 0 || (n_q > 0 && (!starts || !goals))) return fail(MPLX_ERR_ARG, "%s: bad query arrays", fn);
-  if (!out->valid || !out->cost || !out->expanded || !out->n_closed || !out->n_actions || !out->searched)
-    return fail(MPLX_ERR_ARG, "%s: missing output array", fn);
-  if (first_cap < 0 || max_cap < 0 || pool_bytes < 0)
-    return fail(MPLX_ERR_ARG, "%s: first_cap, max_cap and pool_bytes must be >= 0", fn);
-  rc = check_tunnels(c, fn, n_q);
-  if (rc) return rc;
-  rc = mplx_bind(c);
-  if (rc) return rc;
-  const int nU = c->P.nU;
-  const int block = ((nU + 31) / 32) * 32;
   const bool ct = cost_terms != 0;
-
-  // the per-query arrays, the trajectory room and the pool's automatic size come off the budget first
-  size_t budget = 0;
-  rc = search_budget(c, budget);
+  int rc = open_call(c, fn, ct, max_expand, true, n_q, [&] {
+    if (const int rq = check_queries(fn, out, n_q, starts, goals)) return rq;
+    if (!out->valid || !out->cost || !out->expanded || !out->n_closed || !out->n_actions || !out->searched)
+      return fail(MPLX_ERR_ARG, "%s: missing output array", fn);
+    if (first_cap < 0 || max_cap < 0 || pool_bytes < 0)
+      return fail(MPLX_ERR_ARG, "%s: first_cap, max_cap and pool_bytes must be >= 0", fn);
+    return MPLX_OK;
+  });
   if (rc) return rc;
-  SearchBufs &B = c->sb;
-  const int64_t troom = traj_room(B, budget);
-  const size_t results = (size_t)n_q * kQueryBytes + (size_t)troom * sizeof(mplx_waypoint) + c->tun.bytes();
-  const size_t pool_auto = budget / 8;
-  const size_t avail = results + pool_auto < budget ? budget - results - pool_auto : 0;
-  const int64_t resident = resident_ctas(c->P, ct, true, B.traj_on, c->tun.n_q > 0, block);
-  int64_t cap_max = cap_fitting(1, avail);
-  if (cap_max < 1)
-    return fail(MPLX_ERR_ALLOC, "%s: one search arena and the results (%lld bytes) exceed the budget of %lld bytes",
-                fn, (long long)results, (long long)budget);
-  if (max_expand > 0) cap_max = std::min<int64_t>(cap_max, 1 + (int64_t)max_expand * nU);
-  if (max_cap > 0) cap_max = std::min(cap_max, max_cap);
-  int64_t cap = first_cap > 0 ? first_cap : cap_fitting(std::min<int64_t>(std::max(n_q, 1), resident), avail);
-  cap = std::max<int64_t>(1, std::min(cap, cap_max));
-  const int64_t pool_units =
-      std::max<int64_t>(1, pool_bytes > 0 ? pool_bytes / (int64_t)sizeof(uint64_t) : (int64_t)(pool_auto / 8));
 
-  traj_begin(B);
-  memset(out->valid, 0, sizeof(int32_t) * n_q);
-  memset(out->expanded, 0, sizeof(int32_t) * n_q);
-  memset(out->n_closed, 0, sizeof(int32_t) * n_q);
-  memset(out->n_actions, 0, sizeof(int32_t) * n_q);
-  memset(out->searched, 0, sizeof(int32_t) * n_q);
+  // the per-query arrays, the trajectory room and the pool's automatic size (an eighth of the budget, whatever
+  // pool_bytes is) come off the budget first; the slots of every round are those of the kernel with the capacity check
+  Schedule s;
+  size_t budget = 0, held = 0;
+  rc = size_call(c, ct, true, n_q, [](size_t total) { return total / 8; }, s, budget, held);
+  if (rc) return rc;
+  s.max_cap = cap_fitting(1, s.avail);
+  if (s.max_cap < 1)
+    return fail(MPLX_ERR_ALLOC, "%s: one search arena and the results (%lld bytes) exceed the budget of %lld bytes",
+                fn, (long long)held, (long long)budget);
+  if (max_expand > 0) s.max_cap = std::min<int64_t>(s.max_cap, 1 + (int64_t)max_expand * c->P.nU);
+  if (max_cap > 0) s.max_cap = std::min(s.max_cap, max_cap);
+  const int64_t cap =
+      first_cap > 0 ? first_cap : cap_fitting(std::min<int64_t>(std::max(n_q, 1), s.resident), s.avail);
+  s.first_cap = std::max<int64_t>(1, std::min(cap, s.max_cap));
+  s.pool_units =
+      std::max<int64_t>(1, pool_bytes > 0 ? pool_bytes / (int64_t)sizeof(uint64_t) : (int64_t)(budget / 8 / 8));
+  s.unsearched_ok = true;
+
+  for (int32_t *a : {out->valid, out->expanded, out->n_closed, out->n_actions, out->searched})
+    memset(a, 0, sizeof(int32_t) * n_q);
   for (int q = 0; q < n_q; q++) out->cost[q] = INFINITY;
   out->rounds = 0;
   out->slots = 0;
-  out->first_cap = cap;
+  out->first_cap = s.first_cap;
   out->last_cap = 0;
   out->arena_bytes = 0;
   out->reruns = 0;
   out->seconds = 0;
-  std::vector<std::vector<int32_t>> acts(n_q);
-  std::vector<std::vector<uint64_t>> keys(n_q);
-  std::vector<int64_t> tsrc(n_q, 0);
-  auto publish = [&]() {
-    traj_publish(B, n_q, tsrc, [&](int q) { return (int)acts[q].size(); }, [&](int q) { return acts[q].data(); });
+  const Batch b{n_q, max_expand, ct, with_closed != 0, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
+  SearchBufs &B = c->sb;
+  return search(c, fn, b, starts, goals, start_free, s, [&](const Searched &S) {
     B.grow_aoff.assign((size_t)n_q + 1, 0);
     B.grow_coff.assign((size_t)n_q + 1, 0);
     B.grow_actions.clear();
     B.grow_closed.clear();
     for (int q = 0; q < n_q; q++) {
-      B.grow_actions.insert(B.grow_actions.end(), acts[q].begin(), acts[q].end());
-      std::sort(keys[q].begin(), keys[q].end());
-      B.grow_closed.insert(B.grow_closed.end(), keys[q].begin(), keys[q].end());
-      B.grow_aoff[q + 1] = (int64_t)B.grow_actions.size();
-      B.grow_coff[q + 1] = (int64_t)B.grow_closed.size();
-    }
-  };
-  if (n_q == 0) {
-    publish();
-    return MPLX_OK;
-  }
-
-  rc = upload(c, starts, goals, start_free, n_q);
-  if (rc) return rc;
-  const Batch b{n_q, max_expand, ct, with_closed != 0, start_free != nullptr, eps, tol_pos, tol_vel, tol_acc, tol_yaw};
-  std::vector<int32_t> cur(n_q), next;
-  std::iota(cur.begin(), cur.end(), 0);
-  Round R;
-  double seconds = 0;
-  int32_t rounds = 0;
-  int64_t reruns = 0;
-  int64_t again_units = 0;  // the most pool units a query of this round's list found no room for
-  int64_t again_t = 0;      // the trajectory slots the queries of this round's list found no room for
-  for (;;) {
-    const Layout L = layout_cap(cap);
-    const int64_t n = (int64_t)cur.size();
-    const int64_t slots = std::max<int64_t>(1, std::min({n, resident, (int64_t)(avail / (size_t)L.bytes)}));
-    // a pool that holds the largest query that found it full: the first of them to reserve fits, so every
-    // round completes at least one query
-    rc = run_round(c, b, cur, L, slots, std::max(pool_units, again_units), troom > 0 ? next_room(B, troom, again_t) : 0, R);
-    if (rc) return rc;
-    seconds += R.seconds;
-    if (rounds == 0) {
-      out->slots = (int32_t)slots;
-      out->arena_bytes = L.bytes;
-    }
-    rounds++;
-    out->last_cap = cap;
-
-    std::vector<int32_t> again;  // the result pool was full: the same capacity again
-    again_units = 0;
-    again_t = 0;
-    for (const int32_t q : cur) {
-      const int32_t st = R.at(kState, q);
-      if (st == kDone) {
+      if (S.round_of[q] >= 0) {
+        const Round &R = S.kept[S.round_of[q]];
         out->valid[q] = R.at(kValid, q);
         out->expanded[q] = R.at(kExpanded, q);
         out->n_closed[q] = R.at(kNClosed, q);
         out->n_actions[q] = R.at(kNActions, q);
         out->cost[q] = R.cost[q];
         out->searched[q] = 1;
-        const uint64_t *k = R.pool.data() + R.offs[q];
-        const size_t nk = with_closed ? (size_t)out->n_closed[q] : 0;
-        keys[q].assign(k, k + nk);
-        const int32_t *a = reinterpret_cast<const int32_t *>(k + nk);
-        acts[q].assign(a, a + out->n_actions[q]);
-        if (troom > 0) tsrc[q] = R.tbase + (int64_t)R.toffs[q];
-      } else if (st == kPoolFull) {
-        again.push_back(q);
-        again_units = std::max(again_units, (int64_t)R.offs[q]);
-        if (troom > 0) again_t += (int64_t)R.toffs[q];
-      } else if (cap < cap_max) {
-        next.push_back(q);
-      }  // overflowed at the largest capacity: searched stays 0
+        const int32_t *a = R.actions(q, b.with_closed);
+        B.grow_actions.insert(B.grow_actions.end(), a, a + out->n_actions[q]);
+        if (b.with_closed) {
+          const size_t c0 = B.grow_closed.size();
+          B.grow_closed.insert(B.grow_closed.end(), R.keys(q), R.keys(q) + out->n_closed[q]);
+          std::sort(B.grow_closed.begin() + c0, B.grow_closed.end());
+        }
+      }
+      B.grow_aoff[q + 1] = (int64_t)B.grow_actions.size();
+      B.grow_coff[q + 1] = (int64_t)B.grow_closed.size();
     }
-    reruns += (int64_t)again.size();
-    if (!again.empty()) {
-      cur.swap(again);
-    } else if (!next.empty()) {
-      reruns += (int64_t)next.size();
-      cur.swap(next);
-      next.clear();
-      cap = std::min(cap * kGrowFactor, cap_max);
-    } else {
-      break;
-    }
-  }
-  out->rounds = rounds;
-  out->reruns = reruns;
-  out->seconds = seconds;
-  publish();
-  return MPLX_OK;
+    out->rounds = S.rounds;
+    out->slots = S.slots;
+    out->arena_bytes = S.arena_bytes;
+    out->last_cap = S.last_cap;
+    out->reruns = S.reruns;
+    out->seconds = S.seconds;
+    return MPLX_OK;
+  });
 }
 }  // namespace
 

@@ -15,7 +15,7 @@ import numpy as np
 
 from . import abi
 from .abi import LATTICE_MAX, WAYPOINT_DTYPE, PackedOut, SuccOut
-from .traj import pack_lambda, pack_paths
+from .traj import pack_lambda, pack_paths, split_slots
 
 
 class MapUtil:
@@ -504,16 +504,11 @@ class env_map:
         abi.check(self._lib.mplx_plan_batch_grow_results(self._h, aoff.ctypes.data, acts.ctypes.data, acts.size,
                                                          coff.ctypes.data, keys.ctypes.data if closed else None,
                                                          keys.size))
-        res = dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
-                   actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
-                   closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
-                   searched=searched, slots=int(out.slots), arena_bytes=int(out.arena_bytes),
-                   seconds=float(out.seconds), rounds=int(out.rounds), reruns=int(out.reruns),
-                   first_cap=int(out.first_cap), last_cap=int(out.last_cap))
-        if trajectories:
-            res["trajectories"], res["traj_seconds"] = self.batch_trajectories(
-                n_samples, sum(len(a) + 1 for a in res["actions"] if len(a)))
-        return res
+        return self._batch_result(valid, cost, expanded, n_closed, aoff, acts, coff, keys if closed else None,
+                                  trajectories, n_samples, searched=searched, slots=int(out.slots),
+                                  arena_bytes=int(out.arena_bytes), seconds=float(out.seconds),
+                                  rounds=int(out.rounds), reruns=int(out.reruns), first_cap=int(out.first_cap),
+                                  last_cap=int(out.last_cap))
 
     def _record(self, trajectories, traj_room_bytes):
         abi.check(self._lib.mplx_set_batch_trajectories(self._h, 1 if trajectories else 0, int(traj_room_bytes)))
@@ -543,15 +538,7 @@ class env_map:
                 break
             cap = int(out.total)
         abi.check(rc)
-        res = []
-        for q in range(n_q):
-            o, o1 = int(offset[q]), int(offset[q + 1])
-            s = max(o1 - o - 1, 0)
-            r = dict(nodes=nodes[o:o1].copy(), seg_t=seg_t[o:o + s].copy(), coeff=coeff[o:o + s].copy())
-            if samples is not None:
-                r["samples"] = samples[q].copy()
-            res.append(r)
-        return res, float(out.seconds)
+        return split_slots(offset, nodes, seg_t, coeff, samples), float(out.seconds)
 
     def _plan_batch(self, fn, starts, goals, eps, max_expand, tol_pos, tol_vel, tol_acc, tol_yaw, start_free, closed,
                     trajectories=False, n_samples=0, traj_room_bytes=0):
@@ -573,10 +560,17 @@ class env_map:
         abi.check(fn(self._h, starts.ctypes.data, goals.ctypes.data, abi.ptr(sf), n, float(eps), int(max_expand),
                      float(tol_pos), float(tol_vel), float(tol_acc), float(tol_yaw), C.byref(out)))
         self._last_nq = n
+        return self._batch_result(valid, cost, expanded, n_closed, aoff, acts, coff, keys, trajectories, n_samples,
+                                  slots=int(out.slots), arena_bytes=int(out.arena_bytes), seconds=float(out.seconds))
+
+    def _batch_result(self, valid, cost, expanded, n_closed, aoff, acts, coff, keys, trajectories, n_samples,
+                      **extra):
+        """The results dict of the plan_batch* calls: the per-query arrays, the actions and closed lists (keys None:
+        closed None), the call's own fields (extra) and, with trajectories, `trajectories` and `traj_seconds`."""
+        n = valid.size
         res = dict(valid=valid, cost=cost, expanded=expanded, n_closed=n_closed,
                    actions=[acts[aoff[q]:aoff[q + 1]].copy() for q in range(n)],
-                   closed=[keys[coff[q]:coff[q + 1]].copy() for q in range(n)] if closed else None,
-                   slots=int(out.slots), arena_bytes=int(out.arena_bytes), seconds=float(out.seconds))
+                   closed=None if keys is None else [keys[coff[q]:coff[q + 1]].copy() for q in range(n)], **extra)
         if trajectories:
             res["trajectories"], res["traj_seconds"] = self.batch_trajectories(
                 n_samples, sum(len(a) + 1 for a in res["actions"] if len(a)))

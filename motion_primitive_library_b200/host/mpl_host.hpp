@@ -2916,21 +2916,254 @@ class MultiQueryPlanner {
     const bool unbounded_auto =
         path_ == AUTO && max_expand <= 0 &&
         starts.size() >= (gpu_->keys_only_possible() ? kDeviceSearchMinQueries : kDeviceCostTermsMinQueries);
+    int device = 0;  // lastDevicePath() of the device search that serves the plan, 0 for none
     if ((path_ == DEVICE_GROW || unbounded_auto) && gpu_->U_.size() <= 256) {
-      std::vector<Result> res;
-      if (plan_grow(starts, goals, eps, max_expand, res)) return res;
+      device = 3;
     } else if ((path_ == AUTO || path_ == DEVICE) && deviceSearchPossible(max_expand) &&
         (path_ == DEVICE || starts.size() >= kDeviceSearchMinQueries)) {
-      std::vector<Result> res;
-      if (plan_device(starts, goals, eps, max_expand, false, res)) return res;
+      device = 1;
     } else if (costTermsSearchPossible(max_expand) &&
                (path_ == DEVICE_COST_TERMS ||
                 (path_ == AUTO && !gpu_->keys_only_possible() && starts.size() >= kDeviceCostTermsMinQueries))) {
+      device = 2;
+    }
+    if (device) {
       std::vector<Result> res;
-      if (plan_device(starts, goals, eps, max_expand, true, res)) return res;
+      if (plan_device(starts, goals, eps, max_expand, device, res)) return res;
     }
     last_device_ = 0;
-    if (!region_paths_.empty()) return plan_tunnels_lockstep(starts, goals, eps, max_expand);
+    return plan_lockstep(starts, goals, eps, max_expand, region_paths_);
+  }
+
+  /// The tunnels of setSearchRegions on the ctx for the next device search (cleared without them).
+  void install_tunnels() const {
+    std::vector<int64_t> off(region_paths_.size() + 1, 0);
+    std::vector<double> pts;
+    for (std::size_t q = 0; q < region_paths_.size(); q++) {
+      for (const auto &p : region_paths_[q])
+        for (int k = 0; k < Dim; k++) pts.push_back(p(k));
+      off[q + 1] = (int64_t)(pts.size() / Dim);
+    }
+    if (mplx_set_batch_regions(gpu_->ctx(), (int)region_paths_.size(), off.data(), pts.data(), region_radius_.d,
+                               region_dense_ ? 1 : 0) != MPLX_OK)
+      throw std::runtime_error(mplx_last_error());
+  }
+
+  /// The queries in the device's form, with the start-is-free test run on the host map as the lock-step
+  /// loop runs it (env_map.h:48-51).
+  void device_queries(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
+                      std::vector<mplx_waypoint> &S, std::vector<mplx_waypoint> &G, std::vector<uint8_t> &fr) const {
+    const std::size_t Q = starts.size();
+    S.resize(Q);
+    G.resize(Q);
+    fr.resize(Q);
+    for (std::size_t q = 0; q < Q; q++) {
+      S[q] = env_map_gpu<Dim>::pod(starts[q]);
+      G[q] = env_map_gpu<Dim>::pod(goals[q]);
+      fr[q] = map_util_->isFree(map_util_->floatToInt(starts[q].pos)) ? 1 : 0;
+    }
+  }
+
+  /// A device search's per-query results; query q's trajectory is acts[aoff[q], aoff[q+1]) and its closed
+  /// keys are keys[coff[q], coff[q+1]).
+  struct DeviceOut {
+    std::vector<int32_t> valid, expd, ncl, acts;
+    std::vector<double> cost;
+    std::vector<int64_t> aoff, coff;
+    std::vector<uint64_t> keys;
+    explicit DeviceOut(std::size_t Q) : valid(Q), expd(Q), ncl(Q), cost(Q), aoff(Q + 1), coff(Q + 1) {}
+  };
+
+  /// Query q's result from a device search, its expansions counted in iterations_ and nodes_.
+  void take_device_result(const DeviceOut &d, std::size_t q, Result &r) {
+    r.valid = d.valid[q] != 0;
+    r.cost = d.cost[q];
+    r.expanded = d.expd[q];
+    r.n_closed = (std::size_t)d.ncl[q];
+    r.actions.assign(d.acts.begin() + d.aoff[q], d.acts.begin() + d.aoff[q + 1]);
+    if (collect_closed_) r.closed_keys.assign(d.keys.begin() + d.coff[q], d.keys.begin() + d.coff[q + 1]);
+    iterations_ = std::max<long>(iterations_, d.expd[q]);
+    nodes_ += d.expd[q];
+  }
+
+  /// Trajectory recording for the next device search on the ctx: on with setCollectTrajectories(true).
+  void record_trajectories() const {
+    if (mplx_set_batch_trajectories(gpu_->ctx(), collect_traj_ ? 1 : 0, 0) != MPLX_OK)
+      throw std::runtime_error(mplx_last_error());
+  }
+
+  /// Result::traj / traj_end of the queries the last device search gave a trajectory (res[q].actions set), from
+  /// the stored coordinates it recorded (mplx_plan_batch_trajectories).
+  void take_device_trajectories(std::vector<Result> &res) const {
+    const std::size_t Q = res.size();
+    int64_t cap = 0;
+    for (const Result &r : res)
+      if (!r.actions.empty()) cap += (int64_t)r.actions.size() + 1;
+    cap = std::max<int64_t>(cap, 1);
+    std::vector<int64_t> off(Q + 1);
+    std::vector<mplx_waypoint> nodes((std::size_t)cap);
+    std::vector<double> seg((std::size_t)cap), coeff((std::size_t)cap * (Dim + 1) * 6);
+    mplx_batch_traj_out out{off.data(), nodes.data(), seg.data(), coeff.data(), nullptr, cap, 0, 0.0};
+    if (mplx_plan_batch_trajectories(gpu_->ctx(), 0, &out) != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    for (std::size_t q = 0; q < Q; q++) {
+      const int64_t n = off[q + 1] - off[q];
+      if (n == 0) continue;
+      if (n != (int64_t)res[q].actions.size() + 1) throw std::runtime_error("device trajectory length mismatch");
+      for (int64_t j = 0; j + 1 < n; j++)
+        res[q].traj.push_back(Edge<Dim>{gpu_->unpod(nodes[(std::size_t)(off[q] + j)]), res[q].actions[(std::size_t)j]});
+      res[q].traj_end = gpu_->unpod(nodes[(std::size_t)(off[q] + n - 1)]);
+    }
+  }
+
+  /// plan() on the device: every query's whole A* in one call of the device search `path` (lastDevicePath():
+  /// 1 = mplx_plan_batch, 2 = mplx_plan_batch_cost_terms, 3 = mplx_plan_batch_grow, cost_terms for every plan that
+  /// is not occupancy planning).  The start-is-free test runs here on the host map, as in the lock-step loop.  The
+  /// queries the growing search could not fit in its largest arena (searched = 0) run through the lock-step loop,
+  /// and their results are merged.  Returns false, with nothing planned, when the search memory does not fit the
+  /// device-memory budget (MPLX_ERR_ALLOC: the worst-case arenas, or for the growing search a one-record arena)
+  /// under AUTO: the caller then runs the lock-step loop, which served such plans before.  The forced paths report
+  /// it as an error.
+  bool plan_device(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
+                   int max_expand, int path, std::vector<Result> &res) {
+    const std::size_t Q = starts.size();
+    const bool grow = path == 3;
+    res.assign(Q, Result());
+    iterations_ = nodes_ = 0;
+    t_pop_ = t_dev_ = t_relax_ = 0;
+    gpu_->prepare_device();
+    install_tunnels();
+    DeviceOut d(Q);
+    if (!grow) {
+      // sized before any result buffer exists: the host arrays below are as large as the device's
+      const int fit = (path == 2 ? mplx_plan_batch_cost_terms_fits : mplx_plan_batch_fits)(
+          gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
+      if (fit == MPLX_ERR_ALLOC && path_ == AUTO) return false;
+      if (fit != MPLX_OK) throw std::runtime_error(mplx_last_error());
+      last_device_ = path;
+      if (Q == 0) return true;
+      d.acts.resize(Q * (std::size_t)max_expand);
+      d.keys.resize(collect_closed_ ? Q * (std::size_t)max_expand : 0);
+    }
+    std::vector<mplx_waypoint> S, G;
+    std::vector<uint8_t> fr;
+    device_queries(starts, goals, S, G, fr);
+    std::vector<int32_t> nact(Q), searched(Q, 1);
+    mplx_batch_out out{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), d.aoff.data(), d.acts.data(),
+                       (int64_t)d.acts.size(), collect_closed_ ? d.coff.data() : nullptr,
+                       collect_closed_ ? d.keys.data() : nullptr, (int64_t)d.keys.size(), 0, 0, 0.0};
+    mplx_grow_out gout{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), nact.data(), searched.data(), 0, 0, 0,
+                       0, 0, 0, 0.0};
+    record_trajectories();
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc =
+        grow ? mplx_plan_batch_grow(gpu_->ctx(), gpu_->keys_only_possible() ? 0 : 1, S.data(), G.data(), fr.data(),
+                                    (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_, gpu_->tol_acc_,
+                                    gpu_->tol_yaw_, collect_closed_ ? 1 : 0, grow_first_cap_set_, grow_max_cap_set_, 0,
+                                    &gout)
+             : (path == 2 ? mplx_plan_batch_cost_terms : mplx_plan_batch)(
+                   gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_,
+                   gpu_->tol_vel_, gpu_->tol_acc_, gpu_->tol_yaw_, &out);
+    // the device allocation itself can still fail when other users of the card took memory in between
+    if (rc == MPLX_ERR_ALLOC && path_ == AUTO) {
+      last_device_ = 0;
+      return false;
+    }
+    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
+    if (grow) {
+      int64_t na = 0, nc = 0;
+      for (std::size_t q = 0; q < Q; q++) {
+        na += nact[q];
+        nc += collect_closed_ ? d.ncl[q] : 0;
+      }
+      d.acts.resize(std::max<int64_t>(na, 1));
+      d.keys.resize(std::max<int64_t>(nc, 1));
+      if (mplx_plan_batch_grow_results(gpu_->ctx(), d.aoff.data(), d.acts.data(), (int64_t)d.acts.size(),
+                                       d.coff.data(), collect_closed_ ? d.keys.data() : nullptr,
+                                       (int64_t)d.keys.size()) != MPLX_OK)
+        throw std::runtime_error(mplx_last_error());
+    }
+    t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    vec_E<Waypoint<Dim>> restS, restG;
+    std::vector<std::size_t> rest;
+    std::vector<vec_E<Vecf<Dim>>> restP;  // their tunnels, with setSearchRegions
+    for (std::size_t q = 0; q < Q; q++) {
+      if (searched[q]) {
+        take_device_result(d, q, res[q]);
+        continue;
+      }
+      rest.push_back(q);
+      restS.push_back(starts[q]);
+      restG.push_back(goals[q]);
+      if (!region_paths_.empty()) restP.push_back(region_paths_[q]);
+    }
+    // the device's trajectories before the lock-step loop takes the rest (unsearched queries have none)
+    if (collect_traj_) take_device_trajectories(res);
+    if (!rest.empty()) {
+      std::vector<Result> sub = plan_lockstep(restS, restG, eps, max_expand, restP);
+      for (std::size_t i = 0; i < rest.size(); i++) res[rest[i]] = std::move(sub[i]);
+      iterations_ = nodes_ = 0;
+      for (const Result &r : res) {
+        iterations_ = std::max<long>(iterations_, r.expanded);
+        nodes_ += r.expanded;
+      }
+    }
+    last_device_ = path;
+    slots_ = grow ? gout.slots : out.slots;
+    arena_bytes_ = grow ? gout.arena_bytes : out.arena_bytes;
+    if (grow) {
+      grow_rounds_ = gout.rounds;
+      grow_reruns_ = gout.reruns;
+      grow_first_cap_ = gout.first_cap;
+      grow_last_cap_ = gout.last_cap;
+      grow_lockstep_ = (int)rest.size();
+    }
+    return true;
+  }
+  /// Free the search states of the last plan() (tens of millions of states for a large batch), on
+  /// the host cores.  Called by the next plan() and the destructor.
+  void release() {
+    if (ss_.empty()) return;
+    WorkerPool pool(host_threads_ > 0 ? host_threads_ : effective_cpus());
+    pool.run(ss_.size(), [&](std::size_t q) {
+      st_[q].reset();
+      ss_[q].reset();
+      envs_[q].reset();
+    });
+    st_.clear(); ss_.clear(); envs_.clear();
+  }
+  ~MultiQueryPlanner() { release(); }
+
+ private:
+  /// The lock-step loop over the queries.  With tunnels (one path per query; empty for none) it runs one query at a
+  /// time with its tunnel as the env's region, and the env's own region comes back however the loop ends.
+  std::vector<Result> plan_lockstep(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
+                                    decimal_t eps, int max_expand, const std::vector<vec_E<Vecf<Dim>>> &tunnels) {
+    if (!tunnels.empty()) {
+      struct RestoreRegion {
+        env_map_gpu<Dim> &gpu;
+        const std::vector<bool> region;
+        ~RestoreRegion() { gpu.set_search_region(region); }
+      } restore{*gpu_, gpu_->search_region_};
+      std::vector<Result> res(starts.size());
+      long its = 0, nodes = 0;
+      double tp = 0, td = 0, tr = 0;
+      for (std::size_t q = 0; q < starts.size(); q++) {
+        gpu_->set_search_region_path(tunnels[q], region_radius_, region_dense_);
+        res[q] = std::move(plan_lockstep(vec_E<Waypoint<Dim>>{starts[q]}, vec_E<Waypoint<Dim>>{goals[q]}, eps,
+                                         max_expand, {})[0]);
+        its += iterations_;
+        nodes += nodes_;
+        tp += t_pop_;
+        td += t_dev_;
+        tr += t_relax_;
+      }
+      iterations_ = its;
+      nodes_ = nodes;
+      t_pop_ = tp;
+      t_dev_ = td;
+      t_relax_ = tr;
+      return res;
+    }
     // the search states of the previous plan() are recycled, not freed: a planner that answers batch
     // after batch allocates (and page-faults) its state memory once
     if (ss_.size() != starts.size()) release();
@@ -3016,275 +3249,7 @@ class MultiQueryPlanner {
     return res;
   }
 
-  /// The lock-step loop for tunnelled queries: one query at a time with its tunnel as the env's region, which is
-  /// restored afterwards.
-  std::vector<Result> plan_tunnels_lockstep(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
-                                            decimal_t eps, int max_expand) {
-    const std::size_t Q = starts.size();
-    std::vector<vec_E<Vecf<Dim>>> paths;
-    paths.swap(region_paths_);
-    const std::vector<bool> region = gpu_->search_region_;
-    const int path = path_;
-    path_ = LOCKSTEP;
-    std::vector<Result> res(Q);
-    long its = 0, nodes = 0;
-    double tp = 0, td = 0, tr = 0;
-    auto restore = [&]() {
-      path_ = path;
-      region_paths_.swap(paths);
-      gpu_->set_search_region(region);
-    };
-    try {
-      for (std::size_t q = 0; q < Q; q++) {
-        gpu_->set_search_region_path(paths[q], region_radius_, region_dense_);
-        std::vector<Result> one = plan(vec_E<Waypoint<Dim>>{starts[q]}, vec_E<Waypoint<Dim>>{goals[q]}, eps, max_expand);
-        res[q] = std::move(one[0]);
-        its += iterations_;
-        nodes += nodes_;
-        tp += t_pop_;
-        td += t_dev_;
-        tr += t_relax_;
-      }
-    } catch (...) {
-      restore();
-      throw;
-    }
-    restore();
-    iterations_ = its;
-    nodes_ = nodes;
-    t_pop_ = tp;
-    t_dev_ = td;
-    t_relax_ = tr;
-    return res;
-  }
 
-  /// The tunnels of setSearchRegions on the ctx for the next device search (cleared without them).
-  void install_tunnels() const {
-    std::vector<int64_t> off(region_paths_.size() + 1, 0);
-    std::vector<double> pts;
-    for (std::size_t q = 0; q < region_paths_.size(); q++) {
-      for (const auto &p : region_paths_[q])
-        for (int k = 0; k < Dim; k++) pts.push_back(p(k));
-      off[q + 1] = (int64_t)(pts.size() / Dim);
-    }
-    if (mplx_set_batch_regions(gpu_->ctx(), (int)region_paths_.size(), off.data(), pts.data(), region_radius_.d,
-                               region_dense_ ? 1 : 0) != MPLX_OK)
-      throw std::runtime_error(mplx_last_error());
-  }
-
-  /// The queries in the device's form, with the start-is-free test run on the host map as the lock-step
-  /// loop runs it (env_map.h:48-51).
-  void device_queries(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
-                      std::vector<mplx_waypoint> &S, std::vector<mplx_waypoint> &G, std::vector<uint8_t> &fr) const {
-    const std::size_t Q = starts.size();
-    S.resize(Q);
-    G.resize(Q);
-    fr.resize(Q);
-    for (std::size_t q = 0; q < Q; q++) {
-      S[q] = env_map_gpu<Dim>::pod(starts[q]);
-      G[q] = env_map_gpu<Dim>::pod(goals[q]);
-      fr[q] = map_util_->isFree(map_util_->floatToInt(starts[q].pos)) ? 1 : 0;
-    }
-  }
-
-  /// A device search's per-query results; query q's trajectory is acts[aoff[q], aoff[q+1]) and its closed
-  /// keys are keys[coff[q], coff[q+1]).
-  struct DeviceOut {
-    std::vector<int32_t> valid, expd, ncl, acts;
-    std::vector<double> cost;
-    std::vector<int64_t> aoff, coff;
-    std::vector<uint64_t> keys;
-    explicit DeviceOut(std::size_t Q) : valid(Q), expd(Q), ncl(Q), cost(Q), aoff(Q + 1), coff(Q + 1) {}
-  };
-
-  /// Query q's result from a device search, its expansions counted in iterations_ and nodes_.
-  void take_device_result(const DeviceOut &d, std::size_t q, Result &r) {
-    r.valid = d.valid[q] != 0;
-    r.cost = d.cost[q];
-    r.expanded = d.expd[q];
-    r.n_closed = (std::size_t)d.ncl[q];
-    r.actions.assign(d.acts.begin() + d.aoff[q], d.acts.begin() + d.aoff[q + 1]);
-    if (collect_closed_) r.closed_keys.assign(d.keys.begin() + d.coff[q], d.keys.begin() + d.coff[q + 1]);
-    iterations_ = std::max<long>(iterations_, d.expd[q]);
-    nodes_ += d.expd[q];
-  }
-
-  /// Trajectory recording for the next device search on the ctx: on with setCollectTrajectories(true).
-  void record_trajectories() const {
-    if (mplx_set_batch_trajectories(gpu_->ctx(), collect_traj_ ? 1 : 0, 0) != MPLX_OK)
-      throw std::runtime_error(mplx_last_error());
-  }
-
-  /// Result::traj / traj_end of the queries the last device search gave a trajectory (res[q].actions set), from
-  /// the stored coordinates it recorded (mplx_plan_batch_trajectories).
-  void take_device_trajectories(std::vector<Result> &res) const {
-    const std::size_t Q = res.size();
-    int64_t cap = 0;
-    for (const Result &r : res)
-      if (!r.actions.empty()) cap += (int64_t)r.actions.size() + 1;
-    cap = std::max<int64_t>(cap, 1);
-    std::vector<int64_t> off(Q + 1);
-    std::vector<mplx_waypoint> nodes((std::size_t)cap);
-    std::vector<double> seg((std::size_t)cap), coeff((std::size_t)cap * (Dim + 1) * 6);
-    mplx_batch_traj_out out{off.data(), nodes.data(), seg.data(), coeff.data(), nullptr, cap, 0, 0.0};
-    if (mplx_plan_batch_trajectories(gpu_->ctx(), 0, &out) != MPLX_OK) throw std::runtime_error(mplx_last_error());
-    for (std::size_t q = 0; q < Q; q++) {
-      const int64_t n = off[q + 1] - off[q];
-      if (n == 0) continue;
-      if (n != (int64_t)res[q].actions.size() + 1) throw std::runtime_error("device trajectory length mismatch");
-      for (int64_t j = 0; j + 1 < n; j++)
-        res[q].traj.push_back(Edge<Dim>{gpu_->unpod(nodes[(std::size_t)(off[q] + j)]), res[q].actions[(std::size_t)j]});
-      res[q].traj_end = gpu_->unpod(nodes[(std::size_t)(off[q] + n - 1)]);
-    }
-  }
-
-  /// plan() on the device: every query's whole A* in one mplx_plan_batch call (cost_terms:
-  /// mplx_plan_batch_cost_terms).  The start-is-free test runs here on the host map, as in the lock-step
-  /// loop.  Returns false, with nothing planned, when the worst-case search memory does not fit the
-  /// device-memory budget (MPLX_ERR_ALLOC) under AUTO: the caller then runs the lock-step loop, which
-  /// served such plans before.  DEVICE and DEVICE_COST_TERMS report it as an error.
-  bool plan_device(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
-                   int max_expand, bool cost_terms, std::vector<Result> &res) {
-    const std::size_t Q = starts.size();
-    res.assign(Q, Result());
-    iterations_ = nodes_ = 0;
-    t_pop_ = t_dev_ = t_relax_ = 0;
-    gpu_->prepare_device();
-    install_tunnels();
-    // sized before any result buffer exists: the host arrays below are as large as the device's
-    const int fit = (cost_terms ? mplx_plan_batch_cost_terms_fits : mplx_plan_batch_fits)(
-        gpu_->ctx(), (int)Q, max_expand, collect_closed_ ? 1 : 0, nullptr, nullptr);
-    if (fit == MPLX_ERR_ALLOC && path_ == AUTO) return false;
-    if (fit != MPLX_OK) throw std::runtime_error(mplx_last_error());
-    last_device_ = cost_terms ? 2 : 1;
-    if (Q == 0) return true;
-    std::vector<mplx_waypoint> S, G;
-    std::vector<uint8_t> fr;
-    device_queries(starts, goals, S, G, fr);
-    DeviceOut d(Q);
-    d.acts.resize(Q * (std::size_t)max_expand);
-    d.keys.resize(collect_closed_ ? Q * (std::size_t)max_expand : 0);
-    mplx_batch_out out{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), d.aoff.data(), d.acts.data(),
-                       (int64_t)d.acts.size(), collect_closed_ ? d.coff.data() : nullptr,
-                       collect_closed_ ? d.keys.data() : nullptr, (int64_t)d.keys.size(), 0, 0, 0.0};
-    record_trajectories();
-    const auto t0 = std::chrono::steady_clock::now();
-    const int rc = (cost_terms ? mplx_plan_batch_cost_terms : mplx_plan_batch)(
-        gpu_->ctx(), S.data(), G.data(), fr.data(), (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_,
-        gpu_->tol_acc_, gpu_->tol_yaw_, &out);
-    // the device allocation itself can still fail when other users of the card took memory in between
-    if (rc == MPLX_ERR_ALLOC && path_ == AUTO) {
-      last_device_ = 0;
-      return false;
-    }
-    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
-    t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    slots_ = out.slots;
-    arena_bytes_ = out.arena_bytes;
-    for (std::size_t q = 0; q < Q; q++) take_device_result(d, q, res[q]);
-    if (collect_traj_) take_device_trajectories(res);
-    return true;
-  }
-
-  /// plan() with the growing device search (mplx_plan_batch_grow; cost_terms for every plan that is not
-  /// occupancy planning).  The queries it could not fit in its largest arena (searched = 0) run through the
-  /// lock-step loop, and their results are merged.  Returns false, with nothing planned, when not even a
-  /// one-record arena fits the budget under AUTO; DEVICE_GROW reports that as an error.
-  bool plan_grow(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
-                 int max_expand, std::vector<Result> &res) {
-    const std::size_t Q = starts.size();
-    res.assign(Q, Result());
-    iterations_ = nodes_ = 0;
-    t_pop_ = t_dev_ = t_relax_ = 0;
-    gpu_->prepare_device();
-    install_tunnels();
-    std::vector<mplx_waypoint> S, G;
-    std::vector<uint8_t> fr;
-    device_queries(starts, goals, S, G, fr);
-    DeviceOut d(Q);
-    std::vector<int32_t> nact(Q), searched(Q);
-    mplx_grow_out out{d.valid.data(), d.cost.data(), d.expd.data(), d.ncl.data(), nact.data(), searched.data(), 0, 0, 0,
-                      0, 0, 0, 0.0};
-    record_trajectories();
-    const auto t0 = std::chrono::steady_clock::now();
-    const int rc = mplx_plan_batch_grow(gpu_->ctx(), gpu_->keys_only_possible() ? 0 : 1, S.data(), G.data(), fr.data(),
-                                        (int)Q, eps, max_expand, gpu_->tol_pos_, gpu_->tol_vel_, gpu_->tol_acc_,
-                                        gpu_->tol_yaw_, collect_closed_ ? 1 : 0, grow_first_cap_set_, grow_max_cap_set_,
-                                        0, &out);
-    if (rc == MPLX_ERR_ALLOC && path_ == AUTO) return false;
-    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
-    int64_t na = 0, nc = 0;
-    for (std::size_t q = 0; q < Q; q++) {
-      na += nact[q];
-      nc += collect_closed_ ? d.ncl[q] : 0;
-    }
-    d.acts.resize(std::max<int64_t>(na, 1));
-    d.keys.resize(std::max<int64_t>(nc, 1));
-    if (mplx_plan_batch_grow_results(gpu_->ctx(), d.aoff.data(), d.acts.data(), (int64_t)d.acts.size(), d.coff.data(),
-                                     collect_closed_ ? d.keys.data() : nullptr, (int64_t)d.keys.size()) != MPLX_OK)
-      throw std::runtime_error(mplx_last_error());
-    t_dev_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    vec_E<Waypoint<Dim>> restS, restG;
-    std::vector<std::size_t> rest;
-    std::vector<vec_E<Vecf<Dim>>> restP;  // their tunnels, with setSearchRegions
-    for (std::size_t q = 0; q < Q; q++) {
-      if (!searched[q]) {
-        rest.push_back(q);
-        restS.push_back(starts[q]);
-        restG.push_back(goals[q]);
-        if (!region_paths_.empty()) restP.push_back(region_paths_[q]);
-        continue;
-      }
-      take_device_result(d, q, res[q]);
-    }
-    // the device's trajectories before the lock-step loop takes the rest (unsearched queries have none)
-    if (collect_traj_) take_device_trajectories(res);
-    if (!rest.empty()) {
-      const int path = path_;
-      path_ = LOCKSTEP;
-      region_paths_.swap(restP);
-      std::vector<Result> sub;
-      try {
-        sub = plan(restS, restG, eps, max_expand);
-      } catch (...) {
-        path_ = path;
-        region_paths_.swap(restP);
-        throw;
-      }
-      path_ = path;
-      region_paths_.swap(restP);
-      for (std::size_t i = 0; i < rest.size(); i++) res[rest[i]] = std::move(sub[i]);
-      iterations_ = nodes_ = 0;
-      for (const Result &r : res) {
-        iterations_ = std::max<long>(iterations_, r.expanded);
-        nodes_ += r.expanded;
-      }
-    }
-    last_device_ = 3;
-    slots_ = out.slots;
-    arena_bytes_ = out.arena_bytes;
-    grow_rounds_ = out.rounds;
-    grow_reruns_ = out.reruns;
-    grow_first_cap_ = out.first_cap;
-    grow_last_cap_ = out.last_cap;
-    grow_lockstep_ = (int)rest.size();
-    return true;
-  }
-  /// Free the search states of the last plan() (tens of millions of states for a large batch), on
-  /// the host cores.  Called by the next plan() and the destructor.
-  void release() {
-    if (ss_.empty()) return;
-    WorkerPool pool(host_threads_ > 0 ? host_threads_ : effective_cpus());
-    pool.run(ss_.size(), [&](std::size_t q) {
-      st_[q].reset();
-      ss_[q].reset();
-      envs_[q].reset();
-    });
-    st_.clear(); ss_.clear(); envs_.clear();
-  }
-  ~MultiQueryPlanner() { release(); }
-
- private:
   // per-query host env: goal test + heuristic only (its get_succ is never called)
   struct QueryEnv : env_map_host<Dim> {
     using env_map_host<Dim>::env_map_host;

@@ -6,7 +6,9 @@ from pathlib import Path
 
 import numpy as np
 
-PKG = Path(__file__).resolve().parent
+from .traj import split_slots
+
+PKG =Path(__file__).resolve().parent
 LIB = PKG / "lib" / "libmpl_host.so"
 
 class Waypoint(C.Structure):
@@ -431,15 +433,7 @@ class BatchPlanner:
         samples = np.zeros((nq, n_samples + 1, 4 * dim + 3)) if n_samples > 0 else None
         self._call("mplh_batch_trajectories", int(n_samples), offset.ctypes.data, nodes.ctypes.data, seg_t.ctypes.data,
                    coeff.ctypes.data, None if samples is None else samples.ctypes.data, cap, C.byref(total))
-        res = []
-        for q in range(nq):
-            o, o1 = int(offset[q]), int(offset[q + 1])
-            s = max(o1 - o - 1, 0)
-            r = dict(nodes=nodes[o:o1].copy(), seg_t=seg_t[o:o + s].copy(), coeff=coeff[o:o + s].copy())
-            if samples is not None:
-                r["samples"] = samples[q].copy()
-            res.append(r)
-        return res
+        return split_slots(offset, nodes, seg_t, coeff, samples)
 
     def _totals(self, totals):
         t = dict(iterations=int(totals[0]), nodes=int(totals[1]), seconds=float(totals[2]), t_pop=float(totals[3]),

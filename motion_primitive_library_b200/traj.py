@@ -28,6 +28,20 @@ def pack_paths(results, dim):
     return n, offset, seg_t, coeff
 
 
+def split_slots(offset, nodes, seg_t, coeff, samples=None):
+    """The inverse of pack_paths for mplx_batch_traj_out's layout: one dict per path with `nodes` (the path's
+    waypoint slots), `seg_t` and `coeff` (one entry per segment) and, when samples is given, `samples` (its rows)."""
+    res = []
+    for q in range(len(offset) - 1):
+        o, o1 = int(offset[q]), int(offset[q + 1])
+        s = max(o1 - o - 1, 0)
+        r = dict(nodes=nodes[o:o1].copy(), seg_t=seg_t[o:o + s].copy(), coeff=coeff[o:o + s].copy())
+        if samples is not None:
+            r["samples"] = samples[q].copy()
+        res.append(r)
+    return res
+
+
 def pack_lambda(scaled, offset, dim):
     """total_t, n_lambda and the lambda slots (mplx_traj_scale_out's layout) of TrajSolverBatch.scale's results
     (with_lambda=True) for the paths at `offset`."""
