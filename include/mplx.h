@@ -424,6 +424,26 @@ int mplx_plan_batch_trajectories(mplx_ctx *ctx, int n_samples, mplx_batch_traj_o
 int mplx_set_batch_regions(mplx_ctx *ctx, int n_q, const int64_t *pt_offset, const double *pts, const double *radius,
                            int dense);
 
+/* mplx_set_batch_regions with paths the last search call recorded, so that a replanning loop (MapPlanner::
+ * iterativePlan) builds each round's tunnels without bringing the paths to the host: query j's tunnel is
+ * MapPlanner<Dim>::setSearchRegion(path, dense) where path is, for from[j] >= 0, the recorded path of query from[j]
+ * of the last mplx_plan_batch / _cost_terms / _grow call (the positions of its stored path states from start to
+ * goal, the nodes mplx_plan_batch_trajectories returns and MapPlanner::getWaypointPositions gives on the host), and
+ * for from[j] < 0 the points pts[pt_offset[j] .. pt_offset[j+1]), as in mplx_set_batch_regions.  pt_offset and pts
+ * may be NULL when every from[j] >= 0; otherwise pt_offset has n_q + 1 entries, starts at 0 and never decreases, and
+ * increases at every j with from[j] < 0.  The paths are traced on the device, by the same walk as
+ * mplx_set_search_region_path's, so each tunnel is exactly that call's region of the same points.  The recorded
+ * paths are read at this call; the next search call replaces them.  Everything else as mplx_set_batch_regions:
+ * the next search calls must have exactly n_q queries, n_q = 0 clears the tunnels, the store, its budget
+ * (MPLX_ERR_ALLOC, tunnels unchanged), mplx_set_map / mplx_update_cells, mplx_read_batch_region, and a constant
+ * number of launches whatever n_q.  Refusals, each with MPLX_ERR_ARG, the tunnels unchanged and no launch: no map,
+ * n_q < 0, a NULL from or radius (n_q > 0), no completed search call (none yet, or the last one failed), a last
+ * call without recording (mplx_set_batch_trajectories), from[j] at or past the last call's query count, a selected
+ * query with no recorded path (no trajectory, start already a goal, or not searched), and from[j] < 0 without
+ * points (NULL pt_offset or pts, or a pt_offset as above it is not).  Synchronous. */
+int mplx_set_batch_regions_recorded(mplx_ctx *ctx, int n_q, const int32_t *from, const int64_t *pt_offset,
+                                    const double *pts, const double *radius, int dense);
+
 /* The tunnels set on the ctx: their query count (0 = none), bricks and device bytes.  Any pointer may be NULL. */
 int mplx_batch_regions_info(mplx_ctx *ctx, int32_t *n_q, int64_t *n_bricks, int64_t *bytes);
 

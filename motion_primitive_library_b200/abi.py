@@ -55,6 +55,7 @@ EXPORTED_SYMBOLS = (
     "mplx_set_batch_trajectories",
     "mplx_plan_batch_trajectories",
     "mplx_set_batch_regions",
+    "mplx_set_batch_regions_recorded",
     "mplx_batch_regions_info",
     "mplx_read_batch_region",
     "mplx_traj_solve",
@@ -274,6 +275,8 @@ def load() -> C.CDLL:
     lib.mplx_plan_batch_trajectories.restype = i32
     lib.mplx_set_batch_regions.argtypes = [vp, i32, vp, vp, vp, i32]
     lib.mplx_set_batch_regions.restype = i32
+    lib.mplx_set_batch_regions_recorded.argtypes = [vp, i32, vp, vp, vp, vp, i32]
+    lib.mplx_set_batch_regions_recorded.restype = i32
     lib.mplx_batch_regions_info.argtypes = [vp, C.POINTER(C.c_int32), C.POINTER(i64), C.POINTER(i64)]
     lib.mplx_batch_regions_info.restype = i32
     lib.mplx_read_batch_region.argtypes = [vp, i32, vp]

@@ -328,9 +328,12 @@ struct mplx_ctx {
 };
 
 namespace mplx {
-// mplx_maps.cu: the cells and the half-widths of MapPlanner::setSearchRegion, shared by mplx_set_search_region_path
-// and mplx_set_batch_regions
-void region_path_cells(const mplx_ctx *c, const double *path, int n_pts, int dense, std::vector<int> &cells);
+// mplx_maps.cu: the grid the ray trace of MapPlanner::setSearchRegion walks (search::segment_cells) and the tunnel's
+// half-widths, shared by mplx_set_search_region_path and the batch tunnel build (mplx_tunnel.cu)
+namespace search {
+struct Grid;
+}
+search::Grid region_grid(const mplx_ctx *c);
 void region_radius_cells(const mplx_ctx *c, const double *radius, int *rn);
 // mplx_search.cu: the device memory one search call may take
 int search_budget(const mplx_ctx *c, size_t &budget);

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "mplx_internal.h"
+#include "mplx_search.cuh"
 
 namespace mplx {
 
@@ -229,54 +230,40 @@ extern "C" int mplx_update_potential_map(mplx_ctx *c, const double *radius, doub
   return MPLX_OK;
 }
 
+// The grid geometry the ray trace of MapPlanner::setSearchRegion reads (search::segment_cells): no map values.
+search::Grid mplx::region_grid(const mplx_ctx *c) {
+  search::Grid G{};
+  G.map = nullptr;
+  G.dim = c->dim;
+  G.res = c->P.res;
+  for (int k = 0; k < 3; k++) {
+    G.mdim[k] = c->P.mdim[k];
+    G.origin[k] = c->P.origin[k];
+  }
+  return G;
+}
+
 // The path cells of MapPlanner::setSearchRegion (map_planner.cpp:49-58, MapUtil::rayTrace map_util.h:120-137),
 // appended to `cells` as (x, y, z) triples (z = 0 in 2-D): every point's cell with `dense`, else each segment's
-// ray-traced cells up to the first one outside the map, then its end point's cell.
-void mplx::region_path_cells(const mplx_ctx *c, const double *path, int n_pts, int dense, std::vector<int> &cells) {
+// cells as search::segment_cells walks them (the device build of mplx_set_batch_regions walks the same).
+namespace {
+struct PushCells {  // a plain host functor: segment_cells is __host__ __device__, so no (constexpr) lambda
+  std::vector<int> *cells;
+  void operator()(int, const int *pn) const { cells->insert(cells->end(), pn, pn + 3); }
+};
+}  // namespace
+
+static void region_path_cells(const mplx_ctx *c, const double *path, int n_pts, int dense, std::vector<int> &cells) {
   const int dim = c->dim;
-  const double res = c->P.res;
-  auto push = [&](const int *pn) { cells.push_back(pn[0]); cells.push_back(pn[1]); cells.push_back(pn[2]); };
-  auto outside = [&](const int *pn) {
-    for (int k = 0; k < dim; k++)
-      if (pn[k] < 0 || pn[k] >= c->P.mdim[k]) return true;
-    return false;
-  };
+  const search::Grid G = region_grid(c);
+  const PushCells push{&cells};
   if (!dense) {
-    for (int i = 1; i < n_pts; i++) {
-      const double *p1 = path + (size_t)(i - 1) * dim, *p2 = path + (size_t)i * dim;
-      double diff[3] = {0, 0, 0}, linf = 0;
-      for (int k = 0; k < dim; k++) {
-        diff[k] = p2[k] - p1[k];
-        linf = std::max(linf, std::abs(diff[k] / res));
-      }
-      const double kk = 0.8;
-      const int max_diff = linf / kk;
-      const double s = 1.0 / max_diff;
-      int prev[3] = {-1, -1, -1};
-      for (int n = 1; n < max_diff; n++) {
-        double pt[3] = {0, 0, 0};
-        for (int k = 0; k < dim; k++) pt[k] = p1[k] + (diff[k] * s) * n;
-        int pn[3];
-        float_to_int(c, pt, pn);
-        if (outside(pn)) break;
-        bool diffc = false;
-        for (int k = 0; k < dim; k++) diffc = diffc || pn[k] != prev[k];
-        if (diffc) push(pn);
-        for (int k = 0; k < 3; k++) prev[k] = pn[k];
-      }
-      int pe[3];
-      double q[3] = {0, 0, 0};
-      for (int k = 0; k < dim; k++) q[k] = p2[k];
-      float_to_int(c, q, pe);
-      push(pe);
-    }
+    for (int i = 1; i < n_pts; i++) search::segment_cells(G, path + (size_t)(i - 1) * dim, path + (size_t)i * dim, push);
   } else {
     for (int i = 0; i < n_pts; i++) {
-      double q[3] = {0, 0, 0};
-      for (int k = 0; k < dim; k++) q[k] = path[(size_t)i * dim + k];
-      int pn[3];
-      float_to_int(c, q, pn);
-      push(pn);
+      int pn[3] = {0, 0, 0};
+      for (int k = 0; k < dim; k++) pn[k] = search::float_to_int(G, path[(size_t)i * dim + k], k);
+      push(i, pn);
     }
   }
 }

@@ -257,6 +257,39 @@ MPLX_HD bool ray_clear(const Grid &G, const double *p1, const double *p2) {
   }
   return true;
 }
+// One segment of MapPlanner::setSearchRegion's ray trace (map_planner.cpp:49-58, MapUtil::rayTrace map_util.h:120-137),
+// the samples ray_clear walks: the cell of each sample p1 + (diff·s)·n, n = 1 .. max_diff - 1, that differs from the
+// one before, up to the first outside the map, then p2's cell.  emit(i, cell) receives the i-th of them (z = 0 in
+// 2-D); returns their number.  G.map is not read.  emit may be host-only where the walk runs on the host.
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <typename Emit>
+MPLX_HD int segment_cells(const Grid &G, const double *p1, const double *p2, Emit emit) {
+  double diff[3] = {0, 0, 0}, m = 0;
+  for (int k = 0; k < G.dim; k++) {
+    diff[k] = p2[k] - p1[k];
+    const double x = fabs(diff[k] / G.res);
+    m = (m < x) ? x : m;
+  }
+  const int max_diff = (int)(m / 0.8);
+  const double s = 1.0 / max_diff;
+  int n_out = 0;
+  int prev[3] = {-1, -1, -1};
+  for (int n = 1; n < max_diff; n++) {
+    int pn[3] = {0, 0, 0};
+    for (int k = 0; k < G.dim; k++) pn[k] = float_to_int(G, p1[k] + (diff[k] * s) * (double)n, k);
+    if (outside(G, pn)) break;
+    bool differs = false;
+    for (int k = 0; k < G.dim; k++) differs = differs || pn[k] != prev[k];
+    if (differs) emit(n_out++, pn);
+    for (int k = 0; k < 3; k++) prev[k] = pn[k];
+  }
+  int pe[3] = {0, 0, 0};
+  for (int k = 0; k < G.dim; k++) pe[k] = float_to_int(G, p2[k], k);
+  emit(n_out++, pe);
+  return n_out;
+}
 // env_map_host::is_goal (mpl_host.hpp:572-585)
 MPLX_HD bool is_goal(const Grid &G, const Goal &Q, const mplx_waypoint &s) {
   bool goaled = linf(G.dim, s.pos, Q.w.pos) <= Q.tol_pos;

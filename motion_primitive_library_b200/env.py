@@ -268,6 +268,25 @@ class env_map:
         abi.check(self._lib.mplx_set_batch_regions(self._h, len(pts), off.ctypes.data, flat.ctypes.data,
                                                    rad.ctypes.data, 1 if dense else 0))
 
+    def set_batch_regions_recorded(self, from_, radius, dense=False, paths=None):
+        """set_batch_regions from the paths the last plan_batch* call recorded (trajectories=True), traced on the
+        device (mplx_set_batch_regions_recorded): query j's tunnel is built from the recorded path of query from_[j]
+        of that call when from_[j] >= 0 (the positions of batch_trajectories()[from_[j]]["nodes"]), else from
+        paths[j] (points x Dim; paths may be None when every from_[j] >= 0).  Read the recorded paths before the
+        next plan_batch* call replaces them."""
+        fr = np.ascontiguousarray(from_, dtype=np.int32).reshape(-1)
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        off = flat = None
+        if paths is not None:
+            pts = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1, self.Dim) for p in paths]
+            if len(pts) != fr.size:
+                raise ValueError("paths must hold one entry per query")
+            off = np.zeros(len(pts) + 1, np.int64)
+            off[1:] = np.cumsum([len(p) for p in pts])
+            flat = np.ascontiguousarray(np.concatenate(pts) if off[-1] else np.zeros((1, self.Dim)))
+        abi.check(self._lib.mplx_set_batch_regions_recorded(self._h, fr.size, fr.ctypes.data, abi.ptr(off),
+                                                            abi.ptr(flat), rad.ctypes.data, 1 if dense else 0))
+
     def batch_regions_info(self):
         """The tunnels set_batch_regions installed: dict(n_q, n_bricks, bytes) (n_q = 0: none)."""
         n, b, by = C.c_int32(), C.c_int64(), C.c_int64()

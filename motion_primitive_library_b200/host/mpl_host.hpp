@@ -37,6 +37,8 @@
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+
+#include "iterative_rounds.hpp"
 #include <vector>
 
 #include "../../include/mplx.h"
@@ -1415,6 +1417,15 @@ class env_map_gpu : public env_map_host<Dim> {
     potential_map_.assign(out.begin(), out.end());
     potential_on_device_ = true;
   }
+  /// The points setSearchRegion traces for `path`: the path itself, or for an empty path (the waypoints of a plan
+  /// whose start is already a goal) one point two cells below the map's origin, whose region is empty as the
+  /// reference's is for an empty path (map_planner.cpp:49-58 traces nothing).
+  vec_E<Vecf<Dim>> region_points(const vec_E<Vecf<Dim>> &path) const {
+    if (!path.empty()) return path;
+    Vecf<Dim> p = map_util_->getOrigin();
+    for (int k = 0; k < Dim; k++) p(k) -= 2 * map_util_->getRes();
+    return vec_E<Vecf<Dim>>{p};
+  }
   /// MapPlanner::setSearchRegion on the device (mplx_set_search_region_path)
   void search_region_from_path(const vec_E<Vecf<Dim>> &path, const Vecf<Dim> &radius, bool dense) override {
     set_search_region_path(path, radius, dense);
@@ -1422,9 +1433,10 @@ class env_map_gpu : public env_map_host<Dim> {
   void set_search_region_path(const vec_E<Vecf<Dim>> &path, const Vecf<Dim> &radius, bool dense) {
     sync();
     std::vector<double> flat;
-    for (const auto &p : path) for (int k = 0; k < Dim; k++) flat.push_back(p(k));
+    for (const auto &p : region_points(path)) for (int k = 0; k < Dim; k++) flat.push_back(p(k));
     std::vector<uint8_t> out(map_util_->map().size());
-    check(mplx_set_search_region_path(ctx_, flat.data(), (int)path.size(), radius.d, dense ? 1 : 0, out.data()));
+    check(mplx_set_search_region_path(ctx_, flat.data(), (int)(flat.size() / Dim), radius.d, dense ? 1 : 0,
+                                      out.data()));
     this->search_region_.assign(out.begin(), out.end());
     region_on_device_ = true;
   }
@@ -2904,8 +2916,90 @@ class MultiQueryPlanner {
   /// the cost-term device search serves this plan: a bounded search, |U| within one CTA (any plan)
   bool costTermsSearchPossible(int max_expand) const { return max_expand > 0 && gpu_->U_.size() <= 256; }
 
+  /// One query's outcome of iterativePlan.
+  struct IterativeResult {
+    bool ok = true;      // what MapPlanner::iterativePlan returns
+    int iterations = 0;  // plan() calls made (MapPlanner::iterations())
+    Result last;         // the query's last plan (traj / traj_end with setCollectTrajectories(true))
+  };
+  /// MapPlanner::iterativePlan(starts[q], goals[q], raw_paths[q], max_num) with setSearchRadius(radius) for every
+  /// query (map_planner.cpp:393-433): replan inside the tunnel around the last trajectory until the cost stops
+  /// changing, the plan fails or max_num plans were made.  Round r plans the queries still running as one batch,
+  /// through plan(), so every path serves it.  Round 1 tunnels around raw_paths; later rounds around each query's
+  /// last trajectory: a query the previous round's device search recorded gets its tunnel traced on the device from
+  /// that recording (mplx_set_batch_regions_recorded), the others (lock-step results) from their host points in the
+  /// same call.  Each query gives what MapPlanner::iterativePlan gives for it alone.  The env's own region, the
+  /// setSearchRegions tunnels and setCollectTrajectories are restored however the call ends.
+  std::vector<IterativeResult> iterativePlan(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
+                                             const std::vector<vec_E<Vecf<Dim>>> &raw_paths, const Vecf<Dim> &radius,
+                                             decimal_t eps, int max_expand, int max_num) {
+    const std::size_t Q = starts.size();
+    if (goals.size() != Q || raw_paths.size() != Q)
+      throw std::runtime_error("iterativePlan: one start, goal and raw path per query");
+    const RestoreRegion restore_region{*gpu_, gpu_->search_region_};
+    struct RestoreSettings {
+      MultiQueryPlanner &p;
+      std::vector<vec_E<Vecf<Dim>>> paths;
+      Vecf<Dim> radius;
+      bool dense, traj;
+      ~RestoreSettings() {
+        p.region_paths_ = std::move(paths);
+        p.region_radius_ = radius;
+        p.region_dense_ = dense;
+        p.region_from_.clear();
+        p.collect_traj_ = traj;
+      }
+    } restore{*this, region_paths_, region_radius_, region_dense_, collect_traj_};
+    const bool want_traj = collect_traj_;
+    collect_traj_ = true;  // the next round's tunnels follow this round's trajectories
+    std::vector<IterativeResult> out(Q);
+    std::vector<IterativeQuery> st(Q, iterative_begin(max_num));
+    std::vector<vec_E<Vecf<Dim>>> path = raw_paths;
+    std::vector<int32_t> from(Q, -1);  // the query's place in the last round's device search; -1: host points
+    std::vector<std::size_t> run;
+    for (;;) {
+      run.clear();
+      for (std::size_t q = 0; q < Q; q++)
+        if (st[q].running) run.push_back(q);
+      if (run.empty()) break;
+      vec_E<Waypoint<Dim>> S, G;
+      region_paths_.clear();
+      region_from_.clear();
+      for (const std::size_t q : run) {
+        S.push_back(starts[q]);
+        G.push_back(goals[q]);
+        region_paths_.push_back(path[q]);
+        region_from_.push_back(from[q]);
+      }
+      region_radius_ = radius;
+      region_dense_ = false;
+      std::vector<Result> res = plan(S, G, eps, max_expand);
+      for (std::size_t i = 0; i < run.size(); i++) {
+        const std::size_t q = run[i];
+        iterative_round(st[q], res[i].valid, res[i].cost, max_num);
+        if (st[q].running) {
+          path[q].clear();
+          for (const auto &e : res[i].traj) path[q].push_back(e.from.pos);
+          if (!res[i].traj.empty()) path[q].push_back(res[i].traj_end.pos);
+          from[q] = recorded_[i] ? (int32_t)i : -1;
+        }
+        out[q].last = std::move(res[i]);
+      }
+    }
+    for (std::size_t q = 0; q < Q; q++) {
+      out[q].ok = st[q].ok;
+      out[q].iterations = st[q].iterations;
+      if (!want_traj) {
+        out[q].last.traj.clear();
+        out[q].last.traj_end = Waypoint<Dim>();
+      }
+    }
+    return out;
+  }
+
   std::vector<Result> plan(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals, decimal_t eps,
                            int max_expand) {
+    recorded_.assign(starts.size(), 0);
     last_device_ = 0;
     slots_ = 0;
     arena_bytes_ = 0;
@@ -2935,18 +3029,23 @@ class MultiQueryPlanner {
     return plan_lockstep(starts, goals, eps, max_expand, region_paths_);
   }
 
-  /// The tunnels of setSearchRegions on the ctx for the next device search (cleared without them).
+  /// The tunnels of setSearchRegions on the ctx for the next device search (cleared without them).  Within
+  /// iterativePlan a query with region_from_ >= 0 takes the path the last device search recorded for that query.
   void install_tunnels() const {
+    const bool recorded = std::any_of(region_from_.begin(), region_from_.end(), [](int32_t f) { return f >= 0; });
     std::vector<int64_t> off(region_paths_.size() + 1, 0);
     std::vector<double> pts;
     for (std::size_t q = 0; q < region_paths_.size(); q++) {
-      for (const auto &p : region_paths_[q])
-        for (int k = 0; k < Dim; k++) pts.push_back(p(k));
+      if (!recorded || region_from_[q] < 0)
+        for (const auto &p : gpu_->region_points(region_paths_[q]))
+          for (int k = 0; k < Dim; k++) pts.push_back(p(k));
       off[q + 1] = (int64_t)(pts.size() / Dim);
     }
-    if (mplx_set_batch_regions(gpu_->ctx(), (int)region_paths_.size(), off.data(), pts.data(), region_radius_.d,
-                               region_dense_ ? 1 : 0) != MPLX_OK)
-      throw std::runtime_error(mplx_last_error());
+    const int n = (int)region_paths_.size(), dense = region_dense_ ? 1 : 0;
+    const int rc = recorded ? mplx_set_batch_regions_recorded(gpu_->ctx(), n, region_from_.data(), off.data(),
+                                                              pts.data(), region_radius_.d, dense)
+                            : mplx_set_batch_regions(gpu_->ctx(), n, off.data(), pts.data(), region_radius_.d, dense);
+    if (rc != MPLX_OK) throw std::runtime_error(mplx_last_error());
   }
 
   /// The queries in the device's form, with the start-is-free test run on the host map as the lock-step
@@ -3089,6 +3188,7 @@ class MultiQueryPlanner {
     for (std::size_t q = 0; q < Q; q++) {
       if (searched[q]) {
         take_device_result(d, q, res[q]);
+        recorded_[q] = collect_traj_ && !res[q].actions.empty();
         continue;
       }
       rest.push_back(q);
@@ -3139,11 +3239,7 @@ class MultiQueryPlanner {
   std::vector<Result> plan_lockstep(const vec_E<Waypoint<Dim>> &starts, const vec_E<Waypoint<Dim>> &goals,
                                     decimal_t eps, int max_expand, const std::vector<vec_E<Vecf<Dim>>> &tunnels) {
     if (!tunnels.empty()) {
-      struct RestoreRegion {
-        env_map_gpu<Dim> &gpu;
-        const std::vector<bool> region;
-        ~RestoreRegion() { gpu.set_search_region(region); }
-      } restore{*gpu_, gpu_->search_region_};
+      const RestoreRegion restore{*gpu_, gpu_->search_region_};
       std::vector<Result> res(starts.size());
       long its = 0, nodes = 0;
       double tp = 0, td = 0, tr = 0;
@@ -3250,6 +3346,14 @@ class MultiQueryPlanner {
   }
 
 
+  /// Puts the env's own search region back however the scope ends: the lock-step loop and iterativePlan install
+  /// tunnels env-wide.
+  struct RestoreRegion {
+    env_map_gpu<Dim> &gpu;
+    const std::vector<bool> region;
+    ~RestoreRegion() { gpu.set_search_region(region); }
+  };
+
   // per-query host env: goal test + heuristic only (its get_succ is never called)
   struct QueryEnv : env_map_host<Dim> {
     using env_map_host<Dim>::env_map_host;
@@ -3268,6 +3372,8 @@ class MultiQueryPlanner {
   bool collect_closed_ = false;
   bool collect_traj_ = false;
   std::vector<vec_E<Vecf<Dim>>> region_paths_;  // setSearchRegions
+  std::vector<int32_t> region_from_;  // within iterativePlan: per query, its recorded path's query, or -1
+  std::vector<uint8_t> recorded_;     // per query of the last plan(): the device search recorded its path
   Vecf<Dim> region_radius_;
   bool region_dense_ = false;
   int last_device_ = 0;  // lastDevicePath()

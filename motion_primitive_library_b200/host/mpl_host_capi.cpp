@@ -170,6 +170,56 @@ int with_session(void *session, F &&f, bool ok = true, const char *refusal = "nu
   });
 }
 
+/// A plan's per-query results into out and, with keep, its trajectories (action ids) and closed sets into the
+/// session for mplh_batch_kept; with mplh_batch_set_trajectories on, its trajectories for mplh_batch_trajectories.
+template <class MQ, class R>
+void store_results(MQ &mq, BatchSession &s, const std::vector<R> &res, bool keep, mplh_query_result *out) {
+  constexpr int Dim = mq_dim<MQ>::value;
+  const int n_q = (int)res.size();
+  if (keep) {
+    s.aoff.assign((size_t)n_q + 1, 0);
+    s.coff.assign((size_t)n_q + 1, 0);
+    s.actions.clear();
+    s.closed.clear();
+  }
+  for (int q = 0; q < n_q; q++) {
+    out[q].valid = res[q].valid ? 1 : 0;
+    out[q].cost = res[q].cost;
+    out[q].expanded = res[q].expanded;
+    out[q].n_closed = (int)res[q].n_closed;
+    out[q].n_actions = (int)res[q].actions.size();
+    if (!keep) continue;
+    s.actions.insert(s.actions.end(), res[q].actions.begin(), res[q].actions.end());
+    s.closed.insert(s.closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
+    s.aoff[q + 1] = (int64_t)s.actions.size();
+    s.coff[q + 1] = (int64_t)s.closed.size();
+  }
+  s.has_traj = s.traj;
+  if (s.traj) {
+    using Env = std::decay_t<decltype(mq.env())>;
+    s.toff.assign((size_t)n_q + 1, 0);
+    s.tnodes.clear();
+    s.tseg.clear();
+    s.tcoeff.clear();
+    for (int q = 0; q < n_q; q++) {
+      for (const auto &e : res[q].traj) {
+        Primitive<Dim> pr;
+        mq.env().forward_action(e.from, e.action_id, pr);
+        s.tnodes.push_back(Env::pod(e.from));
+        s.tseg.push_back(pr.t());
+        for (int a = 0; a <= Dim; a++)
+          for (int k = 0; k < 6; k++) s.tcoeff.push_back(a < Dim ? pr.pr(a).c[k] : pr.pr_yaw().c[k]);
+      }
+      if (!res[q].traj.empty()) {  // the goal state: no segment
+        s.tnodes.push_back(Env::pod(res[q].traj_end));
+        s.tseg.push_back(0.0);
+        s.tcoeff.insert(s.tcoeff.end(), (size_t)(Dim + 1) * 6, 0.0);
+      }
+      s.toff[q + 1] = (int64_t)s.tnodes.size();
+    }
+  }
+}
+
 /// mplh_batch_plan, and with keep mplh_batch_plan_keep
 int batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q, double eps, int max_num,
                bool keep, bool collect_closed, mplh_query_result *out, double *totals) {
@@ -189,48 +239,7 @@ int batch_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *
     auto t0 = std::chrono::steady_clock::now();
     auto res = mq.plan(S, G, eps, max_num);
     const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    if (keep) {
-      s.aoff.assign((size_t)n_q + 1, 0);
-      s.coff.assign((size_t)n_q + 1, 0);
-      s.actions.clear();
-      s.closed.clear();
-    }
-    for (int q = 0; q < n_q; q++) {
-      out[q].valid = res[q].valid ? 1 : 0;
-      out[q].cost = res[q].cost;
-      out[q].expanded = res[q].expanded;
-      out[q].n_closed = (int)res[q].n_closed;
-      out[q].n_actions = (int)res[q].actions.size();
-      if (!keep) continue;
-      s.actions.insert(s.actions.end(), res[q].actions.begin(), res[q].actions.end());
-      s.closed.insert(s.closed.end(), res[q].closed_keys.begin(), res[q].closed_keys.end());
-      s.aoff[q + 1] = (int64_t)s.actions.size();
-      s.coff[q + 1] = (int64_t)s.closed.size();
-    }
-    s.has_traj = s.traj;
-    if (s.traj) {
-      using Env = std::decay_t<decltype(mq.env())>;
-      s.toff.assign((size_t)n_q + 1, 0);
-      s.tnodes.clear();
-      s.tseg.clear();
-      s.tcoeff.clear();
-      for (int q = 0; q < n_q; q++) {
-        for (const auto &e : res[q].traj) {
-          Primitive<Dim> pr;
-          mq.env().forward_action(e.from, e.action_id, pr);
-          s.tnodes.push_back(Env::pod(e.from));
-          s.tseg.push_back(pr.t());
-          for (int a = 0; a <= Dim; a++)
-            for (int k = 0; k < 6; k++) s.tcoeff.push_back(a < Dim ? pr.pr(a).c[k] : pr.pr_yaw().c[k]);
-        }
-        if (!res[q].traj.empty()) {  // the goal state: no segment
-          s.tnodes.push_back(Env::pod(res[q].traj_end));
-          s.tseg.push_back(0.0);
-          s.tcoeff.insert(s.tcoeff.end(), (size_t)(Dim + 1) * 6, 0.0);
-        }
-        s.toff[q + 1] = (int64_t)s.tnodes.size();
-      }
-    }
+    store_results(mq, s, res, keep, out);
     if (totals) {
       totals[0] = (double)mq.iterations(); totals[1] = (double)mq.nodes_expanded(); totals[2] = secs;
       totals[3] = mq.t_pop(); totals[4] = mq.t_device(); totals[5] = mq.t_relax(); totals[6] = 0.0;
@@ -462,6 +471,86 @@ int mplh_batch_set_regions(void *session, int n_q, const int64_t *pt_offset, con
     for (int k = 0; k < Dim; k++) r(k) = n_q > 0 ? radius[k] : 0.0;
     mq.setSearchRegions(paths, r, dense != 0);
   }, ok, "null session, n_q < 0, a missing array, pt_offset[0] != 0 or a query with no points");
+}
+
+/* MapPlanner::iterativePlan for a batch (MultiQueryPlanner::iterativePlan) with the session's path, eps and
+ * max_num: query q replans inside tunnels of the given radius (dim metres) around its last trajectory until the
+ * cost stops changing, its plan fails or max_iter plans were made.  Round 1 tunnels around the points
+ * pts[pt_offset[q] .. pt_offset[q+1]); with pt_offset and pts NULL the batch is planned first (with the session's
+ * own tunnels, if any) and each query iterates from that plan's trajectory, as mplh_iterative_plan does for one
+ * query: a query whose first plan fails reports 0 iterations and that plan.  info[2q] = plan() calls made by
+ * iterativePlan, info[2q+1] = its return value; out[q] = the query's last plan, whose trajectory (action ids) and
+ * closed set mplh_batch_kept then copies, and with mplh_batch_set_trajectories on its planned trajectory
+ * mplh_batch_trajectories.  The session's tunnels and settings are unchanged afterwards. */
+int mplh_batch_iterative_plan(void *session, const mplx_waypoint *starts, const mplx_waypoint *goals, int n_q,
+                              const int64_t *pt_offset, const double *pts, const double *radius, int max_iter,
+                              double eps, int max_num, mplh_query_result *out, int32_t *info) {
+  bool ok = n_q >= 0 && radius && out && info && (n_q == 0 || (starts && goals)) && (!pt_offset == !pts);
+  if (ok && pt_offset) {
+    ok = pt_offset[0] == 0;
+    for (int q = 0; ok && q < n_q; q++) ok = pt_offset[q + 1] >= pt_offset[q];
+  }
+  return with_session(session, [&](auto &mq, BatchSession &s) {
+    constexpr int Dim = mq_dim<std::decay_t<decltype(mq)>>::value;
+    using Res = typename std::decay_t<decltype(mq)>::Result;
+    struct Reset {
+      decltype(mq) p;
+      bool traj;
+      ~Reset() {
+        p.setCollectClosed(false);
+        p.setCollectTrajectories(traj);
+      }
+    } reset{mq, s.traj};
+    mq.setCollectClosed(true);
+    vec_E<Waypoint<Dim>> S, G;
+    for (int q = 0; q < n_q; q++) {
+      S.push_back(mplh::wp_from<Dim>(starts[q], s.control));
+      G.push_back(mplh::wp_from<Dim>(goals[q], s.control));
+    }
+    std::vector<vec_E<Vecf<Dim>>> raw((std::size_t)n_q);
+    std::vector<Res> last((std::size_t)n_q);
+    std::vector<int> idx;  // the queries that iterate
+    if (pt_offset) {
+      for (int q = 0; q < n_q; q++) {
+        for (int64_t i = pt_offset[q]; i < pt_offset[q + 1]; i++) {
+          Vecf<Dim> p;
+          for (int k = 0; k < Dim; k++) p(k) = pts[i * Dim + k];
+          raw[(std::size_t)q].push_back(p);
+        }
+        idx.push_back(q);
+      }
+    } else {
+      mq.setCollectTrajectories(true);  // the first plan's trajectories are the raw paths
+      last = mq.plan(S, G, eps, max_num);
+      mq.setCollectTrajectories(s.traj);
+      for (int q = 0; q < n_q; q++) {
+        info[2 * q] = info[2 * q + 1] = 0;
+        const Res &r = last[(std::size_t)q];
+        if (!r.valid) continue;
+        for (const auto &e : r.traj) raw[(std::size_t)q].push_back(e.from.pos);
+        if (!r.traj.empty()) raw[(std::size_t)q].push_back(r.traj_end.pos);
+        if (!s.traj) last[(std::size_t)q].traj.clear();
+        idx.push_back(q);
+      }
+    }
+    vec_E<Waypoint<Dim>> IS, IG;
+    std::vector<vec_E<Vecf<Dim>>> IP;
+    for (const int q : idx) {
+      IS.push_back(S[(std::size_t)q]);
+      IG.push_back(G[(std::size_t)q]);
+      IP.push_back(raw[(std::size_t)q]);
+    }
+    Vecf<Dim> r;
+    for (int k = 0; k < Dim; k++) r(k) = radius[k];
+    auto it = mq.iterativePlan(IS, IG, IP, r, eps, max_num, max_iter);
+    for (std::size_t i = 0; i < idx.size(); i++) {
+      const int q = idx[i];
+      info[2 * q] = it[i].iterations;
+      info[2 * q + 1] = it[i].ok ? 1 : 0;
+      last[(std::size_t)q] = std::move(it[i].last);
+    }
+    store_results(mq, s, last, true, out);
+  }, ok, "null session, n_q < 0, a missing array, or pt_offset not starting at 0 and non-decreasing");
 }
 
 /* The session's plans also collect every query's trajectory (on = 1; 0 = off, the default), whichever path runs

@@ -80,6 +80,7 @@ SIGNATURES = {
     "mplh_batch_close": ([_vp, C.POINTER(_d)], _i),
     "mplh_batch_set_trajectories": ([_vp, _i], _i),
     "mplh_batch_set_regions": ([_vp, _i, _vp, _vp, _vp, _i], _i),
+    "mplh_batch_iterative_plan": ([_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _d, _i, _vp, _vp], _i),
     "mplh_batch_trajectories": ([_vp, _i, _vp, _vp, _vp, _vp, _vp, _i64, _i64p], _i),
     "mplh_traj_solve": ([_i, _i, _i, _vp, _vp, _i, _vp, _d, _i, _i32p, _vp, _vp, _vp, _vp], _i),
     "mplh_traj_sample": ([_i, _i, _vp, _vp, _i, _i, _vp, _vp], _i),
@@ -410,18 +411,65 @@ class BatchPlanner:
             if trajectories:
                 self._call("mplh_batch_set_trajectories", 0)
         nq = len(res)
+        out = (res, self._totals(totals)) + self.kept(res, closed)
+        if not trajectories:
+            return out
+        return out + (self._trajectories(nq, int(sum(n + 1 for n in res["n_actions"] if n)), n_samples),)
+
+    def kept(self, res, closed=True):
+        """(actions, closed): every query's trajectory (action ids) and, with closed, closed set (sorted lattice
+        keys) of the last plan_detail or iterative_plan, one array per query; res is that call's results."""
+        nq = len(res)
         na, nc = int(res["n_actions"].sum()), int(res["n_closed"].sum()) if closed else 0
         aoff, coff = np.zeros(nq + 1, np.int64), np.zeros(nq + 1, np.int64)
         acts = np.zeros(max(na, 1), np.int32)
         keys = np.zeros(max(nc, 1), np.uint64) if closed else None
         self._call("mplh_batch_kept", aoff.ctypes.data, acts.ctypes.data, acts.size, coff.ctypes.data,
                    None if keys is None else keys.ctypes.data, 0 if keys is None else keys.size)
-        tot = self._totals(totals)
-        out = (res, tot, [acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
-               [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
+        return ([acts[aoff[q]:aoff[q + 1]].copy() for q in range(nq)],
+                [keys[coff[q]:coff[q + 1]].copy() for q in range(nq)] if closed else None)
+
+    def iterative_plan(self, starts, goals, radius, max_iter=3, raw_paths=None, eps=None, max_num=None,
+                       trajectories=False, n_samples=0):
+        """MapPlanner::iterativePlan for every query as one batch (mplh_batch_iterative_plan): query q replans inside
+        tunnels of `radius` (Dim metres) around its last trajectory until the cost stops changing, its plan fails or
+        max_iter plans were made.  raw_paths (one points x Dim array per query) are the first round's tunnels; None
+        plans the batch first and iterates from those trajectories, as iterative_plan() does for one query (a query
+        whose first plan fails reports 0 iterations and that plan).  Returns (res, iterations, ok): res as plan()'s,
+        for each query's last plan (kept() gives its actions and closed set), iterations the plan() calls
+        iterativePlan made and ok its return value; with trajectories=True also the last plans' trajectories in
+        plan_detail's layout.  The session's tunnels and settings are unchanged afterwards."""
+        dim = self._args.dim
+        starts = np.ascontiguousarray(starts, dtype=WAYPOINT_DTYPE)
+        goals = np.ascontiguousarray(goals, dtype=WAYPOINT_DTYPE)
+        nq = len(starts)
+        off = flat = None
+        if raw_paths is not None:
+            pts = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1, dim) for p in raw_paths]
+            if len(pts) != nq:
+                raise ValueError("one raw path per query")
+            off = np.zeros(nq + 1, np.int64)
+            off[1:] = np.cumsum([len(p) for p in pts])
+            flat = np.ascontiguousarray(np.concatenate(pts) if off[-1] else np.zeros((1, dim)))
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        out = (QueryResult * max(nq, 1))()
+        info = np.zeros(2 * max(nq, 1), np.int32)
+        self._call("mplh_batch_set_trajectories", 1 if trajectories else 0)
+        try:
+            self._call("mplh_batch_iterative_plan", starts.ctypes.data, goals.ctypes.data, nq,
+                       None if off is None else off.ctypes.data, None if flat is None else flat.ctypes.data,
+                       rad.ctypes.data, int(max_iter), self._args.eps if eps is None else eps,
+                       self._args.max_num if max_num is None else max_num, out, info.ctypes.data)
+        finally:
+            if trajectories:
+                self._call("mplh_batch_set_trajectories", 0)
+        res = np.zeros(nq, dtype=_QRES)
+        for q in range(nq):
+            res[q] = (out[q].valid, out[q].cost, out[q].expanded, out[q].n_closed, out[q].n_actions)
+        its, ok = info[0:2 * nq:2].copy(), info[1:2 * nq:2].astype(bool)
         if not trajectories:
-            return out
-        return out + (self._trajectories(nq, int(sum(n + 1 for n in res["n_actions"] if n)), n_samples),)
+            return res, its, ok
+        return res, its, ok, self._trajectories(nq, int(sum(n + 1 for n in res["n_actions"] if n)), n_samples)
 
     def _trajectories(self, nq, cap, n_samples):
         """mplh_batch_trajectories: the last plan's trajectories, one dict per query."""
