@@ -34,6 +34,32 @@ int mplx_bind(mplx_ctx *ctx) {
   return MPLX_OK;
 }
 
+// L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_expand_fxn.  Both halves
+// when they fit it; otherwise the occupancy half, which every sample reads, and not the summary half, which only
+// uncertain samples read (a window larger than the carve-out thrashes it).  Reserved only while the fixed-point
+// kernels can run (fx_supported: a map without a potential field, no yaw control, occ2 within its address
+// range); otherwise none is set aside: the set-aside takes L2 from the kernels that do run (cfg4, which never
+// reads occ2, was 1.5 % slower per step with 22.8 MiB set aside than with 16 MiB).
+void mplx::size_l2_window(mplx_ctx *c) {
+  size_t bytes = 0;
+  int maxp = 0, maxw = 0;
+  if (c->has_map && !c->has_pot && (c->P.control & 16) == 0 && c->P.occ2_sum <= (1u << 27)) {
+    cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
+    cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
+    const size_t half = (size_t)c->P.occ2_sum * sizeof(uint32_t);
+    if (maxp > 0 && maxw > 0) bytes = 2 * half <= (size_t)maxp ? 2 * half : half;
+  }
+  const size_t want = bytes < (size_t)maxp ? bytes : (size_t)maxp;
+  if (want != c->l2_persist) {
+    if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) != cudaSuccess) {
+      cudaGetLastError();
+      bytes = 0;
+    }
+    c->l2_persist = want;
+  }
+  c->occ2_window = bytes < (size_t)maxw ? bytes : (size_t)maxw;
+}
+
 static void refresh_params(mplx_ctx *c) {
   c->P.map = c->has_map ? c->map.p : nullptr;
   c->P.pot = c->has_pot ? c->pot.p : nullptr;
@@ -42,6 +68,7 @@ static void refresh_params(mplx_ctx *c) {
   c->P.stats = c->stats_on ? c->stats.p : nullptr;
   c->P.occ_bits = c->has_map ? c->occ.p : nullptr;
   c->P.occ2 = c->has_map ? c->occ2.p : nullptr;
+  mplx::size_l2_window(c);
   c->P.occ2_bytes = c->has_map ? c->occ2_window : 0;
   c->P.prow = c->prow.p;
   c->P.row_u = c->row_u.p;
@@ -143,28 +170,10 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
   CU(c->occ.reserve((nvox + 31) / 32));
   CU(mplx::launch_pack_bits(c->map.p, nvox, c->occ.p, true, c->stream));
   const int nz = c->dim == 3 ? dim[2] : 1;
-  const size_t npairs = mplx::occ2_pair_count(c->dim, dim[0], dim[1], nz);
+  const size_t npairs = mplx::occ2_guard_pair_count(c->dim, dim[0], dim[1], nz);
   CU(c->occ2.reserve(2 * npairs));
   CU(mplx::launch_pack_occ2(c->occ.p, nvox, c->dim, dim[0], dim[1], nz, c->occ2.p, c->stream));
   c->launches += 2;
-  {
-    // L2 persisting carve-out for the bitmap pairs (up to what the device grants): see launch_expand_fxn.  Both
-    // halves when they fit it; otherwise the occupancy half, which every sample reads, and not the summary
-    // half, which only uncertain samples read (a window larger than the carve-out thrashes it).
-    int maxp = 0, maxw = 0;
-    cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, c->device);
-    cudaDeviceGetAttribute(&maxw, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
-    const size_t half = npairs * sizeof(uint32_t);
-    const size_t bytes = 2 * half <= (size_t)maxp ? 2 * half : half;
-    c->occ2_window = 0;
-    if (maxp > 0 && maxw > 0) {
-      const size_t want = bytes < (size_t)maxp ? bytes : (size_t)maxp;
-      if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess)
-        c->occ2_window = bytes < (size_t)maxw ? bytes : (size_t)maxw;
-      else
-        cudaGetLastError();
-    }
-  }
   CU(cudaStreamSynchronize(c->stream));
   c->nvox = nvox;
   for (int k = 0; k < 3; k++) {
@@ -172,9 +181,8 @@ int mplx_set_map(mplx_ctx *c, const int8_t *data, const int32_t *dim, const doub
     c->P.origin[k] = k < c->dim ? origin[k] : 0.0;
     c->P.dimd[k] = (double)c->P.mdim[k];
   }
-  c->P.occ2_nb[0] = mplx::occ2_bricks_x(c->dim, dim[0]);
-  c->P.occ2_nb[1] = mplx::occ2_bricks_y(c->dim, dim[1]);
-  c->P.occ2_sum = (unsigned)npairs;
+  mplx::occ2_sep_terms(c->dim, dim[0], dim[1], mplx::kFxHiBase, c->P.occ2_e, c->P.occ2_k0);
+  c->P.occ2_sum = npairs < ((size_t)1 << 32) ? (unsigned)npairs : ~0u;  // ~0u: beyond the fixed-point kernels (fx_supported)
   c->P.res = res;
   c->P.rinv = 1.0 / res;
   c->has_map = true;

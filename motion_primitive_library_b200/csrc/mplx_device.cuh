@@ -36,12 +36,14 @@ struct EnvParams {
   const int *tcount;           // [kNMax+1]
   const double *tdt;           // [kNMax+1]  T/n (env_map.h:98)
   int maxn;                    // largest n the flat sample phase accepts (<= kNMax)
-  // {occupancy word, candidate-summary word} pairs of the fixed-point kernels (mplx_fx.cu), in bricks,
-  // occupancy half first (layout: mplx_pack.cuh)
+  // {occupancy word, candidate-summary word} pairs of the fixed-point kernels (mplx_fx.cu), in bricks of
+  // the map padded by a guard band, occupancy half first (layout: mplx_pack.cuh)
   const uint32_t *occ2;
   unsigned occ2_sum;  // words of each half: the summary word of pair p is occ2[occ2_sum + p]
   size_t occ2_bytes;  // bytes of occ2 (from its start) an L2 persisting carve-out was granted for, else 0
-  int occ2_nb[2];     // bricks of occ2 along x and y (occ2_bricks_x, occ2_bricks_y)
+  // the per-axis terms of a cell's bit index from the high words of the fixed-point sample loop
+  // (occ2_sep_k, occ2_sep_terms with H = kFxHiBase)
+  unsigned occ2_e[3], occ2_k0;
   // Per-axis value tables of U for the node-cooperative kernel (mplx_fx.cu): the distinct values of
   // U[.][a] (bitwise) of all axes listed one after the other as "rows"; U[i][a] == row_u[prow[3*i+a]].
   const unsigned char *prow;      // [nU*3]
@@ -49,6 +51,10 @@ struct EnvParams {
   const unsigned char *row_axis;  // [n_rows]
   int n_rows;                     // 0: tables not available (more than 255 rows)
 };
+
+// the fixed-point cell rule of mplx_fx.cu: y + kFxMagic has the high word kFxHiBase + floor(y)
+constexpr double kFxMagic = 1572864.0;   // 1.5 * 2^20: ulp(2^20..2^21) = 2^-32
+constexpr int kFxHiBase = 0x41380000;    // high word of kFxMagic; + floor(y) for |y| < 2^19
 
 constexpr int kNMax = 128;          // rows of the sample-time table
 constexpr int kTStride = kNMax + 2; // doubles per row

@@ -99,8 +99,9 @@ __device__ __forceinline__ void fx_resolve(const EnvParams &P, const mplx_waypoi
 // Threads 256..287 (the helper warp): hash_value(curr) of the CTA's nodes while the others run phase
 // A, then the exact re-evaluation of whatever phase C queued.  Barriers: B1 publishes the node
 // hashes (the self-loop test `tn == curr`, env_map.h:158, is the last step of phase A), B2 the
-// validity ballots of phase B, B3 the queue.
-template <int DIM, int ORD, int UNR, int MINB, bool LAT, bool REGION>
+// validity ballots of phase B, B3 the queue.  CHECK: the sample loop tests every sample against the map
+// (fx_issue); without it a primitive that may leave the guard band of occ2 (fx_band) takes the literal loop.
+template <int DIM, int ORD, int UNR, int MINB, bool LAT, bool REGION, bool CHECK>
 __global__ void __launch_bounds__(kFxThreads, MINB)
 expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__restrict__ nodes, int n_nodes, int npb,
                  int inv_nU, const __grid_constant__ OutPtrs o) {
@@ -230,16 +231,21 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
       double reach = 0.0;
 #pragma unroll
       for (int a = 0; a < DIM; a++) reach = fmax(reach, (fabs(pr.ax[a].c5) + fabs(P.origin[a])) * P.rinv);
-      if (n > kNMax || !(reach < kFxRange)) {
-        // beyond the sample-time table or the range of the fixed-point bound: the literal loop
+      double C[DIM][ORD + 1];
+      bool band = true;
+#pragma unroll
+      for (int a = 0; a < DIM; a++) {
+        fx_axis<ORD>(pr.ax[a], P.origin[a], P.rinv, C[a]);
+        if (!REGION && !CHECK) band = band && fx_band<ORD>(C[a], P.T, P.mdim[a]);
+      }
+      if (n > kNMax || !(reach < kFxRange) || !band) {
+        // beyond the sample-time table, the range of the fixed-point bound or (unchecked loop) able to leave
+        // the guard band: the literal loop
         double cf[CoefLayout<DIM, ORD, false>::NCMAX];
         fill_coef<DIM, ORD, false>(pr, false, cf);
         unsigned ns = 0;
         verdict = isinf(traverse_loop<DIM, ORD, false>(P, cf, false, max_v, ns)) ? 1 : 0;
       } else {
-        double C[DIM][ORD + 1];
-#pragma unroll
-        for (int a = 0; a < DIM; a++) fx_axis<ORD>(pr.ax[a], P.origin[a], P.rinv, C[a]);
         const unsigned *__restrict__ occ_words = P.occ2;
         unsigned long long amask = 0;
         bool full = false;
@@ -247,7 +253,7 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
         int base = 0;
         for (int left = __ldg(P.tcount + n);; left -= UNR, base += UNR) {
           unsigned amb;
-          const int st = fx_group<DIM, ORD, UNR, REGION>(P, occ_words, C, dt, left, t, amb);
+          const int st = fx_group<DIM, ORD, UNR, REGION, CHECK>(P, occ_words, C, dt, left, t, amb);
           if (st == 2) {
             verdict = 1;
             break;
@@ -279,7 +285,9 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
 
 // Occupancy planning only (no potential map, no yaw control), |U| <= 128 (hcurr slots), stats off.
 bool fx_supported(const EnvParams &P) {
-  return P.occ2 != nullptr && P.pot == nullptr && (P.control & 16) == 0 && P.nU <= kThreads && P.stats == nullptr;
+  // occ2_sep_k counts the padded map's cells in 32 bits
+  return P.occ2 != nullptr && P.occ2_sum <= (1u << 27) && P.pot == nullptr && (P.control & 16) == 0 && P.nU <= kThreads &&
+         P.stats == nullptr;
 }
 
 cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, int n_nodes, const OutPtrs &o,
@@ -300,18 +308,22 @@ cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, i
     return with_order(P.control, [&](auto ORD) {
       return with_bool(unr == 8, [&](auto UNR8) {
         return with_bool(o.lattice != nullptr, [&](auto LAT) {
-          return with_bool(P.region_bits != nullptr, [&](auto REGION) {
-            auto launch = [&](auto MINB) {
-              expand_fx_kernel<DIM, ORD, UNR8 ? 8 : 4, MINB, LAT, REGION>
+          // the REGION loop tests every sample; otherwise CHECK as in launch_expand_fxn
+          return with_bool(P.region_bits != nullptr || P.maxn + 2 > kOcc2Guard, [&](auto CHECK) {
+            auto launch = [&](auto MINB, auto REGION) {
+              expand_fx_kernel<DIM, ORD, UNR8 ? 8 : 4, MINB, LAT, REGION, CHECK>
                   <<<grid, kFxThreads, 0, st>>>(P, d_nodes, n_nodes, npb, inv_nU, o);
               return cudaGetLastError();
             };
-            // MPLX_FX_MINB = 5 or 6 is for the plain 3-D ACC plan
-            if constexpr (DIM == 3 && ORD == 2 && !LAT && !REGION) {
-              if (minb_env == 5) return launch(Int<5>());
-              if (minb_env == 6) return launch(Int<6>());
+            if constexpr (CHECK) {
+              if (P.region_bits != nullptr) return launch(Int<4>(), std::true_type{});
             }
-            return launch(Int<4>());
+            // MPLX_FX_MINB = 5 or 6 is for the plain 3-D ACC plan
+            if constexpr (DIM == 3 && ORD == 2 && !LAT) {
+              if (minb_env == 5) return launch(Int<5>(), std::false_type{});
+              if (minb_env == 6) return launch(Int<6>(), std::false_type{});
+            }
+            return launch(Int<4>(), std::false_type{});
           });
         });
       });
@@ -319,14 +331,14 @@ cudaError_t launch_expand_fx(const EnvParams &P, const mplx_waypoint *d_nodes, i
   });
 }
 
-// The {occupancy word, candidate-summary word} pairs in bricks (layout and bits: occ2_brick_pair), each
-// half of the buffer holding one word of every pair.
+// The {occupancy word, candidate-summary word} pairs in bricks of the padded map (layout and bits:
+// occ2_guard_brick_pair), each half of the buffer holding one word of every pair.
 __global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, int dim, int nx, int ny, int nz,
                                  uint32_t *__restrict__ out) {
-  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
+  const size_t npairs = occ2_guard_pair_count(dim, nx, ny, nz);
   for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < npairs; p += (size_t)gridDim.x * blockDim.x) {
     uint32_t o, s;
-    occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
+    occ2_guard_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
     out[p] = o;
     out[npairs + p] = s;
   }
@@ -334,7 +346,7 @@ __global__ void pack_occ2_kernel(const uint32_t *__restrict__ occ, size_t nvox, 
 
 cudaError_t launch_pack_occ2(const uint32_t *d_occ, size_t nvox, int dim, int nx, int ny, int nz, uint32_t *d_out,
                              cudaStream_t st) {
-  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
+  const size_t npairs = occ2_guard_pair_count(dim, nx, ny, nz);
   int grid = (int)((npairs + 255) / 256);
   if (grid > sm_count() * 16) grid = sm_count() * 16;
   if (grid < 1) grid = 1;

@@ -299,6 +299,7 @@ struct mplx_ctx {
   DevBuf<double> row_u;
   int n_rows = 0;
   size_t occ2_window = 0;  // bytes of occ2 (from its start) covered by the L2 access-policy window (0 = none)
+  size_t l2_persist = 0;   // persisting L2 set-aside this ctx last asked for (size_l2_window)
   DevBuf<double> U, ttab, tdt;
   DevBuf<int> tcount;
   int kernel = 0;  // mplx_set_kernel
@@ -334,6 +335,8 @@ namespace search {
 struct Grid;
 }
 search::Grid region_grid(const mplx_ctx *c);
+// mplx_api.cu: the L2 persisting set-aside and window for occ2, sized for the ctx's current plan
+void size_l2_window(mplx_ctx *c);
 void region_radius_cells(const mplx_ctx *c, const double *radius, int *rn);
 // mplx_search.cu: the device memory one search call may take
 int search_budget(const mplx_ctx *c, size_t &budget);

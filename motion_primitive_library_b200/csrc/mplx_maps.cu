@@ -227,6 +227,8 @@ extern "C" int mplx_update_potential_map(mplx_ctx *c, const double *radius, doub
   c->P.pot_w = potential_weight;
   c->P.grad_w = gradient_weight;
   c->P.pot = c->pot.p;
+  size_l2_window(c);  // no occ2 carve-out beside a potential field
+  c->P.occ2_bytes = c->occ2_window;
   return MPLX_OK;
 }
 

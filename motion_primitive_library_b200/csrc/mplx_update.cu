@@ -8,7 +8,8 @@
 //   2. scatter: the last entry of each run writes its byte into the grid;
 //   3. every occupancy word holding an edited voxel is re-packed from its 32 bytes (pack_word);
 //   4. every occ2 brick pair holding a voxel whose summary an edited voxel reaches is recomputed
-//      (occ2_brick_pair, from the occupancy words of step 3 and occ2_summary_word).
+//      (occ2_guard_brick_pair, from the occupancy words of step 3 and occ2_summary_word); the guard band
+//      around the map never changes.
 // Step 3 runs one thread per distinct word (the first entry of each word in sorted order), step 4 one
 // thread per edited voxel that reaches a pair its predecessor does not.  Both use the rules of the full
 // packs on the final grid and occupancy, so the result is bit-identical to mplx_set_map of the edited
@@ -46,9 +47,9 @@ __global__ void repack_occ_kernel(const uint32_t *__restrict__ idx, int n, const
 // of the row) reaches no pair the predecessor does not, and is skipped; duplicates are skipped too.
 __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, const uint32_t *__restrict__ occ, size_t nvox,
                                    int dim, int nx, int ny, int nz, uint32_t *__restrict__ occ2) {
-  const size_t npairs = occ2_pair_count(dim, nx, ny, nz);
+  const size_t npairs = occ2_guard_pair_count(dim, nx, ny, nz);
   const size_t sxy = (size_t)nx * ny;
-  const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
+  const int pbx = occ2_guard_bricks_x(dim, nx), pby = occ2_guard_bricks_y(dim, ny);
   const int xmask = dim == 3 ? 7 : 31;  // x extent of a brick row - 1
   for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
     const uint32_t v = idx[k];
@@ -60,14 +61,14 @@ __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, cons
       for (int dy = 0; dy <= 1; dy++)
         for (int dx = 0; dx <= 1; dx++) {
           if (x + dx >= nx || y + dy >= ny || z + dz >= nz) continue;
-          const unsigned p = dim == 3 ? occ2_pair<3>(x + dx, y + dy, z + dz, nbx, nby)
-                                      : occ2_pair<2>(x + dx, y + dy, 0, nbx, nby);
+          const unsigned p = dim == 3 ? occ2_guard_pair<3>(x + dx, y + dy, z + dz, pbx, pby)
+                                      : occ2_guard_pair<2>(x + dx, y + dy, 0, pbx, pby);
           bool seen = false;
           for (int i = 0; i < nd; i++) seen = seen || done[i] == p;
           if (seen) continue;
           done[nd++] = p;
           uint32_t o, s;
-          occ2_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
+          occ2_guard_brick_pair(occ, p, nvox, dim, nx, ny, nz, o, s);
           occ2[p] = o;
           occ2[npairs + p] = s;
         }
@@ -75,12 +76,12 @@ __global__ void repack_occ2_kernel(const uint32_t *__restrict__ idx, int n, cons
 }
 
 // The pairs in voxel order, as mplx_read_map returns them: pair w holds the occupancy word w and the summary
-// bits of voxels 32w..32w+31, gathered from the bricks; bits at i >= nvox read as they did in voxel order
-// (occupancy 0, summary 1).
+// bits of voxels 32w..32w+31, gathered from the bricks of the padded map; bits at i >= nvox read as they did
+// in voxel order (occupancy 0, summary 1).
 __global__ void unbrick_occ2_kernel(const uint32_t *__restrict__ occ2, size_t npairs, size_t nvox, int dim, int nx,
                                     int ny, uint2 *__restrict__ out) {
   const size_t nwords = (nvox + 31) >> 5, sxy = (size_t)nx * ny;
-  const int nbx = occ2_bricks_x(dim, nx), nby = occ2_bricks_y(dim, ny);
+  const int pbx = occ2_guard_bricks_x(dim, nx), pby = occ2_guard_bricks_y(dim, ny);
   for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < nwords; w += (size_t)gridDim.x * blockDim.x) {
     uint32_t o = 0, s = 0;
     for (int b = 0; b < 32; b++) {
@@ -90,7 +91,7 @@ __global__ void unbrick_occ2_kernel(const uint32_t *__restrict__ occ2, size_t np
         continue;
       }
       const int x = (int)(i % nx), y = (int)(i / nx % ny), z = (int)(i / sxy);
-      const unsigned p = dim == 3 ? occ2_pair<3>(x, y, z, nbx, nby) : occ2_pair<2>(x, y, 0, nbx, nby);
+      const unsigned p = dim == 3 ? occ2_guard_pair<3>(x, y, z, pbx, pby) : occ2_guard_pair<2>(x, y, 0, pbx, pby);
       const unsigned bit = dim == 3 ? occ2_bit<3>(x, y) : occ2_bit<2>(x, y);
       o |= ((occ2[p] >> bit) & 1u) << b;
       s |= ((occ2[npairs + p] >> bit) & 1u) << b;
@@ -169,8 +170,8 @@ extern "C" int mplx_read_map(mplx_ctx *c, int8_t *grid, uint32_t *occ, uint32_t 
     ScopedDevBuf<uint2> tmp;
     CU(tmp.reserve(nwords));
     const int grid = grid_for_entries(nwords < (1u << 30) ? (int)nwords : 1 << 30);
-    unbrick_occ2_kernel<<<grid, 256, 0, st>>>(c->occ2.p, c->P.occ2_sum, c->nvox, c->dim, c->P.mdim[0], c->P.mdim[1],
-                                              tmp.p);
+    const size_t npairs = occ2_guard_pair_count(c->dim, c->P.mdim[0], c->P.mdim[1], c->dim == 3 ? c->P.mdim[2] : 1);
+    unbrick_occ2_kernel<<<grid, 256, 0, st>>>(c->occ2.p, npairs, c->nvox, c->dim, c->P.mdim[0], c->P.mdim[1], tmp.p);
     CU(cudaGetLastError());
     c->launches += 1;
     CU(cudaMemcpyAsync(occ2, tmp.p, nwords * sizeof(uint2), cudaMemcpyDeviceToHost, st));
