@@ -235,6 +235,22 @@ struct OutPtrs {
   int32_t *lattice;
 };
 
+// hash_value(waypoint) (waypoint.h:93-125) as phase_ab folds it into hcurr: once per node in the fixed-point
+// kernels, and the device search's start and goal keys.
+template <int DIM, int ORD, bool YAW>
+__device__ __forceinline__ uint64_t node_hash(const mplx_waypoint *w) {
+  uint64_t h = 0;
+#pragma unroll
+  for (int k = 0; k < DIM; k++) {
+    hash_combine(h, lattice_id(w->pos[k], 0.01, 100.0));
+    if (ORD >= 2) hash_combine(h, lattice_id(w->vel[k], 0.1, 10.0));
+    if (ORD >= 3) hash_combine(h, lattice_id(w->acc[k], 0.1, 10.0));
+    if (ORD >= 4) hash_combine(h, lattice_id(w->jrk[k], 0.1, 10.0));
+  }
+  if (YAW) hash_combine(h, lattice_id(w->yaw, 0.1, 10.0));
+  return h;
+}
+
 // Phases A and B for one item (all threads of the CTA must call it: it contains a barrier).
 // LAT: the caller asked for the lattice ints (mplx_succ_out.lattice); without it the 13-entry
 // array never exists (it would cost 13 registers through phase A).
@@ -307,7 +323,9 @@ __device__ __forceinline__ void phase_ab(const EnvParams &P, const mplx_waypoint
     }
     if (ok) {
       // tn == curr  <=>  hash_value(tn) == hash_value(curr)  (waypoint.h:133-135, 93-125)
-      // hash_value(curr): per thread, or once per node by the caller (s_hcurr[node in CTA])
+      // hash_value(curr): per thread, or once per node by the caller (s_hcurr[node in CTA]).  Per thread it is
+      // node_hash folded in here axis by axis beside the key: calling node_hash after the key loop instead
+      // changes the compiled code of the register, dealing and search kernels.
       uint64_t hcurr = s_hcurr ? s_hcurr[nl] : 0;
       int nl_ = 0;
 #pragma unroll

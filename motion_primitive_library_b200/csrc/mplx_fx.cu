@@ -113,7 +113,7 @@ expand_fx_kernel(const __grid_constant__ EnvParams P, const mplx_waypoint *__res
     const int lane = threadIdx.x - kThreads;
     if (lane == 0) S.q_n = 0;
     for (int j = lane; j < npb; j += 32)
-      if (node0 + j < n_nodes) S.hcurr[j] = curr_hash<DIM, ORD>(nodes + node0 + j);
+      if (node0 + j < n_nodes) S.hcurr[j] = node_hash<DIM, ORD, false>(nodes + node0 + j);
     __syncthreads();  // B1
     __syncthreads();  // B2
     __syncthreads();  // B3
